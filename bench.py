@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of Llama-2-7B with the KIVI (K2V2 g32 R128) cache on B200(s).
+"""bench.py -- decode tokens/s of Llama-2-7B with the KIVI (K2V2 g32 R128) cache on H100(s).
 
     python bench.py --gpus N --steps K --warmup W            # this repo (libkivi_b200 fused decode)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU fake-quant path
@@ -19,8 +19,13 @@ One JSON line on stdout (rank 0):
   reference_gpu  the UNMODIFIED reference CUDA extension (oracle/_ref/kivi_gemv.so, when present) at the same layer
                  shape: kernel-only and wrapper-inclusive (its transpose().contiguous() copies, quant/matmul.py:199-218)
   extra_configs  the other BASELINE.json configs, each with its own tokens/s and roofline: cfg 3 (Llama-3-8B GQA bs64
-                 seq8k), cfg 4 (Mistral-7B K4V4 g64 R64 bs16 seq32k) at N = 1; cfg 5 (Llama-2-7B global batch 256 split
-                 256/N per GPU) at every N.  `--no-extra` skips them.
+                 seq8k), cfg 4 (Mistral-7B K4V4 g64 R64 bs16 seq32k) at N = 1; cfg 5 (Llama-2-7B global batch 96 split
+                 96/N per GPU: at 128 the cache, the weights and the prefill buffers exceed one 80 GB H100) at every N.
+                 `--no-extra` skips them.
+
+`--dump-outputs DIR` writes what the last timed step returned (rank 0): DIR/logits.npy ([B, vocab] fp32, a fixed seeded
+sample of rows when larger than 64 MB) and DIR/next_tokens.npy (the greedy ids of every rank, float64).  Weights, cache
+contents and the first token ids are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -192,17 +197,17 @@ def run_reference(args):
 def workload_config(args, batch, gpus, model="llama-2-7b", seq=None, kb=2, vb=2, g=32, R=128):
     seq = seq or args.seq
     return {"workload": f"{MODEL_TITLES.get(model, model)} K{kb}V{vb} g{g} residual{R}, bs{batch} per GPU, decode steps ending "
-                        f"at seq {seq} (cache pre-filled by the prefill pack kernels), 1xB200 per rank",
+                        f"at seq {seq} (cache pre-filled by the prefill pack kernels), 1xH100 per rank",
             "batch_per_gpu": batch, "seq_len": seq, "k_bits": kb, "v_bits": vb, "group_size": g,
             "residual_length": R, "parallelism": f"dp{gpus}",
-            "l2": "per-step working set (weights + KV cache, tens of GB) >> 126 MB L2: inputs larger than L2"}
+            "l2": "per-step working set (weights + KV cache, tens of GB) >> 50 MB L2: inputs larger than L2"}
 
 
 # --------------------------------------------------------------------------------------------------
 # one decode workload on this rank's GPU
 # --------------------------------------------------------------------------------------------------
 def hbm_peak():
-    peak, src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, src = 3350.0, "H100 SXM data-sheet HBM3 bandwidth (not measured; MEASURED_PEAKS.json absent)"
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             peak = float(json.load(f)["hbm_gbs"])
@@ -256,7 +261,20 @@ def attention_roofline(model, cache, step_ms):
     return roof
 
 
-def run_decode(model_name, B, seq, K, W, rank, ws, local, sampler=None, e2e=True, kivi=None, roofline=True):
+def dump_outputs(out_dir, logits, tokens, limit=64 << 20):
+    """The arrays the caller of the timed step receives, as float32 / float64 .npy files (at most `limit` bytes)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    lg = logits.float().cpu().numpy()
+    ids = tokens.cpu().numpy().astype(np.float64)
+    room = max(1, (limit - ids.nbytes) // (lg.shape[1] * 4))
+    if lg.shape[0] > room:                                   # a fixed, seeded sample of the rows
+        lg = lg[np.sort(np.random.default_rng(0).choice(lg.shape[0], room, replace=False))]
+    np.save(os.path.join(out_dir, "logits.npy"), lg)
+    np.save(os.path.join(out_dir, "next_tokens.npy"), ids)
+
+
+def run_decode(model_name, B, seq, K, W, rank, ws, local, sampler=None, e2e=True, kivi=None, roofline=True, dump=None):
     """Build the model, pre-fill the cache so that the K timed steps end at kv length `seq`, time K graph-replayed steps."""
     import torch
     from kivi_b200 import dist as kdist
@@ -331,10 +349,12 @@ def run_decode(model_name, B, seq, K, W, rank, ws, local, sampler=None, e2e=True
     t_host0 = time.perf_counter()
     ev[0].record()
     for i in range(K):
-        model.decode_step()
+        logits = model.decode_step()
         ev[i + 1].record()
     torch.cuda.synchronize()
     t_host1 = time.perf_counter()
+    if dump and rank == 0:
+        dump_outputs(dump, logits, model.all_tokens)
     kdist.barrier()
     ms = kdist.max_over_ranks(ev[0].elapsed_time(ev[K]))
     per_step = [ev[i].elapsed_time(ev[i + 1]) for i in range(K)]
@@ -493,19 +513,12 @@ def run_ours(args):
         sampler.start()
     B = args.batch if args.global_batch is None else args.global_batch // ws
     kivi = dict(k_bits=args.k_bits, v_bits=args.v_bits, group_size=args.group_size, residual_length=args.residual_length)
-    main = run_decode(args.model, B, args.seq, K, W, rank, ws, local, sampler=sampler, kivi=kivi)
+    main = run_decode(args.model, B, args.seq, K, W, rank, ws, local, sampler=sampler, kivi=kivi, dump=args.dump_outputs)
     if main is None:
         return 0
     model = main.pop("model")
     mcfg = model.config
     roof = main.get("roofline")
-    if roof is not None:
-        try:   # DRAM bytes of the call from the committed ncu --set full capture of the same shape (NOT measured in this run)
-            with open(os.path.join(ROOT, "profiles", "r02_attention_ncu.json")) as f:
-                roof["traffic"] = json.load(f).get("dram_bytes_per_launch")
-                roof["traffic_source"] = "profiles/r02_attention_ncu.json (ncu --set full capture of this shape; not measured in this run)"
-        except Exception:
-            roof["traffic_source"] = "no ncu capture committed for this build"
     shape = (B, mcfg.num_attention_heads, mcfg.num_key_value_heads)
     del model
     gc.collect()
@@ -537,8 +550,8 @@ def run_ours(args):
         if ws == 1:
             plan += [("cfg3", "llama-3-8b", 64, 8192, dict(k_bits=2, v_bits=2, group_size=32, residual_length=128)),
                      ("cfg4", "mistral-7b", 16, 32768, dict(k_bits=4, v_bits=4, group_size=64, residual_length=64))]
-        if 256 % ws == 0:
-            plan += [("cfg5", "llama-2-7b", 256 // ws, 4096, dict(k_bits=2, v_bits=2, group_size=32, residual_length=128))]
+        if 96 % ws == 0:
+            plan += [("cfg5", "llama-2-7b", 96 // ws, 4096, dict(k_bits=2, v_bits=2, group_size=32, residual_length=128))]
         for key, mname, bx, sx, kv in plan:
             try:
                 r = run_decode(mname, bx, sx, Kx, Wx, rank, ws, local, sampler=None, e2e=False, kivi=kv)
@@ -546,7 +559,7 @@ def run_ours(args):
                 r.pop("clocks", None)
                 r.update({"metric": f"decode tokens/sec @ {MODEL_TITLES[mname]} bs{bx * ws} seq{sx} K{kv['k_bits']}V{kv['v_bits']}",
                           "unit": UNIT, "steps": Kx, "warmup": Wx, "n_gpus": ws,
-                          "scaling": "strong (global batch 256 split over the GPUs)" if key == "cfg5" else "n/a (1 GPU)",
+                          "scaling": "strong (global batch 96 split over the GPUs)" if key == "cfg5" else "n/a (1 GPU)",
                           "config": workload_config(args, bx, ws, mname, sx, kv["k_bits"], kv["v_bits"], kv["group_size"],
                                                     kv["residual_length"])})
                 if key == "cfg4":
@@ -608,6 +621,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-reference-gpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra BASELINE configs (cfg 3 / 4 / 5)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the logits and sampled ids of the last timed step as .npy files into DIR")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

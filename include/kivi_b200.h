@@ -1,5 +1,5 @@
 /*
- * kivi_b200.h -- C ABI of libkivi_b200.so, the B200-native (sm_100a) implementation of the
+ * kivi_b200.h -- C ABI of libkivi_b200.so, the H100-native (sm_90a) implementation of the
  * KIVI decode hot path: 2/4-bit asymmetric pack of new K/V tokens and the batched dequant-GEMVs
  * q.K^T and softmax.V over the packed cache (+ fp16 residual window).
  *

@@ -1,4 +1,4 @@
-"""kivi_b200 -- B200-native (sm_100a) implementation of KIVI's decode hot path.
+"""kivi_b200 -- H100-native (sm_90a) implementation of KIVI's decode hot path.
 
 Host side mirrors the reference's Python surface (quant/new_pack.py, quant/matmul.py, quant/gemv.py,
 the `kivi_gemv` extension module, the attention hook of models/llama_kivi.py); all compute runs in

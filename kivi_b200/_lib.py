@@ -41,7 +41,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(SO_PATH):
             raise RuntimeError(
                 f"kivi_b200: CUDA library {SO_PATH} is missing. Build it with `python -m kivi_b200.build` "
-                "(nvcc, sm_100a). There is no CPU or PyTorch fallback for this package.")
+                "(nvcc, sm_90a). There is no CPU or PyTorch fallback for this package.")
         L = ctypes.CDLL(SO_PATH)
         for name, (res, args) in _SIGNATURES.items():
             if hasattr(L, name):

@@ -1,4 +1,4 @@
-// kivi_bgemv.cu -- batched "outer-dim" dequant-GEMV on caller-supplied (reference) layouts, sm_100a.
+// kivi_bgemv.cu -- batched "outer-dim" dequant-GEMV on caller-supplied (reference) layouts, sm_90a.
 //
 //   C[u_q, n] = sum_k A[u_q, k] * (scale[u_kv, k, n/g] * code[u_kv, k, n] + zero[u_kv, k, n/g])
 //

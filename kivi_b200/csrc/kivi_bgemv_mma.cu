@@ -1,4 +1,4 @@
-// kivi_bgemv_mma.cu -- the "outer-dim" dequant-GEMV on the REFERENCE layouts with the tensor cores as unpack amortiser (sm_100a).
+// kivi_bgemv_mma.cu -- the "outer-dim" dequant-GEMV on the REFERENCE layouts with the tensor cores as unpack amortiser (sm_90a).
 //
 //   C[u_q, n] = sum_k A[u_q, k] * (scale[u_kv, k, n/g] * code[u_kv, k, n] + zero[u_kv, k, n/g])        (quant/matmul.py:178-219)
 //
@@ -22,7 +22,7 @@
 // Data movement: every warp owns two private shared-memory stages and streams its own 128-outer x 128-inner (wide) /
 // 128-inner x 128-outer (tall) tiles with cp.async (16-byte code units, 8/4-byte scale units; zero-fill past the ends), no CTA
 // barrier in the loops.  tall: the CTAs of a thread-block CLUSTER split the tokens of a unit and reduce their fp32 partials
-// through distributed shared memory, so few-long-unit shapes (B16 x 8 KV heads x 32k tokens) still fill the 148 SMs.
+// through distributed shared memory, so few-long-unit shapes (B16 x 8 KV heads x 32k tokens) still fill the 132 SMs.
 #include <cooperative_groups.h>
 
 #include "kivi_decode.cuh"
@@ -588,9 +588,9 @@ int bgemv_ref_mma(const __half* A, long long a_stride, const uint32_t* qB, long 
     }
     if (wide) {
         if (N % 64 != 0) return KIVI_ERR_UNSUPPORTED;                       // 16-byte code units must not straddle a row end mid-word pair
-        // Measured (tools/microbench.py, profiles/r02_microbench*.json): on THIS layout the merge (PRMT) and the scattered
-        // scale loads eat most of what the MMA saves; with one query head per KV head the SIMT kernel (one LOP3 + one FFMA per
-        // code on two different pipes) is 25 % faster, with shared KV heads (one FFMA per code AND head) the MMA kernel wins.
+        // On THIS layout the merge (PRMT) and the scattered scale loads eat most of what the MMA saves: with one query head
+        // per KV head the SIMT kernel (one LOP3 + one FFMA per code on two different pipes) is used, with shared KV heads (one
+        // FFMA per code AND head) the MMA kernel (tools/microbench.py compares them).
         if (ratio < 2 || ratio / G > 2) return KIVI_ERR_UNSUPPORTED;
         KIVI_MMA_DISPATCH(launch_wide)
     }

@@ -1,5 +1,5 @@
 // kivi_cache.cu -- pre-allocated, blocked KIVI cache: sizing, prefill pack, state advance, export to
-// the reference's 9-tuple layout (sm_100a).  Layout: kivi_decode.cuh.
+// the reference's 9-tuple layout (sm_90a).  Layout: kivi_decode.cuh.
 //
 // Replaces the cache handling of LlamaFlashAttention_KIVI.forward (models/llama_kivi.py):
 //   prefill split + pack  :425-452   -> kivi_cache_prefill_f16 (fused transpose + quantise + fragment pack of

@@ -1,4 +1,4 @@
-// kivi_common.cuh -- shared device helpers for libkivi_b200 (sm_100a only).
+// kivi_common.cuh -- shared device helpers for libkivi_b200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -9,8 +9,8 @@
 #ifndef __CUDA_ARCH__
 #define KIVI_HOST_ONLY 1
 #endif
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libkivi_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 900)
+#error "libkivi_b200 is written for sm_90a (H100) only"
 #endif
 
 #include <atomic>

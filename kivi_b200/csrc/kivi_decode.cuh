@@ -1,5 +1,5 @@
 // kivi_decode.cuh -- KIVI cache layout in HBM (tensor-core friendly blocks) + mbarrier / bulk-copy (TMA)
-// PTX helpers (sm_100a).
+// PTX helpers (sm_90a).
 //
 // Every packed store is a sequence of 128 x 128 BLOCKS "inner x outer":
 //     K store: inner = channel d (the reduction index of q.K^T), outer = token   -> one block = 128 tokens
@@ -58,8 +58,8 @@ struct Lay {
     static constexpr int kCodeBytes = 8 * kChunkBytes;   // 4096 / 8192
     // Unpack: field j of a 16-bit half is brought to bit offset P(j) in [4, 10) by an optional shift of the whole
     // word, isolated with one AND, and consumed AS IS: the fp16 denormal  code * 2^(P - 24).  mma.sync handles
-    // denormal inputs exactly when their set bits sit at offset >= 4 (measured: tools/probes/mma_unpack_variants.cu,
-    // error identical to normal inputs; fields at offsets 0..3 lose up to 4 bits), so no magic-number subtraction
+    // denormal inputs exactly when their set bits sit at offset >= 4 (tools/probes/mma_unpack_variants.cu probes it; fields
+    // at lower offsets can lose bits, and the GPU tests hold every kernel to the oracle), so no magic-number subtraction
     // is needed: ONE LOP3 per pair of codes.
     //   2-bit: fields 0,1 <- (w << 4);  fields 2,3,4 in place;  fields 5,6,7 <- (w >> 6)
     //   4-bit: field 0 <- (w << 4);  field 1 in place;  field 2 <- (w >> 4);  field 3 <- (w >> 8)

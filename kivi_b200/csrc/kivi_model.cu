@@ -1,4 +1,4 @@
-// kivi_model.cu -- small fused glue kernels of the decode step around the hot path (sm_100a):
+// kivi_model.cu -- small fused glue kernels of the decode step around the hot path (sm_90a):
 // residual-add + RMSNorm, RoPE + q/k/v split, SiLU*mul.  They replace ~16 ATen elementwise launches per
 // layer per step with 4; arithmetic follows the HF Llama modules the reference forks
 // (models/llama_kivi.py star-imports transformers.models.llama): every fp16 op rounds to fp16.

@@ -1,4 +1,4 @@
-// kivi_pack.cu -- fused asymmetric min/max quantise + bit-pack along the last dim (sm_100a).
+// kivi_pack.cu -- fused asymmetric min/max quantise + bit-pack along the last dim (sm_90a).
 //
 // Replaces triton_quantize_and_pack_along_last_dim (quant/new_pack.py:217-252): Triton min/max
 // kernel (:158-177) + 6 ATen elementwise kernels (:238-242, incl. an int32 temp 16x the packed

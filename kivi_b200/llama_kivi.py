@@ -631,8 +631,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def _ensure_fast(self):
         """Fused q|k|v, o and gate|up weights in [in, out] layout + static activation buffers for the 9-launch-per-layer
-        step.  At M = B rows cuBLAS streams the weights 9-13 % faster from this layout (tools/gemm_probe.py: q|k|v 27.6 vs
-        31.8 us, o 15.4 vs 17.4 us, gate|up 42.0 vs 46.1 us; down is layout-neutral).  The fused buffers OWN the storage:
+        step.  At M = B rows cuBLAS streams the weights faster from this layout (tools/gemm_probe.py compares the two
+        layouts; down is layout-neutral).  The fused buffers OWN the storage:
         the nn.Linear parameters become transposed views of them, so there is one copy of every weight (the reference's
         mem_spd_test reports peak memory) and load_state_dict / in-place edits reach the decode path."""
         if self._fast is not None and self._fast.B == self.cache.batch:

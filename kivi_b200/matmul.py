@@ -1,4 +1,4 @@
-"""Drop-in surface of the reference's quant/matmul.py, backed by libkivi_b200 (sm_100a CUDA)."""
+"""Drop-in surface of the reference's quant/matmul.py, backed by libkivi_b200 (sm_90a CUDA)."""
 from __future__ import annotations
 
 import torch

@@ -1,4 +1,4 @@
-"""Drop-in surface of the reference's quant/new_pack.py, backed by libkivi_b200 (sm_100a CUDA).
+"""Drop-in surface of the reference's quant/new_pack.py, backed by libkivi_b200 (sm_90a CUDA).
 
 Same names, argument order, return shapes/dtypes and assert behaviour as the reference
 (jy-yuan/KIVI quant/new_pack.py).  All functions require CUDA tensors.

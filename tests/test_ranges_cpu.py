@@ -57,8 +57,7 @@ def test_ranges_partition_the_items(split, n_units, n_b, n_w, w_cap, kernel):
 
 
 def test_default_split_is_equal_item_counts(split):
-    """The shipped build weighs every item the same (KIVI_UNIFORM_RANGES = 1; the fitted cost model lost the A/B,
-    profiles/r02_range_costs.txt): range sizes differ by at most one item."""
+    """The shipped build weighs every item the same (KIVI_UNIFORM_RANGES = 1): range sizes differ by at most one item."""
     for kernel in (0, 1):
         W, lo, owner = split(1024, 31, 9, 2368, kernel)
         counts = np.bincount(owner, minlength=W)

@@ -23,7 +23,7 @@ for name, flags in zip(args[0::2], args[1::2]):
         objs.append(obj)
     assert all(p.wait() == 0 for p in procs), name
     so = os.path.join(out_dir, f"libkivi_{name}.so")
-    subprocess.check_call([kb._nvcc(), "-shared", "-o", so] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-lcudart"])
+    subprocess.check_call([kb._nvcc(), "-shared", "-o", so] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-lcudart"])
     for o in objs:
         os.remove(o)
     print(so)

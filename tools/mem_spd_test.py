@@ -12,7 +12,7 @@ generation is this package's greedy `generate()` (pre-allocated KiviCache, CUDA-
 
 `--fp16-baseline` runs the OTHER arm of the reference's script (`mem_spd_test.py:33-42`: K_BITS = 16 -> stock Hugging Face
 `LlamaForCausalLM`, fp16 KV cache, HF `generate`) on the same random-init architecture, so that the README's peak-memory and
-throughput ratios (`README.md:29`) have a B200 counterpart.  Results of the round: profiles/r02_mem_spd.json."""
+throughput ratios (`README.md:29`) have a counterpart on this implementation."""
 import argparse
 import json
 import os

@@ -3,7 +3,7 @@
 //   denorm : A = (w & mask_j)  (fp16 denormal)              = c * 4^j * 2^-24         (LOP3 per pair)
 //   offset : A = (w & mask_j) | 0x6400                      = 1024 + c * 4^j          (LOP3 per pair; minus 1024*sum(B))
 // B = hi/lo split of x*s (x, s random fp16), K = 128 (8 accumulating MMAs), compared with fp64.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mma_unpack_variants mma_unpack_variants.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mma_unpack_variants mma_unpack_variants.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>

@@ -1,7 +1,6 @@
-// Pipe-rate microbenchmark for the decode-attention design space (sm_100a): legacy mma.sync fp16 vs u8 vs e4m3,
+// Pipe-rate microbenchmark for the decode-attention design space (sm_90a): legacy mma.sync fp16 vs u8 vs e4m3,
 // fp8 conversions, LOP3 / PRMT.  One CTA per SM, W warps per CTA; cycles per warp instruction per sub-partition.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/ubench/pipes tools/ubench/pipes.cu && tools/ubench/pipes
-// Results on B200: profiles/r02_pipe_rates.txt (mma.sync with e4m3 operands is lowered by ptxas to F2FP unpacks + HMMA).
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/ubench/pipes tools/ubench/pipes.cu && tools/ubench/pipes
 #include <cstdio>
 #include <cstdint>
 #include <cuda_fp16.h>
@@ -32,7 +31,7 @@ __global__ void k(uint32_t *out, long long *cyc, uint32_t seed) {
                 asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                              : "+r"(ci[i][0]), "+r"(ci[i][1]), "+r"(ci[i][2]), "+r"(ci[i][3])
                              : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-            } else if (OP == 11) {     // e4m3 mma.sync: ptxas lowers it to F2FP unpacks + HMMA on sm_100a (no QMMA)
+            } else if (OP == 11) {     // e4m3 mma.sync
                 asm volatile("mma.sync.aligned.m16n8k32.row.col.f32.e4m3.e4m3.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                              : "+f"(c[i][0]), "+f"(c[i][1]), "+f"(c[i][2]), "+f"(c[i][3])
                              : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
