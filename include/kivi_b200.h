@@ -125,7 +125,8 @@ int kivi_unpack_dequant_lastdim_f16(const void* code, const void* scale, const v
  * int32[8] shared by all layers of a model {tk, r, tv, L, vhead, kv_len, -, -}: tk = tokens in the
  * packed K store, r = tokens in the fp16 K window, tv = tokens in the packed V store, L = tokens in
  * the fp16 V window (ring buffer starting at vhead).  All sequences of the batch have the same
- * length, as in the reference (one kv_seq_len per cache, :309, :455).
+ * length, as in the reference (one kv_seq_len per cache, :309, :455); a left-padded batch keeps
+ * that length and names each sequence's first real token (kivi_decode_attention_ragged_f16).
  * head_dim is 128 (every model the reference ships); group_size in {32,64,128};
  * residual_length % group_size == 0 (:344), residual_length in {32, 64, 128, 256}.
  * ========================================================================================== */
@@ -205,10 +206,32 @@ int kivi_decode_attention_f16(const kivi_cache_t* cache, const void* q, const vo
                               const void* mask, void* out, void* workspace, int64_t workspace_bytes,
                               void* dbg_logits, void* dbg_probs, int64_t dbg_stride, int max_kv_len, void* stream);
 
+/* The same step for a LEFT-PADDED batch: sequence b's tokens before position kv_start[b] are padding.
+ *   kv_start: NULL (= all zeros: this is then kivi_decode_attention_f16) or a device int32[B]; with
+ *   s_b = clamp(kv_start[b], 0, kv_len), the positions p < s_b of sequence b are excluded -- the same result as an
+ *   additive finfo(fp16).min at those positions of `mask` -- and the new token is always visible.  `mask` keeps its
+ *   meaning and may be combined with kv_start.  The offsets are read on the device: the call is CUDA-graph capturable
+ *   and the caller may rewrite them between replays (not from the kernel enqueued directly before the call when
+ *   cache->flags has KIVI_CACHE_OVERLAP_PROLOGUE).
+ * A packed 128-token block (K or V) that lies wholly in the padding is neither read nor contracted; a partly padded block
+ * and the fp16 window items are masked in their epilogues, so the HBM bytes read follow the visible tokens.  The cache
+ * update is that of kivi_decode_attention_f16 (pad tokens stay in the K / V stores and their quantisation groups). */
+int kivi_decode_attention_ragged_f16(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,
+                                     const int32_t* kv_start, const void* mask, void* out, void* workspace,
+                                     int64_t workspace_bytes, void* dbg_logits, void* dbg_probs, int64_t dbg_stride,
+                                     int max_kv_len, void* stream);
+
 /* Test hook: the (unit, item) work split of the two decode kernels evaluated on the host (kernel 0 = q.K^T, 1 = p.V cost
  * model); a unit has n_b packed blocks, n_w window items and the new token.  out_lo: 2 * (W + 1) ints, (unit, item) of the first
  * position of every range and of the end; out_owner: NULL or one int per position.  Returns the number of ranges W. */
 int kivi_debug_range_split(int n_units, int n_b, int n_w, int w_cap, int kernel, int* out_lo, int* out_owner);
+
+/* Test hook: the stage sequence of every warp of a ragged call (kernel 0 = q.K^T, 1 = p.V; unit_start[u] = the kv_start of
+ * work unit u's sequence, clamped to kv_len), evaluated on the host with the kernels' own skip predicate and cursor walk.
+ * issued / consumed: cap entries of 4 ints (warp, unit, item, half) each -- the copies the producer issues and the stages
+ * the item loop waits on; n_out[0] / n_out[1] receive their counts.  Returns the number of ranges W or a KIVI_ERR_*. */
+int kivi_debug_ragged_items(int n_units, int n_b, int n_w, int w_cap, int kernel, const int* unit_start, int kv_len,
+                            int* issued, int* consumed, int64_t cap, int64_t* n_out);
 
 /* Advance `state` by one token (the bookkeeping of :343-356, :386-399); once per step, all layers. */
 int kivi_cache_advance(const kivi_cache_t* cache, void* stream);

@@ -4,6 +4,8 @@ Host-side mirror of the cache policy of LlamaFlashAttention_KIVI.forward (models
 the reference keeps a per-layer 9-tuple that it regrows with torch.cat every step; here the buffers are
 allocated once (sizes from the C ABI), the lengths live in a device int32[8] shared by all layers, and
 one CUDA launch per layer does attention + cache update.  `export(layer)` returns the reference's 9-tuple.
+A left-padded batch keeps one length for all sequences; `set_kv_start` names each sequence's first real token, and the
+attention then skips the padding on the device (kivi_decode_attention_ragged_f16).
 """
 from __future__ import annotations
 
@@ -25,6 +27,24 @@ class _CacheStruct(ctypes.Structure):
 _BOUND = False
 
 
+def kv_start_from_mask(attention_mask) -> torch.Tensor:
+    """HF padding mask [B, n] (1 = real token) of a LEFT-padded batch -> int32 [B] number of pad tokens in front of each
+    sequence (the first visible position), on the mask's device.  Raises ValueError for right padding, holes in the
+    middle of a sequence, or a sequence without any real token."""
+    m = torch.as_tensor(attention_mask)
+    if m.dim() != 2:
+        raise ValueError(f"attention_mask must be 2-D [batch, tokens], got shape {tuple(m.shape)}")
+    keep = m != 0
+    pad = (~keep).sum(1)
+    left = torch.arange(m.shape[1], device=m.device)[None, :] >= pad[:, None]
+    if not torch.equal(keep, left):
+        raise ValueError("attention_mask: left padding is required (zeros only before each sequence's first real token); "
+                         "right padding and holes in the middle are not supported")
+    if bool((pad == m.shape[1]).any()):
+        raise ValueError("attention_mask: every sequence needs at least one real token")
+    return pad.to(torch.int32)
+
+
 def _bind():
     global _BOUND
     if _BOUND:
@@ -35,6 +55,7 @@ def _bind():
     _lib.bind("kivi_cache_prefill_f16", i32, [P, vp, vp, i32, vp])
     _lib.bind("kivi_decode_workspace_bytes", i64, [P, i32])
     _lib.bind("kivi_decode_attention_f16", i32, [P, vp, vp, vp, vp, vp, vp, i64, vp, vp, i64, i32, vp])
+    _lib.bind("kivi_decode_attention_ragged_f16", i32, [P, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, i64, i32, vp])
     _lib.bind("kivi_cache_advance", i32, [P, vp])
     _lib.bind("kivi_cache_export_f16", i32, [P, i32, i32, i32, i32, i32] + [vp] * 9)
     _lib.bind("kivi_cache_import_f16", i32, [P, i32, i32, i32, i32] + [vp] * 9)
@@ -82,6 +103,10 @@ class KiviCache:
         if nws < 0:
             _lib.check(nws, "kivi_decode_workspace_bytes")
         self._ws = torch.zeros(nws, dtype=torch.uint8, device=self.device)
+        # left padding: first visible position of every sequence (device-resident, so a captured step reads the current
+        # values); used only while `ragged` is set, otherwise the unpadded entry runs
+        self.kv_start = torch.zeros(batch, dtype=torch.int32, device=self.device)
+        self.ragged = False
         # host mirror of `state` (its evolution is deterministic)
         self.tk = self.r = self.tv = self.L = self.vhead = self.kv_len = 0
 
@@ -108,9 +133,23 @@ class KiviCache:
             self.L = R
         self.kv_len += 1
 
+    def set_kv_start(self, kv_start):
+        """Mark the batch as left-padded: kv_start [B] = each sequence's first visible position (its number of pad tokens);
+        positions before it are excluded from attention.  None = no padding.  The values are copied into the cache's own
+        device buffer, so they may change between replays of a captured step."""
+        if kv_start is None:
+            self.ragged = False                                      # the buffer is not read while the flag is clear
+            return
+        t = torch.as_tensor(kv_start).reshape(-1)
+        if t.numel() != self.batch:
+            raise ValueError(f"kv_start needs {self.batch} entries, got {t.numel()}")
+        self.kv_start.copy_(t.to(torch.int32))
+        self.ragged = True
+
     # ------------------------------------------------------------------ operations
-    def prefill(self, layer: int, k: torch.Tensor, v: torch.Tensor):
-        """k, v [B, Hkv, n, 128] fp16 (K post-RoPE): models/llama_kivi.py:425-452 in three launches."""
+    def prefill(self, layer: int, k: torch.Tensor, v: torch.Tensor, kv_start=None):
+        """k, v [B, Hkv, n, 128] fp16 (K post-RoPE): models/llama_kivi.py:425-452 in three launches.  kv_start: see
+        set_kv_start (None: the batch is not padded)."""
         _lib.require_cuda(k, v)
         B, Hkv, n, D = k.shape
         assert (B, Hkv, D) == (self.batch, self.num_kv_heads, self.head_dim) and v.shape == k.shape
@@ -122,6 +161,7 @@ class KiviCache:
             _lib.check(_lib.lib().kivi_cache_prefill_f16(ctypes.byref(self._structs[layer]), k.data_ptr(), v.data_ptr(),
                                                          n, _lib.stream_ptr(self.device)), "kivi_cache_prefill_f16")
         self._mirror_prefill(n)
+        self.set_kv_start(kv_start)
 
     def decode_attention(self, layer: int, q: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
                          mask: torch.Tensor | None = None, out: torch.Tensor | None = None,
@@ -146,14 +186,18 @@ class KiviCache:
             if d is not None:
                 assert d.dtype == torch.float16 and d.is_contiguous() and d.shape[:2] == (self.batch, self.num_heads)
                 stride = d.shape[-1]
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().kivi_decode_attention_f16(
-                ctypes.byref(self._structs[layer]), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
-                mask.data_ptr() if mask is not None else None, out.data_ptr(),
-                self._ws.data_ptr(), self._ws.numel(),
+        args = (mask.data_ptr() if mask is not None else None, out.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
                 dbg_logits.data_ptr() if dbg_logits is not None else None,
-                dbg_probs.data_ptr() if dbg_probs is not None else None, stride, self.max_tokens,
-                _lib.stream_ptr(self.device)), "kivi_decode_attention_f16")
+                dbg_probs.data_ptr() if dbg_probs is not None else None, stride, self.max_tokens, _lib.stream_ptr(self.device))
+        with torch.cuda.device(self.device):
+            if self.ragged:                                          # left-padded batch: padded blocks are skipped
+                _lib.check(_lib.lib().kivi_decode_attention_ragged_f16(
+                    ctypes.byref(self._structs[layer]), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                    self.kv_start.data_ptr(), *args), "kivi_decode_attention_ragged_f16")
+            else:
+                _lib.check(_lib.lib().kivi_decode_attention_f16(
+                    ctypes.byref(self._structs[layer]), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(), *args),
+                    "kivi_decode_attention_f16")
         return out
 
     def advance(self):
@@ -175,11 +219,11 @@ class KiviCache:
                                f"lengths {st[:6]} exceed the capacity the cache was created with")
         return st
 
-    def import_tuple(self, layer: int, past):
+    def import_tuple(self, layer: int, past, kv_start=None):
         """Load `layer` from the reference's per-layer 9-tuple (models/llama_kivi.py:454-455), the inverse of
         export(): a cache that was built by the reference's own hook (or by kivi_prefill_tuple /
         kivi_decode_attention_tuple) continues on the fused path.  All layers of a model share one `state`, so every
-        layer must be imported from tuples of the same lengths."""
+        layer must be imported from tuples of the same lengths.  kv_start: see set_kv_start."""
         kc, kfull, ks, km, vc, vfull, vs, vm, seen = past
         B, Hkv, D, g = self.batch, self.num_kv_heads, self.head_dim, self.group_size
         kf, vf = 32 // self.k_bits, 32 // self.v_bits
@@ -210,6 +254,7 @@ class KiviCache:
                 ctypes.byref(self._structs[layer]), tk, r, tv, L, ptr(kc), ptr(ks), ptr(km), ptr(kfull),
                 ptr(vc), ptr(vs), ptr(vm), ptr(vfull), _lib.stream_ptr(self.device)), "kivi_cache_import_f16")
         self.tk, self.r, self.tv, self.L, self.vhead, self.kv_len = tk, r, tv, L, 0, seen
+        self.set_kv_start(kv_start)
 
     def export(self, layer: int):
         """The reference's per-layer 9-tuple (models/llama_kivi.py:454-455):

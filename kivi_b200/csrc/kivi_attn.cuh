@@ -21,6 +21,9 @@
 //   1-D bulk copies (cp.async.bulk = the TMA engine, SASS UBLKCP, L2 evict-first) completing on the stage's
 //   mbarrier; right after consuming a stage its elected lane issues the copy of the item S positions ahead
 //   (fence.proxy.async orders its reads before the async write).
+//   Left-padded batches (RAGGED = true, kivi_decode_attention_ragged_f16): a per-sequence start offset read on the device;
+//   packed blocks wholly in the padding are skipped by producer and consumer alike (ragged_skip), partly padded blocks and
+//   window items are masked in their epilogues.  RAGGED = false is the unpadded kernel, without any of it.
 //
 // Arithmetic of a packed block (128 inner x 128 outer, kivi_decode.cuh):
 //     sum_i x_i * (s_i,G * c_i,o + z_i,G) = sum_i (x_i * s_i,G) * c_i,o  +  sum_i x_i * z_i,G
@@ -188,6 +191,7 @@ struct Workspace {                     // carved from the caller's buffer (kivi_
 struct AttnParams {
     CacheDesc c;
     const __half* q; const __half* k_new; const __half* v_new; const __half* mask;
+    const int32_t* kv_start;            // NULL, or [B] first visible position of every sequence (left padding)
     __half* out; __half* dbg_logits; __half* dbg_probs;
     long long dbg_stride;
     Workspace w;
@@ -745,7 +749,42 @@ struct Ranges {
 
 struct Cursor {                         // (unit, pseudo-block, half) position of a warp in its range
     int unit, j, half, left;            // left = pseudo-blocks remaining in the range (including j)
+    int s_unit, s_pos;                  // ragged kernels: the unit whose start s_pos is held (-1: none yet)
 };
+
+// the producer's step after issuing the copy of (unit, j, half): the next stage-item of the range
+__host__ __device__ __forceinline__ void cursor_step(Cursor& cur, int per_unit, int n_b) {
+    if (cur.j < n_b && cur.half + 1 < kParts) { ++cur.half; return; }
+    cur.half = 0;
+    --cur.left;
+    if (++cur.j == per_unit) { cur.j = 0; ++cur.unit; }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Left-padded batches (kivi_decode_attention_ragged_f16).  Sequence b sees the positions p >= s_b = clamp(kv_start[b], 0,
+// kv_len) and the new token.  A packed block (K or V, 128 tokens) that lies wholly below s_b is neither copied nor contracted;
+// a partly padded block and every window item are masked in their epilogues (q.K^T: no statistics, p.V: probability 0).
+// The skip decision is ONE predicate that the producer (*_issue_next, through ragged_seek) and the consumer (the item loops)
+// both evaluate, so a warp waits on exactly the stages it has issued, in the same order (kivi_debug_ragged_items replays
+// both walks on the host).  The unpadded entry runs the RAGGED = false instantiations: none of this is in them.
+// ------------------------------------------------------------------------------------------------
+__host__ __device__ __forceinline__ int clamp_start(int start, int kv_len) {
+    return start < 0 ? 0 : (start > kv_len ? kv_len : start);
+}
+__host__ __device__ __forceinline__ bool ragged_skip(int j, int n_b, int start) {
+    return j < n_b && (j + 1) * kBlockTokens <= start;
+}
+// producer: move the cursor past the items that need no copy -- the new token and the wholly padded packed blocks.  False
+// when the range is exhausted.  start_of(unit) = the unit's clamped start.
+template <class SF>
+__host__ __device__ __forceinline__ bool ragged_seek(Cursor& cur, int per_unit, int n_b, SF&& start_of) {
+    while (cur.left > 0) {
+        if (cur.j == per_unit - 1) { cur.j = 0; ++cur.unit; --cur.left; }
+        else if (cur.half == 0 && ragged_skip(cur.j, n_b, start_of(cur.unit))) { ++cur.j; --cur.left; }
+        else return true;
+    }
+    return false;
+}
 
 // exp(x - m) with the subtraction folded into the multiply: ex2.approx(fma(x, log2 e, nml)), nml = -m * log2 e (one FFMA + MUFU)
 #ifndef KIVI_EXP_FMA
@@ -782,15 +821,30 @@ __device__ __forceinline__ void fold_stats(float& m, float& s, const float (&x)[
 // ------------------------------------------------------------------------------------------------
 // q . K^T  (+ scale, mask, per-range softmax statistics)
 // ------------------------------------------------------------------------------------------------
-template <int KB, int GS>
+// the clamped start of work unit `unit` (its sequence's first visible position)
+__device__ __forceinline__ int unit_start(const AttnParams& p, const Sched& s, int unit) {
+    const int u = p.hchunks == 1 ? unit : unit / p.hchunks;
+    return clamp_start(__ldg(p.kv_start + u / p.c.Hkv), s.T - 1);
+}
+// the same, held in the cursor: the producer asks once per unit
+__device__ __forceinline__ int cursor_start(Cursor& cur, const AttnParams& p, const Sched& s, int unit) {
+    if (unit != cur.s_unit) { cur.s_unit = unit; cur.s_pos = unit_start(p, s, unit); }
+    return cur.s_pos;
+}
+
+template <int KB, int GS, bool RAGGED>
 __device__ __forceinline__ void qk_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s,
                                               int lane, uint64_t pol)
 {
     const CacheDesc& c = p.c;
-    if (cur.left > 0 && cur.j == s.ipu - 1) {                     // the new token needs no load
-        cur.j = 0; ++cur.unit; --cur.left;
+    if constexpr (RAGGED) {
+        if (!ragged_seek(cur, s.ipu, s.n_kb, [&](int un) { return cursor_start(cur, p, s, un); })) return;
+    } else {
+        if (cur.left > 0 && cur.j == s.ipu - 1) {                 // the new token needs no load
+            cur.j = 0; ++cur.unit; --cur.left;
+        }
+        if (cur.left <= 0) return;
     }
-    if (cur.left <= 0) return;
     if (lane == 0) {
         const int u = p.hchunks == 1 ? cur.unit : cur.unit / p.hchunks;
         uint8_t* dst = pp.prod();
@@ -814,13 +868,10 @@ __device__ __forceinline__ void qk_issue_next(Pipe& pp, Cursor& cur, const AttnP
         }
     }
     pp.push();
-    if (cur.j < s.n_kb && cur.half + 1 < kParts) { ++cur.half; return; }
-    cur.half = 0;
-    --cur.left;
-    if (++cur.j == s.ipu) { cur.j = 0; ++cur.unit; }
+    cursor_step(cur, s.ipu, s.n_kb);
 }
 
-template <int KB, int G, int GS, int CW>
+template <int KB, int G, int GS, int CW, bool RAGGED>
 __global__ void __launch_bounds__(CW * 32, KIVI_MINB)
 qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
 {
@@ -856,11 +907,11 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     Pipe pp;
     pp.init(smem + (size_t)warp * p.spw * p.stage_bytes, full_all + warp * p.spw, p.spw, p.stage_bytes);
     Cursor cur;
-    cur.unit = u_lo; cur.j = j_lo; cur.half = 0; cur.left = n_mine;
+    cur.unit = u_lo; cur.j = j_lo; cur.half = 0; cur.left = n_mine; cur.s_unit = -1; cur.s_pos = 0;
     // ONE stage goes out before the grid-dependency wait (the packed cache does not depend on the predecessor); the others
     // follow the q fetch below: issued after all of a warp's first stages, the few q words would queue behind the first-stage
     // copies every warp of the grid requests at this moment and arrive last.
-    for (int i = 0; i < (Lat<G>::q_first ? 1 : p.spw); ++i) qk_issue_next<KB, GS>(pp, cur, p, s, lane, pol);
+    for (int i = 0; i < (Lat<G>::q_first ? 1 : p.spw); ++i) qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
 
     constexpr int NG = Cols<G, GS>::NG;
     const int ratio = c.H / c.Hkv;
@@ -883,7 +934,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     pdl_wait();                                                              // q / k_new come from the previous kernel of the stream
     fetch_q(unit);
     if (Lat<G>::q_first)
-        for (int i = 1; i < p.spw; ++i) qk_issue_next<KB, GS>(pp, cur, p, s, lane, pol);
+        for (int i = 1; i < p.spw; ++i) qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
     KIVI_TL(0, gw, 1);
     #pragma unroll 1
     while (left > 0) {
@@ -892,6 +943,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
         const int uq0 = u * ratio + hc * G;
         const int j_first = j;
         const int n_here = min(left, s.ipu - j);                             // this warp's pseudo-blocks of this unit
+        const int start = RAGGED ? unit_start(p, s, unit) : 0;              // positions below it are padding
 
         // ---- this warp's copy of q: half2 pairs in B-fragment order, fp32 in channel order
         __syncwarp();
@@ -911,6 +963,9 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
 
         #pragma unroll 1
         for (int k = 0; k < n_here; ++k, ++j) {
+            if constexpr (RAGGED) {
+                if (ragged_skip(j, s.n_kb, start)) continue;                 // wholly padded: never copied (qk_issue_next)
+            }
             if (j < s.n_kb) {                                                // ---- packed K block (tensor cores)
                 float acc[8][4];
                 float zc[4];
@@ -931,20 +986,21 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     }, acc, zc, lane);
                     __syncwarp();
                     pp.pop();
-                    qk_issue_next<KB, GS>(pp, cur, p, s, lane, pol);
+                    qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
                 const int64_t rowi = uq0 + h_l;
                 __half* row = p.w.lg + rowi * p.w.ld + j * kBlockTokens;
                 const int nvalid = s.tk - j * kBlockTokens;                  // < 128 only in the last block when R < 128
+                const bool padded = RAGGED && j * kBlockTokens < start;      // partly padded: the masking epilogue
                 // the lane's logits by compile-time slot; slots of MMAs this lane does not own and tokens past the packed
                 // length stay -inf.  ONE arithmetic for the production and the instrumented / masked / partial-block
                 // epilogues (same fold order, hence bit-identical statistics): they differ only in predicated side work.
                 float x[Slots<G, GS>::k];
                 #pragma unroll
                 for (int e = 0; e < Slots<G, GS>::k; ++e) x[e] = -INFINITY;
-                if (!slow && nvalid >= kBlockTokens) {
+                if (!slow && !padded && nvalid >= kBlockTokens) {
                     finalize<KB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int o, float v) {
                         const __half hv = scale_logit(v);
                         row[o] = hv;
@@ -957,7 +1013,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + j * kBlockTokens + o);
                             row[o] = hv;
                             if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + j * kBlockTokens + o] = hv;
-                            x[slot] = __half2float(hv);
+                            if (!padded || j * kBlockTokens + o >= start) x[slot] = __half2float(hv);   // padding: no value
                         }
                     });
                 }
@@ -982,7 +1038,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 __syncwarp();
                 pp.pop();
-                qk_issue_next<KB, GS>(pp, cur, p, s, lane, pol);
+                qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
                 // lane (g8 < G, t): head g8, tokens 2t, 2t+1 (tile 0) and 8+2t, 9+2t (tile 1)
                 if (g8 < G) {
                     const int64_t rowi = uq0 + g8;
@@ -996,7 +1052,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + s.tk + t0 + t);
                             p.w.lg[rowi * p.w.ld + s.tk + t0 + t] = hv;
                             if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + s.tk + t0 + t] = hv;
-                            x[e] = __half2float(hv);
+                            if (!RAGGED || s.tk + t0 + t >= start) x[e] = __half2float(hv);   // padding: no value
                         }
                     }
                     fold_stats(m_win, s_win, x);
@@ -1118,15 +1174,19 @@ __device__ __forceinline__ void wait_unit_ready(const AttnParams& p, const Sched
 #endif
 }
 
-template <int VB, int G, int GS>
+template <int VB, int G, int GS, bool RAGGED>
 __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s,
                                               int ratio, int lane, uint64_t pol, const Ranges<CostQK>& rq, int& ready_unit)
 {
     const CacheDesc& c = p.c;
-    if (cur.left > 0 && cur.j == s.bpu - 1) {                     // the new token needs no load
-        cur.j = 0; ++cur.unit; --cur.left;
+    if constexpr (RAGGED) {
+        if (!ragged_seek(cur, s.bpu, s.n_vb, [&](int un) { return cursor_start(cur, p, s, un); })) return;
+    } else {
+        if (cur.left > 0 && cur.j == s.bpu - 1) {                 // the new token needs no load
+            cur.j = 0; ++cur.unit; --cur.left;
+        }
+        if (cur.left <= 0) return;
     }
-    if (cur.left <= 0) return;
     if (cur.unit != ready_unit) { wait_unit_ready(p, s, rq, cur.unit, lane); ready_unit = cur.unit; }
     if (lane == 0) {
         const int u = p.hchunks == 1 ? cur.unit : cur.unit / p.hchunks, hc = p.hchunks == 1 ? 0 : cur.unit % p.hchunks;
@@ -1172,10 +1232,7 @@ __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnP
         }
     }
     pp.push();
-    if (cur.j < s.n_vb && cur.half + 1 < kParts) { ++cur.half; return; }
-    cur.half = 0;
-    --cur.left;
-    if (++cur.j == s.bpu) { cur.j = 0; ++cur.unit; }
+    cursor_step(cur, s.bpu, s.n_vb);
 }
 
 // fp16 probability of a scaled logit: fp16(exp(x - M) / S)   (models/llama_kivi.py:375); rS = 1 / S
@@ -1185,7 +1242,7 @@ __device__ __forceinline__ float prob_f32(float x, float M, float nMl, float S, 
     return fmaf(fmaf(-q, S, e), rS, q);     // one Newton step on the quotient = the correctly rounded e / S
 }
 
-template <int KB, int VB, int G, int GS, int CW>
+template <int KB, int VB, int G, int GS, int CW, bool RAGGED>
 __global__ void __launch_bounds__(CW * 32, KIVI_MINB)
 sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
 {
@@ -1223,7 +1280,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
     Pipe pp;
     pp.init(smem + (size_t)warp * p.spw * p.stage_bytes, full_all + warp * p.spw, p.spw, p.stage_bytes);
     Cursor cur;
-    cur.unit = u_lo; cur.j = j_lo; cur.half = 0; cur.left = n_mine;
+    cur.unit = u_lo; cur.j = j_lo; cur.half = 0; cur.left = n_mine; cur.s_unit = -1; cur.s_pos = 0;
     int ready_unit = -1;                                                     // last unit whose q.K^T ranges are known to be complete
     if (s.r + 1 == c.R) {                                                    // the step that completes the K window: flush it now
         const int n_slices = 4 * c.B * c.Hkv, n_workers = (int)rg.W;
@@ -1299,7 +1356,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         }
         pp.push();
     }
-    for (int i = commit_async ? 1 : 0; i < p.spw; ++i) sv_issue_next<VB, G, GS>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+    for (int i = commit_async ? 1 : 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
     KIVI_TL(1, gw, 1);
     if (commit_async) {
         pp.wait();
@@ -1311,12 +1368,12 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         if (s.L + 1 > c.R) in.vold = *reinterpret_cast<const uint2*>(st + 512 + 2 * (win_off(s.vhead, lane * 4) - s.vhead * kD));
         __syncwarp();
         pp.pop();
-        sv_issue_next<VB, G, GS>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);     // the freed stage takes the next item at once
+        sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);     // the freed stage takes the next item at once
         commit_unit<KB, VB>(p, s, cu0, lane, scratch, in);
         for (int uu = cu0 + 1; uu < cu1; ++uu) commit_unit<KB, VB>(p, s, uu, lane, scratch, commit_fetch(p, s, uu, lane));
     }
 #else
-    for (int i = 0; i < p.spw; ++i) sv_issue_next<VB, G, GS>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+    for (int i = 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
     KIVI_TL(1, gw, 1);
 #if KIVI_EARLY_COMMIT && KIVI_COMMIT_LATE && !KIVI_COMMIT_IN_QK
     commit_share();
@@ -1401,6 +1458,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         const int u = p.hchunks == 1 ? unit : unit / p.hchunks, hc = p.hchunks == 1 ? 0 : unit % p.hchunks;
         const int uq0 = u * ratio + hc * G;
         const int n_here = min(left, s.bpu - j);                             // this warp's pseudo-blocks of this unit
+        const int start = RAGGED ? unit_start(p, s, unit) : 0;              // positions below it are padding
 
         // ---- (M, S) of every head of the unit from the statistics slots of the qk ranges (identical in every warp);
         // the slots were fetched one unit ahead
@@ -1435,6 +1493,9 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
 
         #pragma unroll 1
         for (int k = 0; k < n_here; ++k, ++j) {
+            if constexpr (RAGGED) {
+                if (ragged_skip(j, s.n_vb, start)) continue;                 // wholly padded: never copied (sv_issue_next)
+            }
             if (j < s.n_vb) {                                                // ---- packed V block (tensor cores)
                 float acc[8][4];
                 float zc[4];
@@ -1461,6 +1522,10 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                             __half2 pr = __floats2half2_rn(prob_f32(f.x, M[h], nMl[h], S[h], rS[h]), prob_f32(f.y, M[h], nMl[h], S[h], rS[h]));
                             if (tt >= nt) pr = __float2half2_rn(0.f);        // tokens beyond the packed length belong to the window
                             else if (tt + 1 >= nt) pr = __halves2half2(__low2half(pr), __float2half_rn(0.f));
+                            if constexpr (RAGGED) {                          // padding: probability 0
+                                if (t0 + tt + 1 < start) pr = __float2half2_rn(0.f);
+                                else if (t0 + tt < start) pr = __halves2half2(__float2half_rn(0.f), __high2half(pr));
+                            }
                             if (p.dbg_probs) {
                                 if (tt < nt) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + t0 + tt] = __low2half(pr);
                                 if (tt + 1 < nt) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + t0 + tt + 1] = __high2half(pr);
@@ -1476,7 +1541,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     }, acc, zc, lane);
                     __syncwarp();
                     pp.pop();
-                    sv_issue_next<VB, G, GS>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+                    sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
@@ -1504,7 +1569,8 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                         } else {
                             x = __half2float(__ldcg(p.w.lg + (int64_t)(uq0 + h) * p.w.ld + s.tv + l0 + lane));
                         }
-                        const __half pr = __float2half_rn(prob_f32(x, M[h], nMl[h], S[h], rS[h]));
+                        __half pr = __float2half_rn(prob_f32(x, M[h], nMl[h], S[h], rS[h]));
+                        if (RAGGED && s.tv + l0 + lane < start) pr = __float2half_rn(0.f);   // padding: probability 0
                         if (p.dbg_probs) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + s.tv + l0 + lane] = pr;
                         pl[h] = __half2float(pr);
                     }
@@ -1538,7 +1604,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 __syncwarp();
                 pp.pop();
-                sv_issue_next<VB, G, GS>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+                sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
                 // lane (g8, t): oacc[mt] = D[16mt + g8 | + 8][heads 2t, 2t+1] -> channel order through shared memory
                 #pragma unroll
                 for (int mt = 0; mt < 8; ++mt)
@@ -1647,7 +1713,7 @@ static inline int64_t carve_workspace(const CacheDesc& c, int n_units, int G, in
     return off;
 }
 
-template <int KB, int VB, int G, int GS>
+template <int KB, int VB, int G, int GS, bool RAGGED>
 static int launch_attention(AttnParams& p, bool overlap_prologue, cudaStream_t st)
 {
     const CacheDesc& c = p.c;
@@ -1676,8 +1742,8 @@ static int launch_attention(AttnParams& p, bool overlap_prologue, cudaStream_t s
     if (tn.stages_per_warp >= 1 && tn.stages_per_warp <= p.spw) p.spw = tn.stages_per_warp;
     if (p.spw < 1) return KIVI_ERR_CAPACITY;
     const size_t smem = (size_t)kCW * p.spw * p.stage_bytes + fixed;
-    auto kqk = qk_kernel<KB, G, GS, kCW>;
-    auto ksv = sv_kernel<KB, VB, G, GS, kCW>;
+    auto kqk = qk_kernel<KB, G, GS, kCW, RAGGED>;
+    auto ksv = sv_kernel<KB, VB, G, GS, kCW, RAGGED>;
     static std::atomic<unsigned long long> optin_qk{0}, optin_sv{0};        // per kernel instantiation, one bit per device
     rc = ensure_dynamic_smem(kqk, max_smem, di.ordinal, optin_qk); if (rc) return rc;
     rc = ensure_dynamic_smem(ksv, max_smem, di.ordinal, optin_sv); if (rc) return rc;
@@ -1706,20 +1772,28 @@ static int launch_attention(AttnParams& p, bool overlap_prologue, cudaStream_t s
     return post_launch();
 }
 
-template <int KB, int VB>
-static int dispatch_attention(AttnParams& p, int G, bool overlap_prologue, cudaStream_t st)
+template <int KB, int VB, bool RAGGED>
+static int dispatch_attention_g(AttnParams& p, int G, bool overlap_prologue, cudaStream_t st)
 {
     #define KIVI_GS(GS_)                                                                  \
         if (p.c.g == GS_) {                                                               \
-            if (G == 4) return launch_attention<KB, VB, 4, GS_>(p, overlap_prologue, st);                   \
-            if (G == 2) return launch_attention<KB, VB, 2, GS_>(p, overlap_prologue, st);                   \
-            return launch_attention<KB, VB, 1, GS_>(p, overlap_prologue, st);                               \
+            if (G == 4) return launch_attention<KB, VB, 4, GS_, RAGGED>(p, overlap_prologue, st);           \
+            if (G == 2) return launch_attention<KB, VB, 2, GS_, RAGGED>(p, overlap_prologue, st);           \
+            return launch_attention<KB, VB, 1, GS_, RAGGED>(p, overlap_prologue, st);                       \
         }
     KIVI_GS(32)
     KIVI_GS(64)
     KIVI_GS(128)
     #undef KIVI_GS
     return KIVI_ERR_GROUP;
+}
+
+// kv_start == NULL runs the instantiations without any padding logic
+template <int KB, int VB>
+static int dispatch_attention(AttnParams& p, int G, bool overlap_prologue, cudaStream_t st)
+{
+    if (p.kv_start) return dispatch_attention_g<KB, VB, true>(p, G, overlap_prologue, st);
+    return dispatch_attention_g<KB, VB, false>(p, G, overlap_prologue, st);
 }
 
 }  // namespace kivi

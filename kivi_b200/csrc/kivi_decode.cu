@@ -31,9 +31,10 @@ extern "C" int64_t kivi_decode_workspace_bytes(const kivi_cache_t* cache, int ma
     return carve_workspace(c, c.B * c.Hkv * (ratio / G), G, max_kv_len, nullptr, nullptr);
 }
 
-extern "C" int kivi_decode_attention_f16(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,
-                                         const void* mask, void* out, void* workspace, int64_t workspace_bytes,
-                                         void* dbg_logits, void* dbg_probs, int64_t dbg_stride, int max_kv_len, void* stream)
+// both entries: kv_start == NULL is the unpadded call (the kernels without any padding logic)
+static int decode_attention(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,
+                            const int32_t* kv_start, const void* mask, void* out, void* workspace, int64_t workspace_bytes,
+                            void* dbg_logits, void* dbg_probs, int64_t dbg_stride, int max_kv_len, void* stream)
 {
     AttnParams p;
     int rc = make_desc(cache, &p.c);
@@ -42,7 +43,9 @@ extern "C" int kivi_decode_attention_f16(const kivi_cache_t* cache, const void* 
     if (max_kv_len <= 0) return KIVI_ERR_SHAPE;
     if (max_kv_len > p.c.k_cap_blocks * kBlockTokens) return KIVI_ERR_CAPACITY;
     if (reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return KIVI_ERR_ALIGN;
+    if (reinterpret_cast<uintptr_t>(kv_start) % 4 != 0) return KIVI_ERR_ALIGN;
     p.q = (const __half*)q; p.k_new = (const __half*)k_new; p.v_new = (const __half*)v_new; p.mask = (const __half*)mask;
+    p.kv_start = kv_start;
     p.out = (__half*)out; p.dbg_logits = (__half*)dbg_logits; p.dbg_probs = (__half*)dbg_probs; p.dbg_stride = dbg_stride;
     const bool overlap = (cache->flags & KIVI_CACHE_OVERLAP_PROLOGUE) != 0;   // the q.K^T launch may overlap its predecessor
     const int ratio = p.c.H / p.c.Hkv;
@@ -61,6 +64,23 @@ extern "C" int kivi_decode_attention_f16(const kivi_cache_t* cache, const void* 
     return KIVI_ERR_BITS;
 }
 
+extern "C" int kivi_decode_attention_f16(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,
+                                         const void* mask, void* out, void* workspace, int64_t workspace_bytes,
+                                         void* dbg_logits, void* dbg_probs, int64_t dbg_stride, int max_kv_len, void* stream)
+{
+    return decode_attention(cache, q, k_new, v_new, nullptr, mask, out, workspace, workspace_bytes, dbg_logits, dbg_probs,
+                            dbg_stride, max_kv_len, stream);
+}
+
+extern "C" int kivi_decode_attention_ragged_f16(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,
+                                                const int32_t* kv_start, const void* mask, void* out, void* workspace,
+                                                int64_t workspace_bytes, void* dbg_logits, void* dbg_probs, int64_t dbg_stride,
+                                                int max_kv_len, void* stream)
+{
+    return decode_attention(cache, q, k_new, v_new, kv_start, mask, out, workspace, workspace_bytes, dbg_logits, dbg_probs,
+                            dbg_stride, max_kv_len, stream);
+}
+
 // Test hook (tests/test_ranges_cpu.py): the work split of the decode kernels, evaluated on the host.  kernel 0 = q.K^T costs,
 // 1 = p.V costs; out_lo receives (unit, item) of the first position of ranges 0 .. W (2 * (W + 1) ints, the last = the end);
 // out_owner (may be NULL) receives owner(unit, item) for every position in order.  Returns W (or a negative error).
@@ -72,6 +92,63 @@ extern "C" int kivi_debug_range_split(int n_units, int n_b, int n_w, int w_cap, 
         if (out_owner)
             for (int u = 0; u < n_units; ++u)
                 for (int j = 0; j < rg.per_unit; ++j) out_owner[(long long)u * rg.per_unit + j] = rg.owner(u, j);
+        return (int)rg.W;
+    };
+    if (kernel == 0) { Ranges<CostQK> rg; rg.init(n_units, n_b, n_w, w_cap); return run(rg); }
+    Ranges<CostSV> rg; rg.init(n_units, n_b, n_w, w_cap);
+    return run(rg);
+}
+
+// Test hook (tests/test_ragged_cpu.py): the stage sequence of every warp of a ragged call, evaluated on the host with the
+// kernels' own cursor functions.  kernel 0 = q.K^T (n_b = K blocks, n_w = K window items), 1 = p.V; unit_start[u] = the start
+// of work unit u's sequence (clamped to kv_len as the kernels do).  issued: (warp, unit, item, half) of every copy the producer
+// (ragged_seek + cursor_step) issues; consumed: the same for every stage the item loop waits on.  n_out[0], n_out[1] receive
+// the counts; cap = entries (of 4 ints) each array holds.  Returns W, or a negative error.
+extern "C" int kivi_debug_ragged_items(int n_units, int n_b, int n_w, int w_cap, int kernel, const int* unit_start, int kv_len,
+                                       int* issued, int* consumed, int64_t cap, int64_t* n_out)
+{
+    if (n_units <= 0 || n_b < 0 || n_w < 0 || w_cap <= 0 || kv_len < 0) return KIVI_ERR_SHAPE;
+    if (!unit_start || !issued || !consumed || !n_out) return KIVI_ERR_NULL;
+    auto run = [&](auto rg) -> int {
+        const int per_unit = rg.per_unit;
+        auto start_of = [&](int un) { return clamp_start(unit_start[un], kv_len); };
+        int64_t ni = 0, nc = 0;
+        auto put = [&](int* dst, int64_t& n, int w, int u, int j, int h) {
+            if (n >= cap) return false;
+            dst[4 * n] = w; dst[4 * n + 1] = u; dst[4 * n + 2] = j; dst[4 * n + 3] = h;
+            ++n;
+            return true;
+        };
+        for (int w = 0; w < (int)rg.W; ++w) {
+            int u_lo, j_lo, u_hi, j_hi;
+            rg.lo(w, u_lo, j_lo); rg.lo(w + 1, u_hi, j_hi);
+            const int n_mine = (u_hi - u_lo) * per_unit + (j_hi - j_lo);
+            // producer: *_issue_next
+            Cursor cur;
+            cur.unit = u_lo; cur.j = j_lo; cur.half = 0; cur.left = n_mine; cur.s_unit = -1; cur.s_pos = 0;
+            while (ragged_seek(cur, per_unit, n_b, start_of)) {
+                if (!put(issued, ni, w, cur.unit, cur.j, cur.half)) return KIVI_ERR_CAPACITY;
+                cursor_step(cur, per_unit, n_b);
+            }
+            // consumer: the item loop of the kernels (one visit per unit)
+            int unit = u_lo, j = j_lo, left = n_mine;
+            while (left > 0) {
+                const int n_here = left < per_unit - j ? left : per_unit - j;
+                const int start = start_of(unit);
+                for (int k = 0; k < n_here; ++k, ++j) {
+                    if (ragged_skip(j, n_b, start)) continue;
+                    if (j < n_b) {
+                        for (int h = 0; h < kParts; ++h)
+                            if (!put(consumed, nc, w, unit, j, h)) return KIVI_ERR_CAPACITY;
+                    } else if (j < per_unit - 1) {
+                        if (!put(consumed, nc, w, unit, j, 0)) return KIVI_ERR_CAPACITY;
+                    }
+                }
+                left -= n_here;
+                if (j == per_unit) { j = 0; ++unit; }
+            }
+        }
+        n_out[0] = ni; n_out[1] = nc;
         return (int)rg.W;
     };
     if (kernel == 0) { Ranges<CostQK> rg; rg.init(n_units, n_b, n_w, w_cap); return run(rg); }

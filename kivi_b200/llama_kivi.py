@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .cache import KiviCache
+from .cache import KiviCache, kv_start_from_mask
 from .matmul import cuda_bmm_fA_qB_outer
 from .new_pack import triton_quantize_and_pack_along_last_dim
 
@@ -344,6 +344,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._rope = None
         self.cache: KiviCache | None = None
         self._graph = None
+        self._graph_ragged = False          # the captured step calls the left-padded attention entry
         self._fast = None
         self._dist_tokens = None            # [world * B] ids gathered inside the step (greedy sampling, world > 1)
         self._dist_in_graph = True
@@ -541,7 +542,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                cfg.hidden_size // cfg.num_attention_heads, cfg.k_bits, cfg.v_bits, cfg.group_size,
                                cfg.residual_length, max_tokens, device=dev,
                                overlap_prologue=True)       # the attention call follows the layer's RoPE kernel
-        self._graph = None
+        self._graph, self._graph_ragged = None, False
         self._pos = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._ids = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._logits = torch.zeros((batch, cfg.vocab_size), dtype=torch.float32, device=dev)
@@ -561,14 +562,32 @@ class LlamaForCausalLM_KIVI(nn.Module):
         return self.cache
 
     @torch.no_grad()
-    def prefill(self, input_ids):
-        """Run the prompt, fill the cache (models/llama_kivi.py:401-452), return last-position logits."""
+    def prefill(self, input_ids, attention_mask=None):
+        """Run the prompt, fill the cache (models/llama_kivi.py:401-452), return last-position logits.
+        attention_mask: None or an HF padding mask [B, n] of a LEFT-padded batch (ValueError otherwise).  The prompt
+        attention then takes the additive mask of the tuple path, positions follow HF (cumsum - 1, pad positions 1), and
+        the decode steps skip each sequence's padding (KiviCache.set_kv_start).  An all-ones mask is no mask."""
         assert self.cache is not None, "call init_cache() first"
         B, n = input_ids.shape
-        positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
         pasts = [(self.cache, i) for i in range(len(self.model.layers))]
-        h, _ = self._run_layers(input_ids, positions, pasts)
-        self._pos.fill_(n)
+        starts = None
+        if attention_mask is not None:
+            starts = kv_start_from_mask(attention_mask)
+            if not bool(starts.any()):
+                starts = None
+        if starts is None:
+            positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
+            h, _ = self._run_layers(input_ids, positions, pasts)
+            self._pos.fill_(n)
+        else:
+            am = attention_mask.to(input_ids.device)
+            positions = am.long().cumsum(-1) - 1                            # prepare_inputs_for_generation (:908-948)
+            positions.masked_fill_(am == 0, 1)
+            mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device)
+            h, _ = self._run_layers(input_ids, positions, pasts, mask)
+            starts = starts.to(self._pos.device)
+            self._pos.copy_((n - starts).to(torch.long).view(B, 1))
+            self.cache.set_kv_start(starts)
         return self.lm_head(h[:, -1]).float()
 
     @torch.no_grad()
@@ -712,6 +731,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if not use_graph:
             self._step_body()
         else:
+            if self._graph is not None and self._graph_ragged != self.cache.ragged:
+                self._graph = None                                           # captured with the other attention entry
             if self._graph is None:
                 # warm-up on a side stream (cuBLAS workspaces, lazy module loading, NCCL channels), then capture
                 state = self.cache.state.clone()
@@ -735,7 +756,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                     self._step_body()
                 self.launches_per_step = _lib.launch_count() - n0            # libkivi_b200 launches replayed by every step
                 # capture does not execute: state is still the pre-step state
-                self._graph = g
+                self._graph, self._graph_ragged = g, self.cache.ragged
             self._graph.replay()
         if self._dist_tokens is not None and not self._dist_in_graph:
             from . import dist as kdist
@@ -748,12 +769,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
                  max_length: int | None = None, do_sample: bool = False, **unused):
         """Greedy decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
         max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Sampling is outside
-        the hot path: do_sample is rejected; a padding mask must be all ones (equal-length prompts, as everywhere the
-        reference's cache keeps ONE kv_seq_len per batch, :309, :455)."""
+        the hot path: do_sample is rejected.  attention_mask: an HF padding mask of a LEFT-padded batch (prefill(); the
+        decode steps skip each sequence's padding); right padding raises ValueError."""
         if do_sample:
             raise NotImplementedError("kivi_b200.generate decodes greedily; sample from decode_step() logits instead")
-        if attention_mask is not None and not bool(attention_mask.to(torch.bool).all()):
-            raise NotImplementedError("padded prompts: use forward() with the 9-tuple cache (mask support) instead")
+        if attention_mask is not None:
+            kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
         B, n = input_ids.shape
         if max_new_tokens is None:
             if max_length is None:
@@ -761,7 +782,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             max_new_tokens = max_length - n
         if self.cache is None or self.cache.batch != B or self.cache.max_tokens < n + max_new_tokens:
             self.init_cache(B, n + max_new_tokens)
-        logits = self.prefill(input_ids)
+        logits = self.prefill(input_ids, attention_mask)
         out = [input_ids]
         tok = logits.argmax(-1, keepdim=True)
         for _ in range(max_new_tokens - 1):
