@@ -198,8 +198,13 @@ int64_t kivi_decode_workspace_bytes(const kivi_cache_t* cache, int max_kv_len);
  * fp16 logits of its blocks and one (max, sum exp) pair per unit it touches.  (2) p.V (programmatic dependent launch
  * on (1)): a warp normalises its logits slices with the unit's combined statistics, accumulates, and writes one
  * partial record per unit; the last arriver of a unit adds the records in fixed order, rounds, writes `out` and
- * updates the cache.  The contraction of a packed block runs on mma.sync (codes as exact fp16 denormals x exact
- * hi/lo split of x*scale, fp32 accumulate); the query heads of a KV head share the MMAs (GQA).
+ * updates the cache.  The contraction of a packed block runs on mma.sync (codes as exact fp16 denormals x a hi/lo
+ * split of x*scale into two fp16, fp32 accumulate); the query heads of a KV head share the MMAs (GQA).  The split is
+ * exact while |x*scale| >~ 2^-4 (the residual lo above fp16's smallest step 2^-24); x is brought into that range by
+ * exact powers of two undone on the fp32 accumulators where it would not be: a query head with max|q| < 1/8 is scaled
+ * into [1, 2) (2-bit K) or [4, 8) (4-bit K), and in a packed V block whose largest scale is below 1/16 the probabilities
+ * are scaled up by a further power of two chosen from that scale and the softmax denominator.  Other inputs are computed
+ * exactly as without the prescale.
  * Launch (1) reads `state` and its first K blocks at once: it is an ordinary launch unless cache->flags has
  * KIVI_CACHE_OVERLAP_PROLOGUE (see there). */
 int kivi_decode_attention_f16(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,

@@ -30,9 +30,9 @@
 //   SIMT needs one LOP3 + one FFMA per code and is bound by the 16-lane ALU pipe.  Here the tensor cores are an UNPACK
 //   AMORTISER: the only per-code work left is isolating the field, ONE LOP3 per PAIR of codes:
 //     A (16 outer x 16 inner, fp16)  codes as fp16 denormals code * 2^(P-24), P >= 4 (exact in mma.sync: Lay<>::shr)
-//     B (16 inner x 8 cols,  fp16)  column (group, head, part): x_i * s_i,G split EXACTLY with two half2
-//                                   instructions: hi = x*s (rounded), lo = fma(x, s, -hi) (the residual of
-//                                   an fp16 product is an fp16); G query heads share the MMA (GQA is free)
+//     B (16 inner x 8 cols,  fp16)  column (group, head, part): x_i * s_i,G split with two half2 instructions:
+//                                   hi = x*s (rounded), lo = fma(x, s, -hi) (exact while lo stays above 2^-24;
+//                                   x is prescaled into range, see kProbScale); G query heads share the MMA
 //     C (16 outer x 8 cols,  fp32)  row o, columns (G(o), h, hi | lo) are the wanted sums; the other
 //                                   columns are cross terms and are ignored.  Products exact, fp32 accumulate.
 //   The zero term is one more MMA per 16 inner indices with exact fp16 operands (rows = z_G, cols = x_h).
@@ -155,9 +155,41 @@ constexpr int kPartTokens = 16 * kHalfChunks;   // inner indices (V: tokens) per
 constexpr int kResTile = 16;                // tokens per fp16-window item (256 B each): one MMA tile of tokens
 constexpr int kResBytes = kResTile * kD * 2;
 constexpr float kRcpSqrtD = 1.0f / 11.313708f;   // ATen: x * (1.0f / float(math.sqrt(128)))  (llama_kivi.py:339)
-// probabilities are kept x 2^6 while they feed the MMAs: exact, and it keeps the fp16 residual fma(p, s, -hi) of
-// small probabilities out of the denormal range
+// The hi / lo split of x*s in the B operands (b_prep) is exact only while the residual lo stays above fp16's smallest step
+// 2^-24, i.e. for |x*s| >~ 2^-4; below that lo is rounded and the error grows as the magnitudes shrink.  Where the error
+// would be material, x is brought into range by exact powers of two that the fp32 epilogues undo (scaling by 2^k commutes
+// with every fp32 rounding of the contraction).  Inputs outside those regimes take exactly the arithmetic they always took:
+//   q.K^T: a head whose max|q| is below 2^-3 enters scaled into [2^Q, 2^(Q+1)) (q_prescale), Q = 0 for 2-bit K, 2 for 4-bit
+//          K; other heads enter as they are.  A finite K scale is at most 65504 / (2^bits - 1), so hi = fp16(q*s) cannot
+//          overflow for a prescaled head.
+//   p.V:   probabilities enter x 2^6.  A packed block whose largest V scale m is below 2^-4 (pv_boost) takes them
+//          x 2^(6 + e + b) instead, e = floor(log2 S) of the softmax denominator S, b = min(-4 - floor(log2 m), 9): max p <= 1 / S,
+//          so the scaled probabilities stay below 2^(6 + b) <= 2^15 and p*s below 8, at any context length.
 constexpr float kProbScale = 64.f, kProbScaleInv = 1.f / 64.f;
+constexpr float kQPrescaleBelow = 0.125f;
+
+// (2^k, 2^-k) with max|q| * 2^k in [2^Q, 2^(Q+1)) for 0 < max|q| < 2^-3, (1, 1) otherwise; every fp16 is a normal fp32
+template <int KB>
+__device__ __forceinline__ float2 q_prescale(float mx) {
+    constexpr int Q = KB == 4 ? 2 : 0;
+    if (!(mx > 0.f) || !(mx < kQPrescaleBelow)) return make_float2(1.f, 1.f);
+    const int k = Q - ((int)((__float_as_uint(mx) >> 23) & 0xff) - 127);   // Q - floor(log2 max|q|) in [Q + 4, Q + 24]
+    return make_float2(__uint_as_float((uint32_t)(127 + k) << 23), __uint_as_float((uint32_t)(127 - k) << 23));
+}
+// b of a packed V block whose largest |scale| is m: 0 unless 0 < m < 2^-4 (NaN, inf: 0)
+__device__ __forceinline__ int pv_boost(float m) {
+    if (!(m > 0.f) || !(m < 0.0625f)) return 0;
+    return min(-4 - ((int)((__float_as_uint(m) >> 23) & 0xff) - 127), 9);     // >= 1: floor(log2 m) <= -5
+}
+// exponent of the extra probability scale of a boosted block: e + b, e = floor(log2 S) in [0, 15] (S >= 1: the largest
+// logit contributes exp(0) = 1; NaN -> 15)
+__device__ __forceinline__ int pv_extra_exp(float S, int b) {
+    return min(max((int)((__float_as_uint(S) >> 23) & 0xff) - 127, 0), 15) + b;
+}
+__device__ __forceinline__ __half2 pow2_h2(int e) {                           // 2^e as an fp16 pair, 0 <= e <= 15
+    const uint32_t h = (uint32_t)(15 + e) << 10, hh = h | (h << 16);
+    return *reinterpret_cast<const __half2*>(&hh);
+}
 
 // Programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization attribute may start while its
 // predecessor in the stream is still draining; pdl_wait() blocks until the predecessor has completed and flushed, and
@@ -259,8 +291,8 @@ __device__ __forceinline__ float fast_exp(float x) {
 __device__ __forceinline__ uint32_t h2_as_u32(const __half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
 __device__ __forceinline__ __half2 u32_as_h2(const uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
 
-// One B-fragment register: column part 0 -> hi = fp16(x*s); part 1 -> lo = x*s - hi (exact: the residual of an fp16
-// product is an fp16).
+// One B-fragment register: column part 0 -> hi = fp16(x*s); part 1 -> lo = x*s - hi, exact while it is not below fp16's
+// smallest step (the callers prescale x where it would not be: q_prescale, pv_boost).
 #ifndef KIVI_BPREP2
 #define KIVI_BPREP2 1                    // 1: hi, then a PREDICATED fma(x, s, -hi) in the lo lanes (2 instructions); 0: branch-free 3
 #endif
@@ -945,14 +977,26 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
         const int n_here = min(left, s.ipu - j);                             // this warp's pseudo-blocks of this unit
         const int start = RAGGED ? unit_start(p, s, unit) : 0;              // positions below it are padding
 
-        // ---- this warp's copy of q: half2 pairs in B-fragment order, fp32 in channel order
+        // ---- this warp's copy of q: half2 pairs in B-fragment order (prescaled: q_prescale), fp32 in channel order (as is);
+        // qpost_blk / qpost_win undo the prescale of the head of this lane's packed-block / window-item outputs
+        float qpost_blk = 1.f, qpost_win = 1.f;
         __syncwarp();
         #pragma unroll
         for (int h = 0; h < G; ++h) {
-            q2[h * 32 + lane] = qf[h];
             const __half2* qh = reinterpret_cast<const __half2*>(&ql[h]);
             const float2 a = __half22float2(qh[0]), b2 = __half22float2(qh[1]);
             *reinterpret_cast<float4*>(qlin + h * kD + lane * 4) = make_float4(a.x, a.y, b2.x, b2.y);
+            float mx = fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(b2.x), fabsf(b2.y)));
+            #pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            const float2 ps = q_prescale<KB>(mx);
+            auto sc = [&](uint32_t w) {                                      // exact: max|q| * 2^k < 8
+                const float2 f = __half22float2(u32_as_h2(w));
+                return h2_as_u32(__floats2half2_rn(f.x * ps.x, f.y * ps.x));
+            };
+            q2[h * 32 + lane] = make_uint2(sc(qf[h].x), sc(qf[h].y));
+            if (h == h_l) qpost_blk = ps.y;
+            if (h == (lane >> 2)) qpost_win = ps.y;
         }
         __syncwarp();
         if (left > n_here) fetch_q(unit + 1);                                // the range continues into the next unit
@@ -1001,13 +1045,13 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 #pragma unroll
                 for (int e = 0; e < Slots<G, GS>::k; ++e) x[e] = -INFINITY;
                 if (!slow && !padded && nvalid >= kBlockTokens) {
-                    finalize<KB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int o, float v) {
+                    finalize<KB, G, GS>(acc, zsel, lane, qpost_blk, [&](int slot, int o, float v) {
                         const __half hv = scale_logit(v);
                         row[o] = hv;
                         x[slot] = __half2float(hv);
                     });
                 } else {
-                    finalize<KB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int o, float v) {
+                    finalize<KB, G, GS>(acc, zsel, lane, qpost_blk, [&](int slot, int o, float v) {
                         if (o < nvalid) {
                             __half hv = scale_logit(v);                      // fp16 scaled (+ mask): the softmax input
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + j * kBlockTokens + o);
@@ -1048,7 +1092,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                         const int t = (e >> 1) * 8 + 2 * t4 + (e & 1);
                         x[e] = -INFINITY;
                         if (t < nt) {
-                            __half hv = scale_logit(e < 2 ? d0[e] : d1[e - 2]);
+                            __half hv = scale_logit((e < 2 ? d0[e] : d1[e - 2]) * qpost_win);
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + s.tk + t0 + t);
                             p.w.lg[rowi * p.w.ld + s.tk + t0 + t] = hv;
                             if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + s.tk + t0 + t] = hv;
@@ -1507,14 +1551,41 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     #pragma unroll
                     for (int e = 0; e < 4; ++e) zc[e] = 0.f;
                 }
+                static_assert(kParts == 1, "the probability scale of a block (pv_boost) is chosen from the whole block's scales");
+                int boost = 0;                                               // pv_boost of the block (warp-uniform)
                 #pragma unroll 1
                 for (int half = 0; half < kParts; ++half) {
                     const int t0 = j * kBlockTokens + half * kPartTokens, nt = s.tv - t0;   // nt >= kPartTokens except at the end of the store
                     pp.wait();
                     uint8_t* st = pp.cons();
-                    __half* prob = reinterpret_cast<__half*>(st + kHalfBytes);   // [G][kPartTokens] logits -> probabilities x 2^6
+                    __half* prob = reinterpret_cast<__half*>(st + kHalfBytes);   // [G][kPartTokens] logits -> scaled probabilities
+                    {   // the block's largest |V scale|: lane reads the (chunk, group, t) meta units lane, lane + 32, ...
+                        const uint4* mt = reinterpret_cast<const uint4*>(st + kHalfChunks * Lay<VB>::kChunkBytes);
+                        const __half h0 = __float2half_rn(0.f);
+                        __half2 m2 = __half2half2(h0);
+                        #pragma unroll
+                        for (int i = 0; i < NG; ++i) {
+                            const int idx = lane + 32 * i;               // {z, s} of tokens 16 c + 2 t + {0, 1} and + {8, 9}
+                            const uint4 w = mt[idx];
+                            __half2 sa = __habs2(u32_as_h2(w.y)), sb = __habs2(u32_as_h2(w.w));
+                            if (nt < kPartTokens) {                      // the end of the store: later slots hold no data
+                                const int tok = 16 * ((idx >> 2) / NG) + 2 * (idx & 3);
+                                sa = __halves2half2(tok < nt ? __low2half(sa) : h0, tok + 1 < nt ? __high2half(sa) : h0);
+                                sb = __halves2half2(tok + 8 < nt ? __low2half(sb) : h0, tok + 9 < nt ? __high2half(sb) : h0);
+                            }
+                            m2 = __hmax2(m2, __hmax2(sa, sb));
+                        }
+                        float m = fmaxf(__low2float(m2), __high2float(m2));
+                        #pragma unroll
+                        for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                        boost = pv_boost(m);
+                        if (lane == 0) *reinterpret_cast<volatile int*>(obuf) = boost;   // obuf: unused by packed blocks
+                    }
                     #pragma unroll
                     for (int h = 0; h < G; ++h) {
+                        // x 2^E, E = 6 (+ e + b in a boosted block), as two exact fp16 factors: 2^E may exceed the fp16 range
+                        const int E = 6 + (boost ? pv_extra_exp(S[h], boost) : 0), E1 = min(E, 15);
+                        const __half2 f1 = pow2_h2(E1), f2 = pow2_h2(E - E1);
                         #pragma unroll
                         for (int e = 0; e < kPartTokens / 64; ++e) {         // 2 tokens per lane and pass
                             const int tt = (e * 32 + lane) * 2;
@@ -1530,7 +1601,9 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                                 if (tt < nt) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + t0 + tt] = __low2half(pr);
                                 if (tt + 1 < nt) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + t0 + tt + 1] = __high2half(pr);
                             }
-                            *reinterpret_cast<__half2*>(prob + h * kPartTokens + tt) = __hmul2(pr, __float2half2_rn(kProbScale));   // exact
+                            pr = __hmul2(pr, f1);                            // exact
+                            if (boost) pr = __hmul2(pr, f2);
+                            *reinterpret_cast<__half2*>(prob + h * kPartTokens + tt) = pr;
                         }
                     }
                     __syncwarp();
@@ -1545,7 +1618,17 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
-                finalize<VB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int, float v) { run[slot] += v; });
+                const int boost_b = *reinterpret_cast<volatile const int*>(obuf);   // parked across the MMAs (register pressure)
+                __syncwarp();
+                if (!boost_b) {
+                    finalize<VB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int, float v) { run[slot] += v; });
+                } else {                                                     // back to the x 2^6 of the running sums
+                    float post = 0.f;
+                    #pragma unroll
+                    for (int h = 0; h < G; ++h)
+                        if (h == h_l) post = __uint_as_float((uint32_t)(127 - pv_extra_exp(S[h], boost_b)) << 23);
+                    finalize<VB, G, GS>(acc, zsel, lane, post, [&](int slot, int, float v) { run[slot] += v; });
+                }
             } else if (j < s.bpu - 1) {                                      // ---- fp16 V window item (tensor cores)
                 // D[channel][head] = sum_tok V[tok][channel] * p_h[tok]: A = the window rows as they lie in the stage
                 // ([token][channel], swizzled units), delivered transposed by ldmatrix; B = the probabilities (exact fp16)

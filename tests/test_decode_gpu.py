@@ -7,6 +7,8 @@ The attention output passes through the reference's fp16 rounding points (fp16 l
 to 2^-7 at |s| ~ 8) legitimately moves a probability by ~1%; so every stage is checked against the
 oracle applied to the kernel's OWN previous-stage values (rtol 1e-3 + fp32 accumulation floor), and
 the end-to-end output against the full oracle chain with the looser, stated E2E tolerance."""
+import itertools
+
 import numpy as np
 import pytest
 import torch
@@ -138,6 +140,17 @@ DECODE_CASES = [  # B, H, Hkv, kb, vb, g, R, n_prefill, steps
 ]
 
 
+def _oracle_prefill(k, v, g, kb, vb, R):
+    """ref.prefill_cache with K and V packed at their own bit widths (the oracle's prefill uses one width for both)."""
+    st = list(ref.prefill_cache(k, v, g, kb, vb, R))
+    if st[0] is not None:
+        nq = st[0].shape[-1] * (32 // kb)
+        st[0], st[2], st[3] = ref.pack_lastdim(np.ascontiguousarray(k[:, :, :nq].transpose(0, 1, 3, 2)), g, kb)
+    if st[4] is not None:
+        st[4], st[6], st[7] = ref.pack_lastdim(np.ascontiguousarray(v[:, :, :-R]), g, vb)
+    return tuple(st)
+
+
 @pytest.mark.parametrize("B,H,Hkv,kb,vb,g,R,n0,steps", DECODE_CASES)
 def test_decode_steps_match_oracle(B, H, Hkv, kb, vb, g, R, n0, steps, mode):
     rng = np.random.default_rng(n0 * 13 + H + R)
@@ -146,13 +159,7 @@ def test_decode_steps_match_oracle(B, H, Hkv, kb, vb, g, R, n0, steps, mode):
         k = rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)
         v = rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)
         cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda())
-        st = list(ref.prefill_cache(k, v, g, kb, vb, R))
-        if st[0] is not None:
-            nq = st[0].shape[-1] * (32 // kb)
-            st[0], st[2], st[3] = ref.pack_lastdim(np.ascontiguousarray(k[:, :, :nq].transpose(0, 1, 3, 2)), g, kb)
-        if st[4] is not None:
-            st[4], st[6], st[7] = ref.pack_lastdim(np.ascontiguousarray(v[:, :, :-R]), g, vb)
-        st = tuple(st)
+        st = _oracle_prefill(k, v, g, kb, vb, R)
     else:
         st = (None, None, None, None, None, np.zeros((B, Hkv, 0, 128), np.float16), None, None, 0)
     tmax = 512
@@ -189,6 +196,127 @@ def test_decode_steps_match_oracle(B, H, Hkv, kb, vb, g, R, n0, steps, mode):
 
 def _oracle_step(st, q, k_new, v_new, g, kb, vb, R, mask=None):
     return ref.decode_step(st, q, k_new, v_new, g, kb, vb, R, mask)
+
+
+NEG16 = np.finfo(np.float16).min
+
+
+def _start_mask(starts, B, T):
+    """The additive finfo(fp16).min mask [B, 1, 1, T] that per-sequence starts stand for (the new token stays visible)."""
+    m = np.zeros((B, 1, 1, T), np.float16)
+    for b, s in enumerate(starts):
+        m[b, ..., :min(max(s, 0), T - 1)] = NEG16
+    return m
+
+
+def _checked_step(cache, st, q, k_new, v_new, g, kb, vb, R, starts=None):
+    """One decode step of `cache` (oracle 9-tuple `st` before it) with every check of the oracle suite:
+      * the production epilogue (no debug pointers) and the instrumented one give the same bits;
+      * every stage against the oracle applied to the kernel's own previous stage (_stage_checks);
+      * the output end to end against ref.decode_step;
+      * the exported cache equals the oracle's 9-tuple bit for bit.
+    starts: per-sequence first visible positions (the cache must be in ragged mode); the oracle then runs with the
+    equivalent additive mask, and the kernel's logits of excluded positions, which are not part of its result (wholly padded
+    blocks are not even computed), are replaced by the masked value before the stage checks.  Returns the new tuple."""
+    B, H = q.shape[:2]
+    T = st[8] + 1
+    qd, kd, vd = (torch.from_numpy(np.ascontiguousarray(a[:, :, 0])).cuda() for a in (q, k_new, v_new))
+    dbg_s = torch.zeros((B, H, T + 8), dtype=torch.float16, device="cuda")
+    dbg_p = torch.zeros_like(dbg_s)
+    out_fast = cache.decode_attention(0, qd, kd, vd).clone()
+    out = cache.decode_attention(0, qd, kd, vd, dbg_logits=dbg_s, dbg_probs=dbg_p)
+    cache.advance()
+    torch.cuda.synchronize()
+    assert torch.equal(out_fast.view(torch.int16), out.view(torch.int16)), "production and instrumented epilogues disagree"
+    got_out = to_np(out)[:, :, None, :]
+    got_s, got_p = to_np(dbg_s)[:, :, None, :T].copy(), to_np(dbg_p)[:, :, None, :T]
+    mask = None
+    if starts is not None:
+        mask = _start_mask(starts, B, T)
+        got_s[np.broadcast_to(mask == NEG16, got_s.shape)] = NEG16
+    _stage_checks(st, q, k_new, v_new, g, kb, vb, R, got_out, got_s, got_p,
+                  mask=None if mask is None else np.broadcast_to(mask, (B, H, 1, T)))
+    exp_out, _, st = _oracle_step(st, q, k_new, v_new, g, kb, vb, R, mask)
+    e, x = got_out.astype(np.float64), exp_out.astype(np.float64)
+    err = np.abs(e - x)
+    tol = E2E_RTOL * np.abs(x) + E2E_ATOL_FRAC * np.abs(x).max()
+    assert (err <= tol).all(), f"end-to-end: worst err / bar {(err / np.maximum(tol, 1e-30)).max():.2f}"
+    _tuple_equal(cache.export(0), st)
+    return st
+
+
+# ---------------------------------------------------------------------------------------------------
+# every attention instantiation against the oracle: k_bits x v_bits x g x G x {unpadded, ragged}
+# ---------------------------------------------------------------------------------------------------
+def _header_set(name):
+    """A supported-value set as include/kivi_b200.h documents it, e.g. `group_size in {32,64,128}`."""
+    import os
+    import re
+    with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "kivi_b200.h")) as f:
+        m = re.search(name + r" in \{([0-9, ]+)\}", f.read())
+    assert m, name
+    return tuple(int(x) for x in m.group(1).split(","))
+
+
+BITS = (2, 4)
+GROUPS = _header_set("group_size")
+RESIDUALS = _header_set("residual_length")
+GQA_CHUNKS = (1, 2, 4)                                    # KIVI_CACHE_GQA_CHUNK: 1 / 2 / 4 query heads per work unit
+RAGGED_STARTS = [0, 300, 129, 512]                        # whole blocks skipped, blocks partly padded (as test_padded_blocks_are_not_read)
+
+
+def _instantiation_cases():
+    cases = []
+    for (ik, kb), (iv, vb), g, (iG, G), ragged in itertools.product(enumerate(BITS), enumerate(BITS), GROUPS,
+                                                                      enumerate(GQA_CHUNKS), (False, True)):
+        Rs = [R for R in RESIDUALS if R % g == 0]
+        # as (k_bits, v_bits) run through their four values for a fixed (g, G), R runs through every residual length
+        R = Rs[(2 * ik + iv + iG + ragged) % len(Rs)]
+        ratio = 2 * G if (2 * ik + iv + iG + GROUPS.index(g)) % 5 == 0 else G   # a few: one KV head spans two units
+        cases.append(pytest.param(kb, vb, g, G, R, ratio, ragged,
+                                  id=f"k{kb}v{vb}-g{g}-G{G}-R{R}-ratio{ratio}-{'ragged' if ragged else 'unpadded'}"))
+    return cases
+
+
+@pytest.mark.parametrize("kb,vb,g,G,R,ratio,ragged", _instantiation_cases())
+def test_every_instantiation_matches_oracle(kb, vb, g, G, R, ratio, ragged):
+    """Every (k_bits, v_bits, g, G, RAGGED) kernel pair the dispatcher can pick, against the C oracle: prefill to
+    r = R - 3, then six steps that cross a K flush and move the V ring head, every step fully checked (_checked_step).
+    Ragged cases: one sequence unpadded, the others with whole 128-token blocks skipped, partly padded blocks, and
+    starts inside the fp16 K and V windows; the oracle runs with the equivalent additive mask."""
+    from kivi_b200.cache import KiviCache
+    Hkv = 2 if ratio == G else 1
+    H = ratio * Hkv
+    n0 = max(3, -(-540 // R)) * R + R - 3
+    rng = np.random.default_rng(1000 * kb + 100 * vb + g + 7 * G + R + ratio + 3 * ragged)
+    B = 6 if ragged else 2
+    cache = KiviCache(1, B, H, Hkv, 128, kb, vb, g, R, n0 + 16, gqa_chunk=G)
+    k = rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)
+    v = rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)
+    starts = None
+    if ragged:
+        tk, r, tv, L = _mirror_lengths(n0, R)
+        starts = RAGGED_STARTS + [tk + r // 2, tv + L // 2]
+        assert len(starts) == B and max(starts) < n0
+    cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda(),
+                  kv_start=None if starts is None else torch.tensor(starts))
+    assert cache.ragged == ragged
+    st = _oracle_prefill(k, v, g, kb, vb, R)
+    r0 = cache.r
+    for step in range(6):
+        q = (rng.standard_normal((B, H, 1, 128)) * 0.7).astype(np.float16)
+        k_new = rng.standard_normal((B, Hkv, 1, 128)).astype(np.float16)
+        v_new = rng.standard_normal((B, Hkv, 1, 128)).astype(np.float16)
+        st = _checked_step(cache, st, q, k_new, v_new, g, kb, vb, R, starts)
+    assert r0 == R - 3 and cache.r == 3 and cache.vhead != 0, "the steps crossed a K flush and moved the V ring head"
+    assert cache.read_state()[:6] == [cache.tk, cache.r, cache.tv, cache.L, cache.vhead, cache.kv_len]
+
+
+def _mirror_lengths(n, R):
+    """(tk, r, tv, L) after a prefill of n tokens (models/llama_kivi.py:425-452)."""
+    nqk = (0 if n < R else n - n % R) if n % R != 0 else n
+    nqv = 0 if n <= R else n - R
+    return nqk, n - nqk, nqv, n - nqv
 
 
 def test_decode_with_mask(mode):
