@@ -243,9 +243,46 @@ int kivi_cache_advance(const kivi_cache_t* cache, void* stream);
 
 /* Copy the 8 words of `state` to host memory (synchronises `stream`).  state[6] is an error word that the decode kernels
  * set instead of touching memory when the device-side lengths exceed what the call declared (max_kv_len, window
- * capacities): KIVI_STATE_ERR_CAPACITY.  kivi_cache_prefill_f16 / kivi_cache_import_f16 clear it. */
+ * capacities): KIVI_STATE_ERR_CAPACITY.  kivi_cache_refill_f16 / kivi_cache_shift_f16 / kivi_cache_shift_state set
+ * KIVI_STATE_ERR_LENGTHS instead of writing when the device-side lengths are not those the call was given.
+ * kivi_cache_prefill_f16 / kivi_cache_import_f16 clear it. */
 #define KIVI_STATE_ERR_CAPACITY 1
+#define KIVI_STATE_ERR_LENGTHS  2
 int kivi_cache_read_state(const kivi_cache_t* cache, int32_t* host_state8, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Continuous batching: the batch rows ("slots") of a live cache are reused without touching the other sequences.
+ * All sequences keep the shared length T = tk + r = tv + L.  A new prompt of n <= T tokens goes into slot `seq`
+ * right-aligned, at positions [T - n, T); the caller then sets kv_start[seq] = T - n and decodes with
+ * kivi_decode_attention_ragged_f16.
+ * ------------------------------------------------------------------------------------------ */
+/* Refill the Hkv units of sequence `seq` (one layer) with a new prompt.  k, v [Hkv, n, 128] fp16 contiguous, K post-RoPE
+ * at the prompt's own positions 0 .. n-1.  Lengths are passed by the host, as for kivi_cache_export_f16 (tk % R == 0,
+ * r < R, L <= R, tk + r == tv + L, L == R once tv > 0; vhead < v_res_cap), and 1 <= n <= T.  With s = T - n the
+ * sequence's units then hold EXACTLY what kivi_cache_prefill_f16 writes for the T-token sequence
+ * x[p] = k/v[max(p - s, 0)] -- every block of the slot, the padding included -- with the V window rotated so that its
+ * token i sits in ring slot (vhead + i) % v_res_cap.  The pad positions repeat the first real token: a per-channel K group
+ * (packed, or still in the fp16 window until a later K flush) that mixes pad and real tokens then takes its min / max,
+ * i.e. its scale and zero, from the real tokens alone; every other pad position is excluded by kv_start.
+ * `state` and the other sequences are not written.  If the device-side lengths are not the ones passed, nothing is
+ * written and KIVI_STATE_ERR_LENGTHS is set in state[6].  Three launches at most (K store, V store, windows). */
+int kivi_cache_refill_f16(const kivi_cache_t* cache, int seq, const void* k, const void* v, int n,
+                          int tk, int r, int tv, int L, int vhead, void* stream);
+
+/* Drop the first `shift` positions of every sequence of one layer: block j of each K and V store moves to block
+ * j - shift/128 (source and destination overlap; the move is ordered) and the vacated last shift/128 blocks that held
+ * tokens are zeroed, as an import leaves the blocks past its lengths.  The fp16 K window and V ring do not move.
+ * shift > 0, shift % max(128, R) == 0 (blocks, K flush periods and quantisation groups stay aligned), shift <= tk,
+ * shift <= tv, with tk / tv the current lengths passed by the host (checked on the device like kivi_cache_refill_f16).
+ * Call it for every layer, then kivi_cache_shift_state once.  The caller guarantees that no live sequence has
+ * kv_start < shift: the dropped positions must be padding for every sequence that still decodes. */
+int kivi_cache_shift_f16(const kivi_cache_t* cache, int shift, int tk, int tv, void* stream);
+
+/* The bookkeeping of a shift, once per model after every layer's kivi_cache_shift_f16 (like kivi_cache_advance): tk, tv
+ * and kv_len of `state` decrease by `shift`, r, L and vhead do not change, and every kv_start[b] decreases by `shift`
+ * (kv_start: a device int32[B], or NULL).  RoPE positions are per sequence and do not change.  Same requirements on
+ * `shift`; if the device-side tk or tv is below it, nothing changes and KIVI_STATE_ERR_LENGTHS is set. */
+int kivi_cache_shift_state(const kivi_cache_t* cache, int shift, int32_t* kv_start, void* stream);
 
 /* Copy the cache out in the reference's 9-tuple layout (models/llama_kivi.py:454-455); lengths are
  * passed by the host (it mirrors `state`).  k_code [U,128,tk/fpi] i32, k_scale/k_mn [U,128,tk/g],

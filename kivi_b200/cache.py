@@ -5,7 +5,9 @@ the reference keeps a per-layer 9-tuple that it regrows with torch.cat every ste
 allocated once (sizes from the C ABI), the lengths live in a device int32[8] shared by all layers, and
 one CUDA launch per layer does attention + cache update.  `export(layer)` returns the reference's 9-tuple.
 A left-padded batch keeps one length for all sequences; `set_kv_start` names each sequence's first real token, and the
-attention then skips the padding on the device (kivi_decode_attention_ragged_f16).
+attention then skips the padding on the device (kivi_decode_attention_ragged_f16).  The same offsets let one batch row
+("slot") take a new sequence while the others decode: `refill` writes a prompt right-aligned to the shared length,
+`release` idles a slot, and `shift` drops timeline positions that no live sequence sees any more.
 """
 from __future__ import annotations
 
@@ -60,7 +62,13 @@ def _bind():
     _lib.bind("kivi_cache_export_f16", i32, [P, i32, i32, i32, i32, i32] + [vp] * 9)
     _lib.bind("kivi_cache_import_f16", i32, [P, i32, i32, i32, i32] + [vp] * 9)
     _lib.bind("kivi_cache_read_state", i32, [P, ctypes.POINTER(ctypes.c_int32), vp])
+    _lib.bind("kivi_cache_refill_f16", i32, [P, i32, vp, vp] + [i32] * 6 + [vp])
+    _lib.bind("kivi_cache_shift_f16", i32, [P, i32, i32, i32, vp])
+    _lib.bind("kivi_cache_shift_state", i32, [P, i32, vp, vp])
     _BOUND = True
+
+
+IDLE_START = 1 << 30        # kv_start of a released slot: beyond any length, so it attends to its new token only
 
 
 class KiviCache:
@@ -106,6 +114,7 @@ class KiviCache:
         # left padding: first visible position of every sequence (device-resident, so a captured step reads the current
         # values); used only while `ragged` is set, otherwise the unpadded entry runs
         self.kv_start = torch.zeros(batch, dtype=torch.int32, device=self.device)
+        self.kv_start_host = [0] * batch                             # host mirror of kv_start (valid while `ragged`)
         self.ragged = False
         # host mirror of `state` (its evolution is deterministic)
         self.tk = self.r = self.tv = self.L = self.vhead = self.kv_len = 0
@@ -143,8 +152,77 @@ class KiviCache:
         t = torch.as_tensor(kv_start).reshape(-1)
         if t.numel() != self.batch:
             raise ValueError(f"kv_start needs {self.batch} entries, got {t.numel()}")
-        self.kv_start.copy_(t.to(torch.int32))
+        t = t.to(torch.int32)
+        self.kv_start.copy_(t)
+        self.kv_start_host = [int(x) for x in t.tolist()]
         self.ragged = True
+
+    # ------------------------------------------------------------------ slots (continuous batching)
+    def set_seq_start(self, seq: int, start: int):
+        """kv_start[seq] = start (one sequence's first visible position) and turn the ragged entry on; the other
+        sequences keep their starts (0 if the batch was not padded)."""
+        if not 0 <= seq < self.batch:
+            raise ValueError(f"sequence {seq} outside the batch of {self.batch}")
+        if not self.ragged:
+            self.kv_start.zero_()
+            self.kv_start_host = [0] * self.batch
+            self.ragged = True
+        self.kv_start[seq] = int(start)
+        self.kv_start_host[seq] = int(start)
+
+    def release(self, seq: int):
+        """Make slot `seq` idle: its start lies beyond every length, so its attention reads no cached byte and returns
+        its own new token's V.  Its cache contents stay until a refill overwrites them."""
+        self.set_seq_start(seq, IDLE_START)
+
+    def live_starts(self):
+        """{seq: start} of the sequences that see part of the cache (start < kv_len)."""
+        starts = self.kv_start_host if self.ragged else [0] * self.batch
+        return {b: s for b, s in enumerate(starts) if s < self.kv_len}
+
+    def refill(self, layer: int, seq: int, k: torch.Tensor, v: torch.Tensor):
+        """Write a new prompt's k, v [Hkv, n, 128] (or [1, Hkv, n, 128]) fp16, K post-RoPE at positions 0 .. n-1, into
+        slot `seq` of `layer`, right-aligned to the shared length T (positions T - n .. T - 1; the positions before repeat
+        its first token).  The slot then holds what prefill() writes for that T-token sequence; the other slots and the
+        lengths do not change.  Call set_seq_start(seq, T - n) once all layers are refilled."""
+        _lib.require_cuda(k, v)
+        if k.dim() == 4:
+            assert k.shape[0] == 1 and v.shape[0] == 1, "refill takes one sequence"
+            k, v = k.reshape(k.shape[1:]), v.reshape(v.shape[1:])
+        Hkv, n, D = k.shape
+        assert (Hkv, D) == (self.num_kv_heads, self.head_dim) and v.shape == k.shape
+        assert k.dtype == torch.float16 and v.dtype == torch.float16
+        if not 1 <= n <= self.kv_len:
+            raise ValueError(f"a prompt of {n} tokens does not fit the shared length {self.kv_len} (1 <= n <= length)")
+        k, v = k.contiguous(), v.contiguous()
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().kivi_cache_refill_f16(
+                ctypes.byref(self._structs[layer]), seq, k.data_ptr(), v.data_ptr(), n, self.tk, self.r, self.tv, self.L,
+                self.vhead, _lib.stream_ptr(self.device)), "kivi_cache_refill_f16")
+
+    def shift(self, tokens: int):
+        """Drop the first `tokens` positions of the shared timeline in every layer (packed blocks move down; windows stay)
+        and lower the lengths and every kv_start by as much.  tokens: a positive multiple of max(128, R), at most tk and tv.
+        Raises ValueError if a live sequence would lose a visible position (start < tokens)."""
+        q = max(128, self.residual_length)
+        if tokens <= 0 or tokens % q != 0:
+            raise ValueError(f"shift must be a positive multiple of {q}, got {tokens}")
+        if tokens > self.tk or tokens > self.tv:
+            raise ValueError(f"shift {tokens} exceeds the packed lengths (tk {self.tk}, tv {self.tv})")
+        low = {b: s for b, s in self.live_starts().items() if s < tokens}
+        if low:
+            raise ValueError(f"shift {tokens} would drop visible positions of live sequences (starts {low})")
+        with torch.cuda.device(self.device):
+            stream = _lib.stream_ptr(self.device)
+            for layer in range(self.n_layers):
+                _lib.check(_lib.lib().kivi_cache_shift_f16(ctypes.byref(self._structs[layer]), tokens, self.tk, self.tv,
+                                                           stream), "kivi_cache_shift_f16")
+            _lib.check(_lib.lib().kivi_cache_shift_state(ctypes.byref(self._structs[0]), tokens,
+                                                         self.kv_start.data_ptr() if self.ragged else None, stream),
+                       "kivi_cache_shift_state")
+        self.tk, self.tv, self.kv_len = self.tk - tokens, self.tv - tokens, self.kv_len - tokens
+        if self.ragged:
+            self.kv_start_host = [s - tokens for s in self.kv_start_host]
 
     # ------------------------------------------------------------------ operations
     def prefill(self, layer: int, k: torch.Tensor, v: torch.Tensor, kv_start=None):
@@ -214,6 +292,9 @@ class KiviCache:
             _lib.check(_lib.lib().kivi_cache_read_state(ctypes.byref(self._structs[0]), host, _lib.stream_ptr(self.device)),
                        "kivi_cache_read_state")
         st = list(host)
+        if st[6] & 2:                                                # KIVI_STATE_ERR_LENGTHS
+            raise RuntimeError(f"kivi_b200: a refill or shift refused to run (state error word {st[6]}): the device-side "
+                               f"lengths {st[:6]} are not the ones the host passed")
         if st[6] != 0:
             raise RuntimeError(f"kivi_b200: the decode kernels refused to run (state error word {st[6]}): the device-side "
                                f"lengths {st[:6]} exceed the capacity the cache was created with")

@@ -6,6 +6,8 @@
 //                                       K, no .transpose(2,3).contiguous() temp; same kernel for V)
 //   torch.cat growth      :350-352, :393-395, :391 -> nothing: blocks / ring slots are written in place
 //   9-tuple               :454-455   -> kivi_cache_export_f16 (tests / interop only)
+// Continuous batching (no counterpart in the reference): kivi_cache_refill_f16 re-runs the prefill kernels for one sequence
+// of a live cache, kivi_cache_shift_f16 / kivi_cache_shift_state drop the oldest blocks of the shared timeline.
 #include "kivi_decode.cuh"
 
 namespace kivi {
@@ -24,25 +26,44 @@ __device__ __forceinline__ __half scale_of(float mnf, float mxf, float maxq) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Where the prefill kernels write.  A prefill fills every unit from its own prompt: FillDesc{} (all zero).  A refill
+// (kivi_cache_refill_f16) fills the units u0 .. u0 + Hkv - 1 of one sequence of a live cache with a T-token sequence x
+// whose first s positions repeat the first real token, x[p] = src[max(p - s, 0)]; window token i of V lands in ring slot
+// (ring + i) % v_res_cap; `state` is read, not written, and must hold the lengths the host passed (tk, tv; T = n + s).
+// ------------------------------------------------------------------------------------------------
+struct FillDesc { int u0, s, ring, refill, tk, tv; };
+
+// a refill whose lengths differ from the device's `state` writes nothing (residual_prefill_kernel flags it)
+__device__ __forceinline__ bool fill_refused(const CacheDesc& c, const FillDesc& f, int T) {
+    if (!f.refill) return false;
+    const int* st = c.state;
+    return st[ST_TK] != f.tk || st[ST_R] != T - f.tk || st[ST_TV] != f.tv || st[ST_L] != T - f.tv ||
+           st[ST_VHEAD] != f.ring || st[ST_KVLEN] != T;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Prefill: one CTA per (unit, block of 128 tokens).  The [128 tokens][128 channels] fp16 tile is staged in
 // shared memory; quantisation runs along the OUTER dim of the block in groups of g (K: tokens of a channel,
 // V: channels of a token); the codes are then gathered into the A-fragment words of the block.
 //   IS_K = true : inner = channel, outer = token     IS_K = false: inner = token, outer = channel
+// x holds n rows per unit (grid.y indexes the units of x; the cache unit is f.u0 + grid.y).
 // ------------------------------------------------------------------------------------------------
 template <int BITS, bool IS_K>
 __global__ void __launch_bounds__(256)
-block_prefill_kernel(CacheDesc c, const __half* __restrict__ x, int n, int nq)
+block_prefill_kernel(CacheDesc c, const __half* __restrict__ x, int n, int nq, FillDesc f)
 {
     extern __shared__ __align__(16) uint8_t sm[];
     __half (*tile)[kD + 8] = reinterpret_cast<__half (*)[kD + 8]>(sm);               // [token][channel]
     uint8_t (*codes)[kD + 4] = reinterpret_cast<uint8_t (*)[kD + 4]>(sm + kBlockTokens * (kD + 8) * 2);  // [inner][outer]
-    const int u = blockIdx.y, blk = blockIdx.x;
+    if (fill_refused(c, f, n + f.s)) return;
+    const int u = f.u0 + blockIdx.y, blk = blockIdx.x;
     const int t0 = blk * kBlockTokens;
     const int nt = min(kBlockTokens, nq - t0);
-    const __half* src = x + ((int64_t)u * n + t0) * kD;
+    const __half* src = x + (int64_t)blockIdx.y * n * kD;
     for (int i = threadIdx.x; i < nt * (kD / 8); i += blockDim.x) {
         const int t = i / (kD / 8), p = i % (kD / 8);
-        *reinterpret_cast<uint4*>(&tile[t][p * 8]) = __ldg(reinterpret_cast<const uint4*>(src + (int64_t)t * kD) + p);
+        const int row = max(t0 + t - f.s, 0);                                      // pad positions repeat source row 0
+        *reinterpret_cast<uint4*>(&tile[t][p * 8]) = __ldg(reinterpret_cast<const uint4*>(src + (int64_t)row * kD) + p);
     }
     for (int i = threadIdx.x; i < kD * (kD + 4); i += blockDim.x) (&codes[0][0])[i] = 0;
     __syncthreads();
@@ -87,22 +108,81 @@ block_prefill_kernel(CacheDesc c, const __half* __restrict__ x, int n, int nq)
     (void)ngrp;
 }
 
-// residual windows of the prompt + state
+// residual windows of the prompt + state (a refill leaves `state` alone, or flags lengths that differ from it)
 __global__ void __launch_bounds__(256)
 residual_prefill_kernel(CacheDesc c, const __half* __restrict__ k, const __half* __restrict__ v, int n,
-                        int nqk, int nqv)
+                        int nqk, int nqv, FillDesc f)
 {
-    const int u = blockIdx.x;
-    const int r = n - nqk, L = n - nqv;
+    const int T = n + f.s;
+    if (fill_refused(c, f, T)) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(&c.state[6], KIVI_STATE_ERR_LENGTHS);
+        return;
+    }
+    const int u = f.u0 + blockIdx.x;
+    const int r = T - nqk, L = T - nqv;
+    const uint4* ks = reinterpret_cast<const uint4*>(k + (int64_t)blockIdx.x * n * kD);
+    const uint4* vs = reinterpret_cast<const uint4*>(v + (int64_t)blockIdx.x * n * kD);
     for (int i = threadIdx.x; i < r * (kD / 8); i += blockDim.x)                 // window rows are unit-swizzled (win_unit)
         reinterpret_cast<uint4*>(c.k_res + (int64_t)u * c.R * kD)[win_unit(i / 16, i % 16)] =
-            __ldg(reinterpret_cast<const uint4*>(k + ((int64_t)u * n + nqk) * kD) + i);
+            __ldg(ks + (int64_t)max(nqk + i / 16 - f.s, 0) * 16 + i % 16);
     for (int i = threadIdx.x; i < L * (kD / 8); i += blockDim.x)
-        reinterpret_cast<uint4*>(c.v_res + (int64_t)u * c.v_res_cap * kD)[win_unit(i / 16, i % 16)] =
-            __ldg(reinterpret_cast<const uint4*>(v + ((int64_t)u * n + nqv) * kD) + i);
-    if (u == 0 && threadIdx.x == 0) {
+        reinterpret_cast<uint4*>(c.v_res + (int64_t)u * c.v_res_cap * kD)[win_unit((f.ring + i / 16) % c.v_res_cap, i % 16)] =
+            __ldg(vs + (int64_t)max(nqv + i / 16 - f.s, 0) * 16 + i % 16);
+    if (!f.refill && u == 0 && threadIdx.x == 0) {
         c.state[ST_TK] = nqk; c.state[ST_R] = r; c.state[ST_TV] = nqv; c.state[ST_L] = L;
         c.state[ST_VHEAD] = 0; c.state[ST_KVLEN] = n; c.state[6] = 0; c.state[7] = 0;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Timeline shift: drop the first d blocks of every unit's K and V store (block j -> j - d) so that the shared length can
+// shrink.  One CTA per (unit, store) moves the bytes of blocks [d, nblk) down by d blocks, D = d blocks at a time: chunk
+// i reads [(i+1)D, (i+2)D) and writes [iD, (i+1)D), which chunk i - 1 read; a CTA barrier per chunk orders the overlap.
+// The windows do not move; the vacated last d blocks are zeroed.  The device lengths must be those the host passed (else: nothing moves, state[6] flagged).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+shift_blocks_kernel(CacheDesc c, int d, int tk, int tv)
+{
+    if (c.state[ST_TK] != tk || c.state[ST_TV] != tv) {
+        if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) atomicOr(&c.state[6], KIVI_STATE_ERR_LENGTHS);
+        return;
+    }
+    const int u = blockIdx.x, isv = blockIdx.y;
+    const int bb = lay_block_bytes(isv ? c.v_bits : c.k_bits, c.g);
+    const int nblk = cdiv(isv ? tv : tk, kBlockTokens);                          // blocks holding tokens before the shift
+    uint4* base = reinterpret_cast<uint4*>((isv ? c.v_store : c.k_store) + (int64_t)u * (isv ? c.v_cap_blocks : c.k_cap_blocks) * bb);
+    const int64_t D = (int64_t)d * bb / 16, total = (int64_t)(nblk - d) * bb / 16;
+    constexpr int kUnroll = 4;                                                   // loads in flight per thread before its stores
+    for (int64_t c0 = 0; c0 < total; c0 += D) {
+        const int64_t cnt = min(D, total - c0);
+        for (int64_t i = threadIdx.x; i < cnt; i += kUnroll * blockDim.x) {
+            uint4 t[kUnroll];
+            #pragma unroll
+            for (int e = 0; e < kUnroll; ++e)
+                if (i + e * blockDim.x < cnt) t[e] = base[c0 + D + i + e * blockDim.x];
+            #pragma unroll
+            for (int e = 0; e < kUnroll; ++e)
+                if (i + e * blockDim.x < cnt) base[c0 + i + e * blockDim.x] = t[e];
+        }
+        __syncthreads();
+    }
+    // the d blocks that held tokens and now lie past the end are cleared, as a prefill or an import leaves them
+    for (int64_t i = threadIdx.x; i < D; i += blockDim.x) base[total + i] = make_uint4(0u, 0u, 0u, 0u);
+}
+
+// the lengths after a shift (once per model, after every layer's shift_blocks_kernel); kv_start: NULL or [B]
+__global__ void shift_state_kernel(int* state, int shift, int32_t* kv_start, int B)
+{
+    const bool ok = state[ST_TK] >= shift && state[ST_TV] >= shift;
+    __syncthreads();
+    if (!ok) {
+        if (threadIdx.x == 0) atomicOr(&state[6], KIVI_STATE_ERR_LENGTHS);
+        return;
+    }
+    if (kv_start)
+        for (int b = threadIdx.x; b < B; b += blockDim.x) kv_start[b] -= shift;
+    if (threadIdx.x == 0) {
+        state[ST_TK] -= shift; state[ST_TV] -= shift; state[ST_KVLEN] -= shift;
     }
 }
 
@@ -274,6 +354,36 @@ int make_desc(const kivi_cache_t* k, CacheDesc* d)
     return KIVI_OK;
 }
 
+// the launches of a prefill (f = FillDesc{}: n_units = B * Hkv) or of a refill of one sequence (n_units = Hkv):
+// K store, V store, windows (+ state)
+int launch_fill(const CacheDesc& c, const void* k, const void* v, int n, int nqk, int nqv, int n_units, FillDesc f,
+                cudaStream_t st)
+{
+    const size_t smem = (size_t)kBlockTokens * (kD + 8) * 2 + (size_t)kD * (kD + 4);
+    DeviceInfo di;
+    int rc = device_info(&di);
+    if (rc) return rc;
+    static std::atomic<unsigned long long> optin[4];                 // 51.7 KB of dynamic shared memory: opt-in per device
+    rc = ensure_dynamic_smem(block_prefill_kernel<2, true>, (int)smem, di.ordinal, optin[0]); if (rc) return rc;
+    rc = ensure_dynamic_smem(block_prefill_kernel<4, true>, (int)smem, di.ordinal, optin[1]); if (rc) return rc;
+    rc = ensure_dynamic_smem(block_prefill_kernel<2, false>, (int)smem, di.ordinal, optin[2]); if (rc) return rc;
+    rc = ensure_dynamic_smem(block_prefill_kernel<4, false>, (int)smem, di.ordinal, optin[3]); if (rc) return rc;
+    if (nqk > 0) {
+        dim3 grid(cdiv(nqk, kBlockTokens), n_units);
+        if (c.k_bits == 2) block_prefill_kernel<2, true><<<grid, 256, smem, st>>>(c, (const __half*)k, n, nqk, f);
+        else               block_prefill_kernel<4, true><<<grid, 256, smem, st>>>(c, (const __half*)k, n, nqk, f);
+        rc = post_launch(); if (rc) return rc;
+    }
+    if (nqv > 0) {
+        dim3 grid(cdiv(nqv, kBlockTokens), n_units);
+        if (c.v_bits == 2) block_prefill_kernel<2, false><<<grid, 256, smem, st>>>(c, (const __half*)v, n, nqv, f);
+        else               block_prefill_kernel<4, false><<<grid, 256, smem, st>>>(c, (const __half*)v, n, nqv, f);
+        rc = post_launch(); if (rc) return rc;
+    }
+    residual_prefill_kernel<<<n_units, 256, 0, st>>>(c, (const __half*)k, (const __half*)v, n, nqk, nqv, f);
+    return post_launch();
+}
+
 }  // namespace kivi
 
 using namespace kivi;
@@ -312,31 +422,47 @@ extern "C" int kivi_cache_prefill_f16(const kivi_cache_t* cache, const void* k, 
     const int nqk = (n % R != 0) ? (n < R ? 0 : n - n % R) : n;
     const int nqv = (n <= R) ? 0 : n - R;
     if (cdiv(nqk, kBlockTokens) > c.k_cap_blocks || cdiv(nqv, kBlockTokens) > c.v_cap_blocks) return KIVI_ERR_CAPACITY;
-    cudaStream_t st = (cudaStream_t)stream;
     const int U = c.B * c.Hkv;
     if (U > 65535) return KIVI_ERR_UNSUPPORTED;                     // grid.y
-    const size_t smem = (size_t)kBlockTokens * (kD + 8) * 2 + (size_t)kD * (kD + 4);
-    DeviceInfo di;
-    rc = device_info(&di);
+    return launch_fill(c, k, v, n, nqk, nqv, U, FillDesc{0, 0, 0, 0, 0, 0}, (cudaStream_t)stream);
+}
+
+extern "C" int kivi_cache_refill_f16(const kivi_cache_t* cache, int seq, const void* k, const void* v, int n,
+                                     int tk, int r, int tv, int L, int vhead, void* stream)
+{
+    CacheDesc c;
+    int rc = make_desc(cache, &c);
     if (rc) return rc;
-    static std::atomic<unsigned long long> optin[4];                 // 51.7 KB of dynamic shared memory: opt-in per device
-    rc = ensure_dynamic_smem(block_prefill_kernel<2, true>, (int)smem, di.ordinal, optin[0]); if (rc) return rc;
-    rc = ensure_dynamic_smem(block_prefill_kernel<4, true>, (int)smem, di.ordinal, optin[1]); if (rc) return rc;
-    rc = ensure_dynamic_smem(block_prefill_kernel<2, false>, (int)smem, di.ordinal, optin[2]); if (rc) return rc;
-    rc = ensure_dynamic_smem(block_prefill_kernel<4, false>, (int)smem, di.ordinal, optin[3]); if (rc) return rc;
-    if (nqk > 0) {
-        dim3 grid(cdiv(nqk, kBlockTokens), U);
-        if (c.k_bits == 2) block_prefill_kernel<2, true><<<grid, 256, smem, st>>>(c, (const __half*)k, n, nqk);
-        else               block_prefill_kernel<4, true><<<grid, 256, smem, st>>>(c, (const __half*)k, n, nqk);
-        rc = post_launch(); if (rc) return rc;
-    }
-    if (nqv > 0) {
-        dim3 grid(cdiv(nqv, kBlockTokens), U);
-        if (c.v_bits == 2) block_prefill_kernel<2, false><<<grid, 256, smem, st>>>(c, (const __half*)v, n, nqv);
-        else               block_prefill_kernel<4, false><<<grid, 256, smem, st>>>(c, (const __half*)v, n, nqv);
-        rc = post_launch(); if (rc) return rc;
-    }
-    residual_prefill_kernel<<<U, 256, 0, st>>>(c, (const __half*)k, (const __half*)v, n, nqk, nqv);
+    if (seq < 0 || seq >= c.B) return KIVI_ERR_SHAPE;
+    if (tk < 0 || r < 0 || tv < 0 || L < 0 || tk % c.R != 0 || r >= c.R || L > c.R || tk + r != tv + L) return KIVI_ERR_SHAPE;
+    if (tv > 0 && L != c.R) return KIVI_ERR_SHAPE;                  // the V store fills only once the window is full
+    if (vhead < 0 || vhead >= c.v_res_cap) return KIVI_ERR_SHAPE;
+    const int T = tk + r;
+    if (n < 1 || n > T) return KIVI_ERR_SHAPE;
+    if (cdiv(tk, kBlockTokens) > c.k_cap_blocks || cdiv(tv, kBlockTokens) > c.v_cap_blocks) return KIVI_ERR_CAPACITY;
+    if (!k || !v) return KIVI_ERR_NULL;
+    return launch_fill(c, k, v, n, tk, tv, c.Hkv, FillDesc{seq * c.Hkv, T - n, vhead, 1, tk, tv}, (cudaStream_t)stream);
+}
+
+extern "C" int kivi_cache_shift_f16(const kivi_cache_t* cache, int shift, int tk, int tv, void* stream)
+{
+    CacheDesc c;
+    int rc = make_desc(cache, &c);
+    if (rc) return rc;
+    if (shift <= 0 || shift % max(kBlockTokens, c.R) != 0 || shift > tk || shift > tv) return KIVI_ERR_SHAPE;
+    if (cdiv(tk, kBlockTokens) > c.k_cap_blocks || cdiv(tv, kBlockTokens) > c.v_cap_blocks) return KIVI_ERR_CAPACITY;
+    const int U = c.B * c.Hkv;
+    shift_blocks_kernel<<<dim3(U, 2), 256, 0, (cudaStream_t)stream>>>(c, shift / kBlockTokens, tk, tv);
+    return post_launch();
+}
+
+extern "C" int kivi_cache_shift_state(const kivi_cache_t* cache, int shift, int32_t* kv_start, void* stream)
+{
+    CacheDesc c;
+    int rc = make_desc(cache, &c);
+    if (rc) return rc;
+    if (shift <= 0 || shift % max(kBlockTokens, c.R) != 0) return KIVI_ERR_SHAPE;
+    shift_state_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(c.state, shift, kv_start, c.B);
     return post_launch();
 }
 

@@ -201,11 +201,19 @@ class LlamaFlashAttention_KIVI(nn.Module):
     def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None):
         """hidden_states [B, q_len, hidden]; cos/sin broadcastable to [B, 1, q_len, D].
         past_key_value: None (prefill, returns a 9-tuple), a 9-tuple (reference semantics), or a
-        (KiviCache, layer) pair (fused path; prefill fills it, decode is one launch).
+        (KiviCache, layer) pair (fused path; prefill fills it, decode is one launch), or a (KiviCache, layer, seq) triple:
+        the B = 1 prompt of a new sequence, written into slot `seq` of a live cache (KiviCache.refill).
         attention_mask: None or additive [B, 1, q_len, kv_len] (models/llama_kivi.py:364-372)."""
         bsz, q_len, _ = hidden_states.shape
         q, k, v = self._qkv(hidden_states, cos, sin)
-        fused = isinstance(past_key_value, tuple) and len(past_key_value) == 2 and isinstance(past_key_value[0], KiviCache)
+        fused = isinstance(past_key_value, tuple) and len(past_key_value) in (2, 3) and \
+            isinstance(past_key_value[0], KiviCache)
+        if fused and len(past_key_value) == 3:                              # a new sequence into one slot
+            cache, layer, seq = past_key_value
+            attn_output = self._prompt_attention(q, k, v, attention_mask)
+            cache.refill(layer, seq, k, v)
+            attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.hidden_size)
+            return self.o_proj(attn_output), None, past_key_value
         if fused:
             cache, layer = past_key_value
             if q_len > 1:                                                   # prefill (:401-452)
@@ -589,6 +597,28 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self._pos.copy_((n - starts).to(torch.long).view(B, 1))
             self.cache.set_kv_start(starts)
         return self.lm_head(h[:, -1]).float()
+
+    @torch.no_grad()
+    def insert(self, seq: int, prompt_ids):
+        """Start a new sequence in slot `seq` of the running batch (continuous batching): a B = 1 prompt pass at positions
+        0 .. n-1 whose K/V go into that slot right-aligned to the shared length T (KiviCache.refill), then
+        kv_start[seq] = T - n and the slot's position = n.  The other slots are not touched.  Returns the prompt's
+        last-position logits [vocab] fp32; the caller writes the first token into the slot's input (`_ids[seq]`)."""
+        assert self.cache is not None, "call init_cache() / prefill() first"
+        ids = torch.as_tensor(prompt_ids, device=self.cache.device).reshape(1, -1)
+        n, T = ids.shape[1], self.cache.kv_len
+        if not 1 <= n <= T:
+            raise ValueError(f"a prompt of {n} tokens does not fit the shared length {T} (1 <= n <= length)")
+        positions = torch.arange(n, device=ids.device).unsqueeze(0)
+        h, _ = self._run_layers(ids, positions, [(self.cache, i, seq) for i in range(len(self.model.layers))])
+        self._pos[seq] = n
+        self.cache.set_seq_start(seq, T - n)
+        return self.lm_head(h[0, -1]).float()
+
+    def release(self, seq: int):
+        """Make slot `seq` idle (KiviCache.release): it keeps its row of every step but reads no cached byte."""
+        self.cache.release(seq)
+        self._pos[seq] = 0
 
     @torch.no_grad()
     def prefill_synthetic(self, n: int, seed: int = 0):

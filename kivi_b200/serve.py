@@ -1,0 +1,146 @@
+"""Continuous batching on the fused cache path: a finished sequence's batch row ("slot") takes the next request while the
+other sequences keep decoding.
+
+All sequences share one length T (one `state` for the whole batch).  A new prompt of n <= T tokens goes into a free slot
+right-aligned, at positions [T - n, T), with kv_start = T - n (LlamaForCausalLM_KIVI.insert -> KiviCache.refill); a
+finished slot is released (kv_start beyond every length: it reads no cached byte).  T grows by one per step; positions
+that no live sequence sees any more are dropped from the front in multiples of max(128, R) (KiviCache.shift), so the
+timeline stays inside the cache.  Decoding is greedy, as everywhere in this package.
+"""
+from __future__ import annotations
+
+from collections import deque
+
+import torch
+
+from .cache import kv_start_from_mask
+
+
+def plan_admission(T: int, tv: int, max_tokens: int, quantum: int, live_starts, prompt_len: int, new_tokens: int,
+                   longest_pending: int):
+    """Whether the next queued request (prompt_len tokens, new_tokens to generate) may enter a running batch whose shared
+    length is T (tv of it in the packed V store), and after which shift.  A request fits when prompt_len <= T and
+    T + new_tokens <= max_tokens.  If it does not, the timeline may shift by the largest multiple of `quantum` that is at
+    most the smallest start of any live sequence (it loses no visible position), at most tv, and leaves T at least the
+    longest pending prompt (every later insert still fits under T).
+    Returns None when no sequence is live (start the next group with a fresh prefill), else (shift, admit):
+    (0, True) fits now, (s, True) fits after shifting s positions, (0, False) wait for a later step."""
+    live_starts = list(live_starts)
+    if not live_starts:
+        return None
+    if prompt_len <= T and T + new_tokens <= max_tokens:
+        return 0, True
+    room = min(min(live_starts), tv, T - longest_pending)
+    s = max(room, 0) // quantum * quantum
+    if s > 0 and prompt_len <= T - s and T - s + new_tokens <= max_tokens:
+        return s, True
+    return 0, False
+
+
+@torch.no_grad()
+def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None = None, use_graph: bool = True,
+          stats: dict | None = None):
+    """Greedy decoding of a stream of requests with `batch` slots on one cache of `max_tokens` positions.
+    requests: a list of (prompt ids 1-D, max_new_tokens).  Yields (index into requests, new token ids [k] int64 on the
+    host) as each request finishes: after max_new_tokens tokens, or after eos_token_id (included, as in HF).
+    The first `batch` requests start with one left-padded prefill, padded to the longest prompt of the whole list, so every
+    later prompt fits under the shared length.  Each step is one decode_step (its CUDA graph is captured once: the batch
+    is ragged from the start) and one device-to-host read of the sampled ids; finished slots are released and refilled
+    from the queue in order.  stats: an optional dict that receives counters (steps, slot_steps = live slots summed over
+    the steps, inserts, shifts, shifted_tokens, prefills)."""
+    reqs = []
+    for p, m in requests:
+        p = torch.as_tensor(p).reshape(-1).to(torch.long).cpu()
+        if p.numel() < 1 or int(m) < 1:
+            raise ValueError("every request needs at least one prompt token and max_new_tokens >= 1")
+        reqs.append((p, int(m)))
+    if not reqs:
+        return
+    longest = max(p.numel() for p, _ in reqs)
+    for i, (p, m) in enumerate(reqs):
+        if longest + m > max_tokens:
+            raise ValueError(f"request {i}: the longest prompt ({longest}) + max_new_tokens ({m}) exceeds max_tokens "
+                             f"({max_tokens})")
+    if stats is None:
+        stats = {}
+    for key in ("steps", "slot_steps", "inserts", "shifts", "shifted_tokens", "prefills"):
+        stats.setdefault(key, 0)
+    cache = model.cache
+    if cache is None or cache.batch != batch or cache.max_tokens != max_tokens:
+        cache = model.init_cache(batch, max_tokens)
+    quantum = max(128, cache.residual_length)
+    dev = cache.device
+    queue = deque(range(len(reqs)))
+    owner = [None] * batch                  # request index decoding in each slot
+    outs = [[] for _ in range(batch)]
+    done = []
+
+    def emit(slot, tok):
+        """Append a token to the slot's output; finish (release) the slot on EOS or on its token budget."""
+        outs[slot].append(tok)
+        i = owner[slot]
+        if tok == eos_token_id or len(outs[slot]) >= reqs[i][1]:
+            done.append((i, torch.tensor(outs[slot], dtype=torch.long)))
+            owner[slot], outs[slot] = None, []
+            model.release(slot)
+
+    def start_group():
+        rows = [queue.popleft() for _ in range(min(batch, len(queue)))]
+        P = max([reqs[i][0].numel() for i in rows] + [reqs[j][0].numel() for j in queue])
+        ids = torch.zeros((batch, P), dtype=torch.long)
+        mask = torch.zeros((batch, P), dtype=torch.long)
+        mask[:, -1] = 1                                                   # rows without a request: one pad token
+        for b, i in enumerate(rows):
+            n = reqs[i][0].numel()
+            ids[b, P - n:] = reqs[i][0]
+            mask[b, P - n:] = 1
+        ids, mask = ids.to(dev), mask.to(dev)
+        logits = model.prefill(ids, attention_mask=mask)
+        cache.set_kv_start(kv_start_from_mask(mask))                      # ragged from the start: one step graph
+        first = logits.argmax(-1)
+        model._ids.copy_(first.view(batch, 1))
+        first = first.tolist()
+        stats["prefills"] += 1
+        for b in range(batch):
+            if b < len(rows):
+                owner[b] = rows[b]
+                emit(b, first[b])
+            else:
+                model.release(b)
+
+    while queue or any(o is not None for o in owner):
+        if all(o is None for o in owner):
+            start_group()
+        else:
+            for slot in range(batch):
+                while owner[slot] is None and queue:                      # a slot may finish on its first token
+                    p, m = reqs[queue[0]]
+                    plan = plan_admission(cache.kv_len, cache.tv, max_tokens, quantum, cache.live_starts().values(),
+                                          p.numel(), m, max(reqs[j][0].numel() for j in queue))
+                    if plan is None or not plan[1]:
+                        break
+                    if plan[0]:
+                        cache.shift(plan[0])
+                        stats["shifts"] += 1
+                        stats["shifted_tokens"] += plan[0]
+                    i = queue.popleft()
+                    tok = int(model.insert(slot, p.to(dev)).argmax())
+                    model._ids[slot] = tok
+                    owner[slot] = i
+                    stats["inserts"] += 1
+                    emit(slot, tok)
+                if not queue:
+                    break
+        yield from done
+        done.clear()
+        live = [b for b in range(batch) if owner[b] is not None]
+        if not live:
+            continue
+        model.decode_step(use_graph=use_graph)
+        toks = model.next_tokens.tolist()                                 # the step's one device-to-host read
+        stats["steps"] += 1
+        stats["slot_steps"] += len(live)
+        for b in live:
+            emit(b, toks[b])
+        yield from done
+        done.clear()
