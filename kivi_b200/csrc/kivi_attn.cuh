@@ -516,13 +516,6 @@ __device__ __forceinline__ void walk_slots(const float (&run)[Slots<G, GS>::k], 
     }
 }
 
-// quantise one value with its group's (min, scale): quant/new_pack.py:238-241 (rint follows)
-__device__ __forceinline__ float q_code(float x, float mnf, float scf, float rcp, float maxq) {
-    const __half t1 = __float2half_rn(x - mnf);
-    const __half t2 = quot_to_half(__half2float(t1), scf, rcp);
-    return fminf(fmaxf(__half2float(t2), 0.f), maxq);
-}
-
 // ------------------------------------------------------------------------------------------------
 // cache data movement of one unit (models/llama_kivi.py:343-356, :386-399), executed by ONE warp (the last
 // arriver of the unit); cold path, kept out of line.  scratch: 128 bytes of shared memory private to the warp.
@@ -553,7 +546,7 @@ __device__ __noinline__ void commit_unit(const AttnParams& p, const Sched& s, in
     if (lane < kD / 8)                                                                  // window rows are unit-swizzled (win_unit)
         reinterpret_cast<uint4*>(c.v_res + (int64_t)u * c.v_res_cap * kD)[win_unit((s.vhead + s.L) % c.v_res_cap, lane)] = vnew4;
     if (s.L + 1 > c.R) {
-        constexpr int F = 16 / VB, kSlabRows = 16 * F, kSlabs = 128 / kSlabRows;
+        using VL = Lay<VB>;
         const float maxq = (float)((1 << VB) - 1);
         const int bb = lay_block_bytes(VB, g);
         uint8_t* blk = c.v_store + ((int64_t)u * c.v_cap_blocks + s.tv / kBlockTokens) * bb;
@@ -568,12 +561,11 @@ __device__ __noinline__ void commit_unit(const AttnParams& p, const Sched& s, in
             mnf = fminf(mnf, __shfl_xor_sync(0xffffffffu, mnf, o));
             mxf = fmaxf(mxf, __shfl_xor_sync(0xffffffffu, mxf, o));
         }
-        const __half d16 = __float2half_rn(mxf - mnf);
-        const __half sc = __float2half_rn(__fdiv_rn(__half2float(d16), maxq));
+        const __half sc = quant_scale(mnf, mxf, VB);
         const float scf = __half2float(sc), rcp = __frcp_rn(scf);
         uint32_t four = 0;
         #pragma unroll
-        for (int e = 0; e < 4; ++e) four |= (uint32_t)__float2int_rn(q_code(x[e], mnf, scf, rcp, maxq)) << (8 * e);
+        for (int e = 0; e < 4; ++e) four |= quant_code(x[e], mnf, scf, rcp, maxq) << (8 * e);
         __syncwarp();
         reinterpret_cast<uint32_t*>(scratch)[lane] = four;                              // codes[channel] as bytes
         if (lane % lpg == 0) {
@@ -581,12 +573,12 @@ __device__ __noinline__ void commit_unit(const AttnParams& p, const Sched& s, in
             *reinterpret_cast<__half*>(blk + lay_zero_off(VB, g, inner, lane / lpg)) = __float2half_rn(mnf);
         }
         __syncwarp();
-        if (lane < kSlabs * 16) {                                                       // one 16-bit half-word per lane
+        if (lane < VL::kSlabs * 16) {                                                   // one 16-bit half-word per lane
             const int sl = lane >> 4, row = lane & 15;
             uint32_t hw = 0;
             #pragma unroll
-            for (int j = 0; j < F; ++j) hw |= (uint32_t)scratch[sl * kSlabRows + 16 * j + row] << (VB * j);
-            *reinterpret_cast<uint16_t*>(blk + lay_word_off(VB, inner, sl * kSlabRows + row) + 2 * (inner & 1)) = (uint16_t)hw;
+            for (int j = 0; j < VL::F; ++j) hw |= (uint32_t)scratch[sl * VL::kSlabRows + 16 * j + row] << (VB * j);
+            *reinterpret_cast<uint16_t*>(blk + lay_word_off(VB, inner, sl * VL::kSlabRows + row) + 2 * (inner & 1)) = (uint16_t)hw;
         }
         __syncwarp();
     }
@@ -611,7 +603,6 @@ __device__ __noinline__ void k_flush_slice(const AttnParams& p, const Sched& s, 
 {
     const CacheDesc& c = p.c;
     const int g = c.g;
-    constexpr int F = 16 / KB, kSlabRows = 16 * F, kSlabs = 128 / kSlabRows;
     const float maxq = (float)((1 << KB) - 1);
     const int bb = lay_block_bytes(KB, g);
     uint8_t* ub = c.k_store + (int64_t)u * c.k_cap_blocks * bb;
@@ -630,8 +621,8 @@ __device__ __noinline__ void k_flush_slice(const AttnParams& p, const Sched& s, 
         const int o0 = tb % kBlockTokens;                                               // its outer index (multiple of R)
         uint8_t* blk = ub + (int64_t)(tb / kBlockTokens) * bb;
         const bool partial = cnt < kBlockTokens;                                        // other fields of the words are live data
-        // word m of slab sl: inner pair 8 cu + 2q (+1), row 2m + hw   (kivi_decode.cuh: lane' = (row & 7) * 4 + q, r = 2 (cu & 1) + (row >> 3))
-        uint32_t* wbase = reinterpret_cast<uint32_t*>(blk) + (cu >> 1) * kSlabs * 128 + (cu & 1) * 2 + q * 4;
+        // word m of slab sl: inner pair 8 cu + 2q (+1), row 2m + hw  ->  wbase[lay_word_row(sl, 2m + hw)]
+        uint32_t* wbase = reinterpret_cast<uint32_t*>(blk) + lay_word_inner(KB, 8 * cu + 2 * q);
         uint32_t words[8];
         int cur_sl = -1;
         #pragma unroll 1
@@ -652,26 +643,25 @@ __device__ __noinline__ void k_flush_slice(const AttnParams& p, const Sched& s, 
             }
             mn0 = fminf(mn0, __shfl_xor_sync(0xffffffffu, mn0, 16)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 16));   // the other token parity
             mn1 = fminf(mn1, __shfl_xor_sync(0xffffffffu, mn1, 16)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 16));
-            const __half sc0 = __float2half_rn(__fdiv_rn(__half2float(__float2half_rn(mx0 - mn0)), maxq));
-            const __half sc1 = __float2half_rn(__fdiv_rn(__half2float(__float2half_rn(mx1 - mn1)), maxq));
+            const __half sc0 = quant_scale(mn0, mx0, KB), sc1 = quant_scale(mn1, mx1, KB);
             const float scf0 = __half2float(sc0), scf1 = __half2float(sc1), rcp0 = __frcp_rn(scf0), rcp1 = __frcp_rn(scf1);
             const int og = o0 + gl * g;                                                 // outer index of the group's first token
             if (hw == 0) {                                                              // meta entry half: { z, z', s, s' } of the pair
                 __align__(8) __half mz[4] = {__float2half_rn(mn0), __float2half_rn(mn1), sc0, sc1};
-                *reinterpret_cast<uint2*>(blk + lay_zero_off(KB, g, 8 * cu + 2 * q, og / g)) = *reinterpret_cast<const uint2*>(mz);
+                *reinterpret_cast<uint2*>(blk + lay_meta_pair_off(KB, g, 8 * cu + 2 * q, og / g)) = *reinterpret_cast<const uint2*>(mz);
             }
             #pragma unroll 1
             for (int q16 = 0; q16 < g / 16; ++q16) {
                 const int o = og + 16 * q16;                                            // outer index of row 0 of this 16-token chunk
-                const int sl = o / kSlabRows, j = (o % kSlabRows) / 16;
+                const int sl = o / Lay<KB>::kSlabRows, j = (o % Lay<KB>::kSlabRows) / 16;
                 if (sl != cur_sl) {
                     if (cur_sl >= 0) {
                         #pragma unroll
-                        for (int m = 0; m < 8; ++m) wbase[cur_sl * 128 + ((2 * m + hw) & 7) * 16 + ((2 * m + hw) >> 3)] = words[m];
+                        for (int m = 0; m < 8; ++m) wbase[lay_word_row(cur_sl, 2 * m + hw)] = words[m];
                     }
                     cur_sl = sl;
                     #pragma unroll
-                    for (int m = 0; m < 8; ++m) words[m] = partial ? wbase[sl * 128 + ((2 * m + hw) & 7) * 16 + ((2 * m + hw) >> 3)] : 0u;
+                    for (int m = 0; m < 8; ++m) words[m] = partial ? wbase[lay_word_row(sl, 2 * m + hw)] : 0u;
                 }
                 const uint32_t keep = ~((((1u << KB) - 1u) * 0x00010001u) << (KB * j));
                 __half2 v[8];
@@ -680,15 +670,15 @@ __device__ __noinline__ void k_flush_slice(const AttnParams& p, const Sched& s, 
                 #pragma unroll
                 for (int m = 0; m < 8; ++m) {
                     const float2 f = __half22float2(v[m]);
-                    const uint32_t c0 = (uint32_t)__float2int_rn(q_code(f.x, mn0, scf0, rcp0, maxq));
-                    const uint32_t c1 = (uint32_t)__float2int_rn(q_code(f.y, mn1, scf1, rcp1, maxq));
+                    const uint32_t c0 = quant_code(f.x, mn0, scf0, rcp0, maxq);
+                    const uint32_t c1 = quant_code(f.y, mn1, scf1, rcp1, maxq);
                     words[m] = (words[m] & keep) | ((c0 | (c1 << 16)) << (KB * j));
                 }
             }
         }
         if (cur_sl >= 0) {
             #pragma unroll
-            for (int m = 0; m < 8; ++m) wbase[cur_sl * 128 + ((2 * m + hw) & 7) * 16 + ((2 * m + hw) >> 3)] = words[m];
+            for (int m = 0; m < 8; ++m) wbase[lay_word_row(cur_sl, 2 * m + hw)] = words[m];
         }
     }
 }

@@ -12,19 +12,6 @@
 
 namespace kivi {
 
-// same arithmetic as kivi_pack.cu (quant/new_pack.py:238-241)
-__device__ __forceinline__ uint32_t q_one(float x, float mnf, float scf, float rcp, float maxq) {
-    const __half t1 = __float2half_rn(x - mnf);
-    const __half t2 = quot_to_half(__half2float(t1), scf, rcp);
-    float f = __half2float(t2);
-    f = fminf(fmaxf(f, 0.f), maxq);
-    return (uint32_t)__float2int_rn(f);
-}
-__device__ __forceinline__ __half scale_of(float mnf, float mxf, float maxq) {
-    const __half d = __float2half_rn(mxf - mnf);
-    return __float2half_rn(__fdiv_rn(__half2float(d), maxq));
-}
-
 // ------------------------------------------------------------------------------------------------
 // Where the prefill kernels write.  A prefill fills every unit from its own prompt: FillDesc{} (all zero).  A refill
 // (kivi_cache_refill_f16) fills the units u0 .. u0 + Hkv - 1 of one sequence of a live cache with a T-token sequence x
@@ -67,7 +54,7 @@ block_prefill_kernel(CacheDesc c, const __half* __restrict__ x, int n, int nq, F
     }
     for (int i = threadIdx.x; i < kD * (kD + 4); i += blockDim.x) (&codes[0][0])[i] = 0;
     __syncthreads();
-    const int g = c.g, ngrp = 128 / g;
+    const int g = c.g;
     const float maxq = (float)((1 << BITS) - 1);
     const int bb = lay_block_bytes(BITS, g);
     const int cap = IS_K ? c.k_cap_blocks : c.v_cap_blocks;
@@ -81,31 +68,16 @@ block_prefill_kernel(CacheDesc c, const __half* __restrict__ x, int n, int nq, F
         const int inner = w % n_inner, G = w / n_inner;
         float mnf = val(inner, G * g), mxf = mnf;
         for (int i = 1; i < g; ++i) { const float v = val(inner, G * g + i); mnf = fminf(mnf, v); mxf = fmaxf(mxf, v); }
-        const __half sc = scale_of(mnf, mxf, maxq);
+        const __half sc = quant_scale(mnf, mxf, BITS);
         const float scf = __half2float(sc), rcp = __frcp_rn(scf);
-        for (int i = 0; i < g; ++i) codes[inner][G * g + i] = (uint8_t)q_one(val(inner, G * g + i), mnf, scf, rcp, maxq);
+        for (int i = 0; i < g; ++i) codes[inner][G * g + i] = (uint8_t)quant_code(val(inner, G * g + i), mnf, scf, rcp, maxq);
         *reinterpret_cast<__half*>(blkp + lay_scale_off(BITS, g, inner, G)) = sc;
         *reinterpret_cast<__half*>(blkp + lay_zero_off(BITS, g, inner, G)) = __float2half_rn(mnf);
     }
     __syncthreads();
     // gather: one thread per word
-    constexpr int F = 16 / BITS, kSlabRows = 16 * F, kSlabs = 128 / kSlabRows;
-    for (int w = threadIdx.x; w < 8 * kSlabs * 128; w += blockDim.x) {
-        const int ch = w / (kSlabs * 128), sl = (w / 128) % kSlabs, lw = w % 128;
-        const int lane = lw >> 2, r = lw & 3;
-        const int g8 = lane >> 2, t = lane & 3;
-        const int row = g8 + 8 * (r & 1);
-        const int i0 = ch * 16 + 2 * t + 8 * (r >> 1);
-        uint32_t word = 0;
-        #pragma unroll
-        for (int j = 0; j < F; ++j) {
-            const int o = sl * kSlabRows + 16 * j + row;
-            word |= (uint32_t)codes[i0][o] << (BITS * j);
-            word |= (uint32_t)codes[i0 + 1][o] << (16 + BITS * j);
-        }
-        reinterpret_cast<uint32_t*>(blkp)[w] = word;
-    }
-    (void)ngrp;
+    for (int w = threadIdx.x; w < Lay<BITS>::kCodeBytes / 4; w += blockDim.x)
+        reinterpret_cast<uint32_t*>(blkp)[w] = lay_word(BITS, w, [&](int inner, int outer) -> uint32_t { return codes[inner][outer]; });
 }
 
 // residual windows of the prompt + state (a refill leaves `state` alone, or flags lengths that differ from it)
@@ -277,7 +249,7 @@ import_kv_kernel(CacheDesc c, int tk, int tv, int L, int r,
     const int stride = gridDim.x * blockDim.x, tid = blockIdx.x * blockDim.x + threadIdx.x;
     for (int isv = 0; isv < 2; ++isv) {                    // 0: K store (inner = channel, outer = token), 1: V store
         const int bits = isv ? c.v_bits : c.k_bits, fpi = 32 / bits, n_tok = isv ? tv : tk;
-        const int F = 16 / bits, slab_rows = 16 * F, slabs = 128 / slab_rows, wpb = 8 * slabs * 128;   // words per block
+        const int wpb = lay_code_bytes(bits) / 4;          // words per block
         const int bb = lay_block_bytes(bits, g), nblk = cdiv(n_tok, kBlockTokens);
         uint8_t* ub = (isv ? c.v_store : c.k_store) + (int64_t)u * (isv ? c.v_cap_blocks : c.k_cap_blocks) * bb;
         const uint32_t* code = isv ? v_code : k_code;
@@ -287,27 +259,14 @@ import_kv_kernel(CacheDesc c, int tk, int tv, int L, int r,
         const int wpt_v = kD / fpi, gpt_v = kD / g;        // V: words / groups per token row
         for (int i = tid; i < nblk * wpb; i += stride) {
             const int blk = i / wpb, w = i % wpb;
-            const int ch = w / (slabs * 128), sl = (w / 128) % slabs, lw = w % 128;
-            const int lane = lw >> 2, rr = lw & 3;
-            const int row = (lane >> 2) + 8 * (rr & 1);
-            const int i0 = ch * 16 + 2 * (lane & 3) + 8 * (rr >> 1);
-            uint32_t word = 0;
-            for (int par = 0; par < 2; ++par) {
-                const int inner = i0 + par;
-                for (int j = 0; j < F; ++j) {
-                    const int o = sl * slab_rows + 16 * j + row;
-                    uint32_t cd = 0;
-                    if (!isv) {
-                        const int tok = blk * kBlockTokens + o;
-                        if (tok < tk) cd = (code[((int64_t)u * kD + inner) * wpr_k + tok / fpi] >> (bits * (tok % fpi))) & ((1u << bits) - 1u);
-                    } else {
-                        const int tok = blk * kBlockTokens + inner;
-                        if (tok < tv) cd = (code[((int64_t)u * tv + tok) * wpt_v + o / fpi] >> (bits * (o % fpi))) & ((1u << bits) - 1u);
-                    }
-                    word |= cd << (16 * par + bits * j);
+            reinterpret_cast<uint32_t*>(ub + (int64_t)blk * bb)[w] = lay_word(bits, w, [&](int inner, int o) -> uint32_t {
+                if (!isv) {
+                    const int tok = blk * kBlockTokens + o;
+                    return tok < tk ? (code[((int64_t)u * kD + inner) * wpr_k + tok / fpi] >> (bits * (tok % fpi))) & ((1u << bits) - 1u) : 0u;
                 }
-            }
-            reinterpret_cast<uint32_t*>(ub + (int64_t)blk * bb)[w] = word;
+                const int tok = blk * kBlockTokens + inner;
+                return tok < tv ? (code[((int64_t)u * tv + tok) * wpt_v + o / fpi] >> (bits * (o % fpi))) & ((1u << bits) - 1u) : 0u;
+            });
         }
         for (int i = tid; i < nblk * 128 * ngrp; i += stride) {
             const int blk = i / (128 * ngrp), inner = (i / ngrp) % 128, G = i % ngrp;
@@ -352,6 +311,13 @@ int make_desc(const kivi_cache_t* k, CacheDesc* d)
     d->k_store = (uint8_t*)k->k_store; d->v_store = (uint8_t*)k->v_store;
     d->k_res = (__half*)k->k_res; d->v_res = (__half*)k->v_res; d->state = (int*)k->state;
     return KIVI_OK;
+}
+
+// host-passed lengths of a cache of tk + r == tv + L tokens: K flushed in whole windows, both windows within R
+static bool lengths_ok(const CacheDesc& c, int tk, int r, int tv, int L)
+{
+    if (tk < 0 || r < 0 || tv < 0 || L < 0 || tk % c.R != 0 || r >= c.R || L > c.R || tk + r != tv + L) return false;
+    return !(tv > 0 && L != c.R);                                   // the V store fills only once the window is full (:442-452)
 }
 
 // the launches of a prefill (f = FillDesc{}: n_units = B * Hkv) or of a refill of one sequence (n_units = Hkv):
@@ -434,8 +400,7 @@ extern "C" int kivi_cache_refill_f16(const kivi_cache_t* cache, int seq, const v
     int rc = make_desc(cache, &c);
     if (rc) return rc;
     if (seq < 0 || seq >= c.B) return KIVI_ERR_SHAPE;
-    if (tk < 0 || r < 0 || tv < 0 || L < 0 || tk % c.R != 0 || r >= c.R || L > c.R || tk + r != tv + L) return KIVI_ERR_SHAPE;
-    if (tv > 0 && L != c.R) return KIVI_ERR_SHAPE;                  // the V store fills only once the window is full
+    if (!lengths_ok(c, tk, r, tv, L)) return KIVI_ERR_SHAPE;
     if (vhead < 0 || vhead >= c.v_res_cap) return KIVI_ERR_SHAPE;
     const int T = tk + r;
     if (n < 1 || n > T) return KIVI_ERR_SHAPE;
@@ -498,8 +463,7 @@ extern "C" int kivi_cache_import_f16(const kivi_cache_t* cache, int tk, int r, i
     CacheDesc c;
     int rc = make_desc(cache, &c);
     if (rc) return rc;
-    if (tk < 0 || r < 0 || tv < 0 || L < 0 || tk % c.R != 0 || r >= c.R || L > c.R || tk + r != tv + L) return KIVI_ERR_SHAPE;
-    if (tv > 0 && L != c.R) return KIVI_ERR_SHAPE;                  // the V store fills only once the window is full (:442-452)
+    if (!lengths_ok(c, tk, r, tv, L)) return KIVI_ERR_SHAPE;
     if (cdiv(tk, kBlockTokens) > c.k_cap_blocks || cdiv(tv, kBlockTokens) > c.v_cap_blocks) return KIVI_ERR_CAPACITY;
     if (tk > 0 && (!k_code || !k_scale || !k_mn)) return KIVI_ERR_NULL;
     if (tv > 0 && (!v_code || !v_scale || !v_mn)) return KIVI_ERR_NULL;

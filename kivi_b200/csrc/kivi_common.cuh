@@ -117,6 +117,21 @@ __device__ __forceinline__ __half quot_to_half(float a, float s, float r) {
     return __float2half_rn(q);
 }
 
+// The reference's asymmetric quantiser (quant/new_pack.py:238-241) in its fp16 rounding order; every writer of packed codes
+// (public pack, prefill / refill, V-token pack, K flush) calls these two, so their codes and scales agree bit for bit.
+// Group scale: fp16(fp16(mx - mn) / (2^bits - 1)), an IEEE division (a reciprocal multiply would round differently).
+__device__ __forceinline__ __half quant_scale(float mnf, float mxf, int bits) {
+    const __half d = __float2half_rn(mxf - mnf);
+    return __float2half_rn(__fdiv_rn(__half2float(d), (float)((1 << bits) - 1)));
+}
+// Code of x in a group with min mnf and scale scf (rcp = __frcp_rn(scf), maxq = 2^bits - 1):
+// rint(clamp(fp16(fp16(x - mn) / scale), 0, maxq)), round half even; the clamp maps NaN (0 / 0 of a flat group) to 0.
+__device__ __forceinline__ uint32_t quant_code(float x, float mnf, float scf, float rcp, float maxq) {
+    const __half t1 = __float2half_rn(x - mnf);
+    const float t2 = __half2float(quot_to_half(__half2float(t1), scf, rcp));
+    return (uint32_t)__float2int_rn(fminf(fmaxf(t2, 0.f), maxq));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
     #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -73,18 +73,42 @@ __host__ __device__ inline int lay_code_bytes(int bits) { return bits == 2 ? 409
 __host__ __device__ inline int lay_meta_bytes(int g) { return 8 * (128 / g) * 4 * 16; }
 __host__ __device__ inline int lay_block_bytes(int bits, int g) { return lay_code_bytes(bits) + lay_meta_bytes(g); }
 
+// The word index (inside a block) of element (inner i, outer o) is the sum of two independent parts:
+//   lay_word_inner(bits, i): chunk c = i >> 4 and the lane / register bits that i selects (t = (i & 7) >> 1, r >> 1 = bit 3 of i);
+//   lay_word_row(sl, row)  : slab sl = o / slab_rows and row = o % 16 in [0, 16) (g8 = row & 7, r & 1 = row >> 3).
+__host__ __device__ inline int lay_word_inner(int bits, int i) {
+    const int F = 16 / bits, slab_rows = 16 * F, slabs = 128 / slab_rows;
+    return (i >> 4) * slabs * 128 + ((i & 7) >> 1) * 4 + ((i >> 3) & 1) * 2;
+}
+__host__ __device__ inline int lay_word_row(int sl, int row) { return sl * 128 + (row & 7) * 16 + (row >> 3); }
+
 // byte offset (inside a block) of the word holding element (inner i, outer o), and its bit position
 __host__ __device__ inline int lay_word_off(int bits, int i, int o) {
-    const int F = 16 / bits, slab_rows = 16 * F, slabs = 128 / slab_rows;
-    const int c = i >> 4, ii = i & 15;
-    const int p = ((ii & 7) >> 1) + 4 * (ii >> 3);
-    const int sl = o / slab_rows, row = o % 16;
-    const int lane = (row & 7) * 4 + (p & 3), r = (p >> 2) * 2 + (row >> 3);
-    return ((c * slabs + sl) * 128 + lane * 4 + r) * 4;
+    const int F = 16 / bits, slab_rows = 16 * F;
+    return 4 * (lay_word_inner(bits, i) + lay_word_row(o / slab_rows, o % 16));
 }
 __host__ __device__ inline int lay_bit_pos(int bits, int i, int o) {
     const int F = 16 / bits, slab_rows = 16 * F;
     return 16 * (i & 1) + bits * ((o % slab_rows) >> 4);
+}
+
+// The inverse of lay_word_off: word w of a block holds, in its low / high 16 bits, field j of the codes of
+// (inner i0, outer o0 + 16 j) / (inner i0 + 1, outer o0 + 16 j), j = 0 .. F - 1.
+struct WordPos { int i0, o0; };
+__host__ __device__ inline WordPos lay_word_pos(int bits, int w) {
+    const int F = 16 / bits, slab_rows = 16 * F, slabs = 128 / slab_rows;
+    const int c = w / (slabs * 128), sl = (w / 128) % slabs, lw = w % 128;
+    const int lane = lw >> 2, r = lw & 3;
+    return {c * 16 + 2 * (lane & 3) + 8 * (r >> 1), sl * slab_rows + (lane >> 2) + 8 * (r & 1)};
+}
+// word w of a block, assembled from code(inner, outer), the b-bit code of one element
+template <class Code>
+__device__ __forceinline__ uint32_t lay_word(int bits, int w, Code&& code) {
+    const WordPos p = lay_word_pos(bits, w);
+    uint32_t word = 0;
+    for (int par = 0; par < 2; ++par)
+        for (int j = 0; j < 16 / bits; ++j) word |= code(p.i0 + par, p.o0 + 16 * j) << (16 * par + bits * j);
+    return word;
 }
 // element offset (halfs, inside a unit's window) of (slot, channel): 16-byte units swizzled with the slot index
 __host__ __device__ inline int win_off(int slot, int ch) { return slot * kD + ((((ch >> 3) ^ (slot & 7)) << 3) | (ch & 7)); }
@@ -98,6 +122,9 @@ __host__ __device__ inline int lay_zero_off(int bits, int g, int i, int G) {
     return lay_code_bytes(bits) + (((c * (128 / g)) + G) * 4 + t) * 16 + (ii >> 3) * 8 + (ii & 1) * 2;
 }
 __host__ __device__ inline int lay_scale_off(int bits, int g, int i, int G) { return lay_zero_off(bits, g, i, G) + 4; }
+// byte offset of the 8-byte meta half { z[i0], z[i0 + 1], s[i0], s[i0 + 1] } of an inner pair (i0 even): the pair's two zeros
+// and, 4 bytes on, its two scales are adjacent, so one 8-byte store writes all four
+__host__ __device__ inline int lay_meta_pair_off(int bits, int g, int i0, int G) { return lay_zero_off(bits, g, i0, G); }
 
 // ---- PTX helpers -------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -3,20 +3,12 @@
 // Replaces triton_quantize_and_pack_along_last_dim (quant/new_pack.py:217-252): Triton min/max
 // kernel (:158-177) + 6 ATen elementwise kernels (:238-242, incl. an int32 temp 16x the packed
 // size) + zeros + Triton OR-pack kernel (:132-154) become ONE kernel that reads x once
-// (128-bit loads) and writes code/scale/mn once.  Bit-exact against the reference chain:
+// (128-bit loads) and writes code/scale/mn once.  Bit-exact against the reference chain (quant_scale / quant_code):
 //   d = fp16(mx - mn); scale = fp16(d / (2^b - 1)); t1 = fp16(x - mn); t2 = fp16(t1 / scale);
 //   q = int(rint(clamp(t2, 0, 2^b - 1)))   (NaN from 0/0 -> 0, the CUDA cvt result)
 #include "kivi_common.cuh"
 
 namespace kivi {
-
-__device__ __forceinline__ uint32_t quantize_one(float x, float mnf, float scf, float rcp, float maxq) {
-    const __half t1 = __float2half_rn(x - mnf);                                   // :239
-    const __half t2 = quot_to_half(__half2float(t1), scf, rcp);                   // :240 (= fp16 of the IEEE fp32 quotient)
-    float f = __half2float(t2);
-    f = fminf(fmaxf(f, 0.f), maxq);                                               // :241 clamp (NaN -> 0)
-    return (uint32_t)__float2int_rn(f);                                           // round half even
-}
 
 // One thread = one output word (fpi = 32/BITS consecutive elements).  LPG = lanes per group =
 // group_size / fpi, a power of two <= 32, so a group never straddles a warp.
@@ -69,12 +61,11 @@ pack_lastdim_kernel(const __half* __restrict__ x, int64_t n_words, int lpg_log2,
         mxf = fmaxf(mxf, __shfl_xor_sync(0xffffffffu, mxf, o));
     }
     if (!active) return;
-    const __half d = __float2half_rn(mxf - mnf);                                   // :238
-    const __half sc = __float2half_rn(__fdiv_rn(__half2float(d), maxq));           // :238
+    const __half sc = quant_scale(mnf, mxf, BITS);
     const float scf = __half2float(sc), rcp = __frcp_rn(scf);
     uint32_t word = 0;
     #pragma unroll
-    for (int j = 0; j < FPI; ++j) word |= quantize_one(v[j], mnf, scf, rcp, maxq) << (BITS * j);
+    for (int j = 0; j < FPI; ++j) word |= quant_code(v[j], mnf, scf, rcp, maxq) << (BITS * j);
     code[wid] = (int32_t)word;
     if ((wid & ((1 << lpg_log2) - 1)) == 0) {
         const int64_t gid = wid >> lpg_log2;
@@ -106,14 +97,13 @@ pack_lastdim_generic_kernel(const __half* __restrict__ x, int64_t n_words, int g
             float mxf;
             mnf = mxf = __half2float(gp[0]);
             for (int i = 1; i < g; ++i) { const float t = __half2float(gp[i]); mnf = fminf(mnf, t); mxf = fmaxf(mxf, t); }
-            const __half d = __float2half_rn(mxf - mnf);
-            const __half sc = __float2half_rn(__fdiv_rn(__half2float(d), maxq));
+            const __half sc = quant_scale(mnf, mxf, BITS);
             scf = __half2float(sc);
             rcp = __frcp_rn(scf);
             if (e == gid * g) { scale[gid] = sc; mn_out[gid] = __float2half_rn(mnf); }
             last_gid = gid;
         }
-        word |= quantize_one(__half2float(x[e]), mnf, scf, rcp, maxq) << (BITS * j);
+        word |= quant_code(__half2float(x[e]), mnf, scf, rcp, maxq) << (BITS * j);
     }
     code[wid] = (int32_t)word;
 }
