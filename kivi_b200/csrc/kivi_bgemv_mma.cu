@@ -90,6 +90,37 @@ __device__ __forceinline__ float pow2_prescale(float mx) {
     return __uint_as_float((uint32_t)(127 + k) << 23);
 }
 
+// Per-tile window of the split.  The row prescale alone does not bound x*s: a large scale overflows hi = fp16(x*s) (a zero
+// code times inf is then NaN), and the tiles of a long softmax tail, or small scales, put the residual in the fp16
+// denormals.  Each warp therefore checks its tile: the largest product x*s should lie in [2^kSplitMinE, 2^(kSplitMaxE+2))
+// (wide: ex + es in [kSplitMinE, kSplitMaxE] with ex, es = floor(log2) of the largest |x| and largest finite |s| as they
+// enter the split; tall: per-lane fp16 bounds of the products and warp votes).  Inside, the tile keeps the row prescale's
+// arithmetic; outside, the largest finite |s| is brought into [2^9, 2^10) and (tall) max|x| into [16, 32) by exact powers of
+// two, undone in the tile's fp32 fold.  wide keeps the row prescale of x, max|x| < 32 (below 16 only for a row whose max|q|
+// is under 2^-10, which pow2_prescale cannot scale further), so there too every product stays below 2^15; the smaller ones
+// remain exact down to 2^-17 of the largest.  A non-finite scale stays non-finite through any factor, and its outputs are
+// non-finite in the reference as well; it does not set the factor of the tile's finite groups.
+constexpr int kSplitMinE = -4, kSplitMaxE = 13;
+
+__device__ __forceinline__ float pow2f(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
+__device__ __forceinline__ int f32_ilogb(float v) { return (int)((__float_as_uint(v) >> 23) & 0xff) - 127; }
+// floor(log2) of a finite non-zero fp16 from its magnitude bits m (0 < m < 0x7c00)
+__device__ __forceinline__ int h_ilogb(uint32_t m) { return m >= 0x400u ? (int)(m >> 10) - 15 : 31 - __clz(m) - 24; }
+// per-half max of fp16 magnitude bits (NaN > inf > every finite value)
+__device__ __forceinline__ uint32_t hmag_max(uint32_t acc, uint32_t w) { return __vmaxu2(acc, w & 0x7fff7fffu); }
+// the same over the finite values only (inf and NaN count as 0)
+__device__ __forceinline__ uint32_t hfin_max(uint32_t acc, uint32_t w) {
+    const uint32_t m = w & 0x7fff7fffu;
+    return __vmaxu2(acc, m & __vcmpltu2(m, 0x7c007c00u));
+}
+// the warp's max of both halves (one redux.sync)
+__device__ __forceinline__ uint32_t warp_hmag_max(uint32_t v) { return __reduce_max_sync(0xffffffffu, max(v & 0xffffu, v >> 16)); }
+// fp16 pair times a power of two, through fp32 (the factor need not be an fp16)
+__device__ __forceinline__ uint32_t h2_scale(uint32_t w, float f) {
+    const float2 v = __half22float2(u2h(w));
+    return h2u(__floats2half2_rn(v.x * f, v.y * f));
+}
+
 // One chunk of 16 inner indices on the tensor cores.  W[sl][r]: the lane's raw words of inner rows (t, t+4, t+8, t+12)[r],
 // word column 8 sl + g8.
 template <int BITS, int SLABS, bool INIT>
@@ -162,6 +193,9 @@ wide_kernel(const Args a)
     uint2* q2 = reinterpret_cast<uint2*>(smem);                              // [G][8 chunks][4 t] half2 pairs (x[t], x[t+4] | x[t+8], x[t+12])
     float* qlin = reinterpret_cast<float*>(smem + G * 256);                  // [G][128] fp32 (prescaled)
     float* xsc = qlin + G * 128;                                             // [G] 1 / prescale
+    int* xex = reinterpret_cast<int*>(xsc + G);                              // [G] floor(log2) of the prescaled max|x| (or a flag)
+    float* wfac = xsc + 2 * G;                                               // [4] per warp: undoes the tile's scale factor (1 if none)
+    constexpr int kZeroRow = -1000, kNonFinite = 1000;
     uint8_t* stage0 = smem + G * 768 + 64;
 
     const int zdim = a.ratio / G;                                           // head chunks of a unit sit in NEIGHBOURING CTAs: the second reader hits L2
@@ -177,7 +211,10 @@ wide_kernel(const Args a)
         const float ps = pow2_prescale(mx);
         #pragma unroll
         for (int i = 0; i < 4; ++i) qlin[warp * 128 + lane + 32 * i] = xv[i] * ps;
-        if (lane == 0) xsc[warp] = 1.f / ps;
+        if (lane == 0) {
+            xsc[warp] = 1.f / ps;
+            xex[warp] = !(mx < 3.0e38f) ? kNonFinite : mx == 0.f ? kZeroRow : f32_ilogb(mx * ps);
+        }
     }
     __syncthreads();
     if (warp < G) {                                                         // lane = (chunk c, t): rows 16c + t + {0, 4, 8, 12}
@@ -247,6 +284,50 @@ wide_kernel(const Args a)
             const uint8_t* sc = stage0 + st * WG::kStage;
             const __half* ss = reinterpret_cast<const __half*>(sc + WG::kCodeBytes);
             const __half* sz = reinterpret_cast<const __half*>(sc + WG::kCodeBytes + WG::kMetaBytes);
+            // the tile's window (kSplitMinE): the warp's scale columns are its own, so it may rescale them in place
+            {
+                uint8_t* swarp = stage0 + st * WG::kStage + WG::kCodeBytes + warp * NG * 2;
+                uint32_t sm = 0;
+                #pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const uint8_t* p = swarp + (lane + 32 * i) * WG::kMetaRow;
+                    if constexpr (NG == 4) {
+                        const uint2 w = *reinterpret_cast<const uint2*>(p);
+                        sm = hfin_max(hfin_max(sm, w.x), w.y);
+                    } else {
+                        sm = hfin_max(sm, *reinterpret_cast<const uint32_t*>(p));
+                    }
+                }
+                const uint32_t msb = warp_hmag_max(sm);                     // largest finite |s| of the tile
+                bool trig = false;
+                float rf = 1.f;
+                if (msb != 0) {
+                    const int es = h_ilogb(msb);
+                    #pragma unroll
+                    for (int h = 0; h < G; ++h) {                           // (a head with a non-finite q is non-finite anyway)
+                        const int ex = xex[h];
+                        if (ex != kZeroRow && ex != kNonFinite) trig |= ex + es > kSplitMaxE || ex + es < kSplitMinE;
+                    }
+                    if (trig) {
+                        const int ks = kSplitMaxE - 4 - es;                 // max finite |s| into [2^9, 2^10): below 2^15 / 32
+                        const float fs = pow2f(ks);
+                        #pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            uint8_t* p = swarp + (lane + 32 * i) * WG::kMetaRow;
+                            if constexpr (NG == 4) {
+                                uint2 w = *reinterpret_cast<const uint2*>(p);
+                                w.x = h2_scale(w.x, fs); w.y = h2_scale(w.y, fs);
+                                *reinterpret_cast<uint2*>(p) = w;
+                            } else {
+                                *reinterpret_cast<uint32_t*>(p) = h2_scale(*reinterpret_cast<const uint32_t*>(p), fs);
+                            }
+                        }
+                        rf = pow2f(-ks);
+                        __syncwarp();
+                    }
+                }
+                if (lane == 0) wfac[warp] = rf;                             // read back in the epilogue: one register less in the MMAs
+            }
             float acc[8][4];
             #pragma unroll
             for (int c = 0; c < 8; ++c) {
@@ -283,6 +364,8 @@ wide_kernel(const Args a)
             zt += __shfl_xor_sync(0xffffffffu, zt, 16);
             // ---- epilogue: the lane owns, per slab, the 2F tokens of word column 8 sl + g8 if their group is its pair's group
             const float rs = xsc[h_c];
+            __syncwarp();
+            const float rfac = wfac[warp];
             #pragma unroll
             for (int sl = 0; sl < SLABS; ++sl) {
                 const int o0 = (sl * 8 + g8) * 2 * F;                       // first of 2F consecutive tokens (within the warp's 128)
@@ -292,7 +375,7 @@ wide_kernel(const Args a)
                         __align__(16) __half o[2 * F];
                         #pragma unroll
                         for (int j = 0; j < F; ++j) {
-                            const float sc_j = inv_pos<BITS>(j);
+                            const float sc_j = inv_pos<BITS>(j) * rfac;
                             o[j] = __float2half_rn(fmaf(acc[sl * F + j][0] + acc[sl * F + j][1], sc_j, zt) * rs);
                             o[F + j] = __float2half_rn(fmaf(acc[sl * F + j][2] + acc[sl * F + j][3], sc_j, zt) * rs);
                         }
@@ -423,7 +506,81 @@ tall_kernel(const Args a)
         const uint8_t* sc = wbase + st * GE::kStage;
         const __half* ss = reinterpret_cast<const __half*>(sc + GE::kCodeBytes);
         const __half* sz = reinterpret_cast<const __half*>(sc + GE::kCodeBytes + GE::kMetaBytes);
-        const __half* xb = xbuf + st * G * 128;
+        __half* xb = xbuf + st * G * 128;
+
+        // the tile's window (kSplitMinE).  Each lane bounds the products x*s of the rows whose scales it reads by max|x| times
+        // max s, in fp16 (inf where hi could overflow; raw bits, so a negative or non-finite scale also reads as >= 0x7c00).
+        // Warp votes decide: any lane's bound overflows, or, for one head, every lane's bound is below 2^kSplitMinE.  A tile
+        // outside the window (rare) gets x (per head) and s rescaled in place -- the stage is the warp's own -- from its exact
+        // maxima (of the finite scales), and its fp32 fold and zero term take the exact inverse.
+        uint4* sv = reinterpret_cast<uint4*>(wbase + st * GE::kStage + GE::kCodeBytes);
+        bool trig;
+        {
+            uint32_t sm = 0;
+            #pragma unroll
+            for (int i = 0; i < GE::kMetaBytes / 512; ++i) {
+                const uint4 w = sv[i * 32 + lane];
+                sm = __vmaxu2(sm, __vmaxu2(__vmaxu2(w.x, w.y), __vmaxu2(w.z, w.w)));
+            }
+            sm = max(sm & 0xffffu, sm >> 16) * 0x10001u;
+            uint32_t xq[G];
+            #pragma unroll
+            for (int h = 0; h < G; ++h) {                                   // x of the same rows: 8 / NG rows per 16-byte scale unit
+                uint32_t m;
+                if constexpr (NG == 4) {
+                    const uint32_t* x2 = reinterpret_cast<const uint32_t*>(xb + h * 128);
+                    m = __vmaxu2(x2[lane] & 0x7fff7fffu, x2[32 + lane] & 0x7fff7fffu);
+                } else {
+                    const uint2 x4 = reinterpret_cast<const uint2*>(xb + h * 128)[lane];
+                    m = __vmaxu2(x4.x & 0x7fff7fffu, x4.y & 0x7fff7fffu);
+                }
+                xq[h] = max(m & 0xffffu, m >> 16);
+            }
+            const uint32_t q = h2u(__hmul2(u2h(xq[0] | (xq[G - 1] << 16)), u2h(sm)));
+            const bool big = __vcmpgeu2(q, 0x7c007c00u) != 0;                // 2^(kSplitMaxE + 2) is past fp16's range
+            const uint32_t small = __vcmpltu2(q, 0x2c002c00u);              // per head: below 2^kSplitMinE
+            trig = __any_sync(0xffffffffu, big);
+            if constexpr (G == 1) trig = trig || __all_sync(0xffffffffu, small != 0);
+            else trig = trig || __all_sync(0xffffffffu, (small & 0xffffu) != 0) || __all_sync(0xffffffffu, (small >> 16) != 0);
+        }
+        float rf = 1.f, zf = 1.f;                                           // bring the lane's head's partials back to the row prescale
+        if (trig) {                                                         // warp-uniform
+            uint32_t sm = 0;
+            #pragma unroll
+            for (int i = 0; i < GE::kMetaBytes / 512; ++i) {
+                const uint4 w = sv[i * 32 + lane];
+                sm = hfin_max(hfin_max(hfin_max(hfin_max(sm, w.x), w.y), w.z), w.w);
+            }
+            const uint32_t msb = warp_hmag_max(sm);                         // largest finite |s| of the tile
+            const int ks = msb == 0 ? 0 : kSplitMaxE - 4 - h_ilogb(msb);    // into [2^9, 2^10)
+            const float fs = pow2f(ks);
+            #pragma unroll
+            for (int i = 0; i < GE::kMetaBytes / 512; ++i) {
+                uint4 w = sv[i * 32 + lane];
+                w.x = h2_scale(w.x, fs); w.y = h2_scale(w.y, fs); w.z = h2_scale(w.z, fs); w.w = h2_scale(w.w, fs);
+                sv[i * 32 + lane] = w;
+            }
+            #pragma unroll
+            for (int h = 0; h < G; ++h) {
+                float x[4];
+                uint32_t m = 0;
+                #pragma unroll
+                for (int i = 0; i < 4; ++i) {                               // the unscaled x again (the row prescale may have lost bits)
+                    const int k = tile * 128 + lane + 32 * i;
+                    const __half xh = k < a.K ? __ldg(arow + h * a.a_stride + k) : __float2half_rn(0.f);
+                    m = max(m, (uint32_t)__half_as_ushort(xh) & 0x7fffu);
+                    x[i] = __half2float(xh);
+                }
+                m = min(__reduce_max_sync(0xffffffffu, m), 0x7bffu);
+                const int eps = f32_ilogb(xsc[h]);                          // log2 of the row prescale
+                const int ecx = m != 0 ? 4 - h_ilogb(m) : eps;              // max|x| into [16, 32)
+                const float cx = pow2f(ecx);
+                #pragma unroll
+                for (int i = 0; i < 4; ++i) xb[h * 128 + lane + 32 * i] = __float2half_rn(x[i] * cx);
+                if (h == h_c) { rf = pow2f(eps - ecx - ks); zf = pow2f(eps - ecx); }
+            }
+            __syncwarp();
+        }
 
         float acc[8][4];
         #pragma unroll
@@ -444,21 +601,35 @@ tall_kernel(const Args a)
             else chunk_mma<BITS, SLABS, false>(W, b0, b1, acc);
         }
         if (t4 < NP) {
-            #pragma unroll 4
-            for (int i = 0; i < 16; ++i) {
-                const int d = g8 * 16 + i;
-                zrun = fmaf(__half2float(xb[h_c * 128 + d]), __half2float(sz[d * NG + gam_c]), zrun);
+            if (trig) {
+                float zt = 0.f;
+                #pragma unroll 4
+                for (int i = 0; i < 16; ++i) {
+                    const int d = g8 * 16 + i;
+                    zt = fmaf(__half2float(xb[h_c * 128 + d]), __half2float(sz[d * NG + gam_c]), zt);
+                }
+                zrun = fmaf(zt, zf, zrun);
+            } else {
+                #pragma unroll 4
+                for (int i = 0; i < 16; ++i) {
+                    const int d = g8 * 16 + i;
+                    zrun = fmaf(__half2float(xb[h_c * 128 + d]), __half2float(sz[d * NG + gam_c]), zrun);
+                }
             }
         }
         // accumulator chains live for ONE tile (mma.sync accumulates with truncation); round-to-nearest adds across tiles
-        #pragma unroll
-        for (int sl = 0; sl < SLABS; ++sl)
+        auto fold = [&](float f) {
             #pragma unroll
-            for (int j = 0; j < F; ++j) {
-                const float sc_j = inv_pos<BITS>(j);
-                run[sl][j] = fmaf(acc[sl * F + j][0] + acc[sl * F + j][1], sc_j, run[sl][j]);
-                run[sl][F + j] = fmaf(acc[sl * F + j][2] + acc[sl * F + j][3], sc_j, run[sl][F + j]);
-            }
+            for (int sl = 0; sl < SLABS; ++sl)
+                #pragma unroll
+                for (int j = 0; j < F; ++j) {
+                    const float sc_j = inv_pos<BITS>(j) * f;
+                    run[sl][j] = fmaf(acc[sl * F + j][0] + acc[sl * F + j][1], sc_j, run[sl][j]);
+                    run[sl][F + j] = fmaf(acc[sl * F + j][2] + acc[sl * F + j][3], sc_j, run[sl][F + j]);
+                }
+        };
+        if (trig) fold(rf);
+        else fold(1.f);                                                     // (constant factor: the fold as it always was)
         __syncwarp();
     }
     // ---- reduce, in a fixed order (deterministic): lanes -> the warp's partial (its own stage memory, every output written
