@@ -303,10 +303,14 @@ int kivi_cache_import_f16(const kivi_cache_t* cache, int tk, int r, int tv, int 
  * Glue kernels of the decode step around the hot path (not part of the KIVI operators; they
  * replace ~16 ATen elementwise launches per layer per step in kivi_b200/llama_kivi.py).  fp16 I/O,
  * arithmetic of the HF Llama modules the reference forks: every fp16 op rounds to fp16.
- *   kivi_add_rmsnorm_f16 : residual += x (x may be NULL); out = weight * fp16(residual * rsqrt(mean(residual^2)+eps))
+ *   kivi_add_rmsnorm_f16 : residual += x (x may be NULL); out = weight * fp16(residual * rsqrt(mean(residual^2)+eps));
+ *                          rows >= 0, hidden % 8 == 0, hidden <= 16384; x, residual, weight and out 16-byte aligned
  *   kivi_rope_split_f16  : qkv [B,(H+2Hkv)*128] -> q [B,H,128], k [B,Hkv,128] (rotary at position pos[b], int64,
- *                          clamped to the table_rows rows of the cos / sin tables [table_rows, 128]), v
- *   kivi_silu_mul_f16    : gate_up [rows, 2*I] -> out [rows, I] = fp16(silu(gate)) * up
+ *                          clamped to the table_rows rows of the cos / sin tables [table_rows, 128]), v;
+ *                          1 <= B <= 65535, table_rows >= 1
+ *   kivi_silu_mul_f16    : gate_up [rows, 2*I] -> out [rows, I] = fp16(silu(gate)) * up;
+ *                          1 <= rows <= 65535, I even; gate_up and out 4-byte aligned
+ * Misaligned pointers return KIVI_ERR_ALIGN before any launch.
  * ------------------------------------------------------------------------------------------ */
 int kivi_add_rmsnorm_f16(const void* x, void* residual, const void* weight, void* out,
                          int rows, int hidden, float eps, void* stream);

@@ -174,6 +174,8 @@ greedy_exchange_kernel(const float* __restrict__ logits, int V, long long* __res
 
 using namespace kivi;
 
+static bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
+
 extern "C" int kivi_greedy_sample_exchange_f32(const void* logits, int batch, int vocab, void* next_local, void* ids_feedback,
                                                const void* peer_buffers, int rank, int world, const void* step, void* err,
                                                void* stream)
@@ -192,6 +194,9 @@ extern "C" int kivi_add_rmsnorm_f16(const void* x, void* residual, const void* w
 {
     if (!residual || !weight || !out) return KIVI_ERR_NULL;
     if (rows < 0 || hidden <= 0 || hidden % 8 != 0 || hidden > 16384) return KIVI_ERR_SHAPE;
+    // the kernel moves 8 halves per uint4 access: a view that starts off a 16-byte boundary would fault
+    if ((x && !aligned_to(x, 16)) || !aligned_to(residual, 16) || !aligned_to(weight, 16) || !aligned_to(out, 16))
+        return KIVI_ERR_ALIGN;
     if (rows == 0) return KIVI_OK;
     cudaStream_t st = (cudaStream_t)stream;
     if (x) add_rmsnorm_kernel<true><<<rows, 512, 0, st>>>((const __half*)x, (__half*)residual,
@@ -217,6 +222,7 @@ extern "C" int kivi_silu_mul_f16(const void* gate_up, void* out, int rows, int i
 {
     if (!gate_up || !out) return KIVI_ERR_NULL;
     if (rows <= 0 || intermediate <= 0 || intermediate % 2 != 0 || rows > 65535) return KIVI_ERR_SHAPE;
+    if (!aligned_to(gate_up, 4) || !aligned_to(out, 4)) return KIVI_ERR_ALIGN;      // half2 accesses
     silu_mul_kernel<<<dim3(cdiv(intermediate / 2, 256), rows), 256, 0, (cudaStream_t)stream>>>(
         (const __half*)gate_up, (__half*)out, intermediate);
     return post_launch();

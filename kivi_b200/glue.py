@@ -1,5 +1,6 @@
 """ctypes wrappers of the decode-step glue kernels (csrc/kivi_model.cu): residual-add + RMSNorm,
-RoPE + q/k/v split, SiLU*mul.  fp16 CUDA tensors only."""
+RoPE + q/k/v split, SiLU*mul.  fp16 CUDA tensors only; each wrapper checks device, dtype, contiguity and shapes
+before the call (ValueError, or RuntimeError for a CPU tensor)."""
 from __future__ import annotations
 
 import ctypes
@@ -23,10 +24,28 @@ def _bind():
     _B = True
 
 
+def _check(name, t, dtype, shape):
+    """t is a contiguous CUDA tensor of `dtype` and `shape`; a kernel would otherwise read or write the wrong bytes."""
+    _lib.require_cuda(t)
+    if t.dtype != dtype:
+        raise ValueError(f"{name}: expected {dtype}, got {t.dtype}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name}: expected a contiguous tensor")
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
+
+
 def add_rmsnorm(x, residual, weight, out, eps: float):
     """residual += x (x may be None); out = weight * fp16(residual * rsqrt(mean(residual^2) + eps))."""
     _bind()
+    if residual.dim() != 2:
+        raise ValueError(f"residual: expected [rows, hidden], got shape {tuple(residual.shape)}")
     rows, hidden = residual.shape
+    f16 = torch.float16
+    for name, t, shape in (("residual", residual, (rows, hidden)), ("weight", weight, (hidden,)), ("out", out, (rows, hidden)),
+                           ("x", x, (rows, hidden))):
+        if t is not None:
+            _check(name, t, f16, shape)
     _lib.check(_lib.lib().kivi_add_rmsnorm_f16(x.data_ptr() if x is not None else None, residual.data_ptr(),
                                                weight.data_ptr(), out.data_ptr(), rows, hidden, eps,
                                                _lib.stream_ptr(residual.device)), "kivi_add_rmsnorm_f16")
@@ -36,7 +55,21 @@ def add_rmsnorm(x, residual, weight, out, eps: float):
 def rope_split(qkv, cos_table, sin_table, pos, q, k, v):
     """qkv [B,(H+2Hkv)*128] -> q [B,H,128], k [B,Hkv,128] rotated at position pos[b] (int64), v [B,Hkv,128]."""
     _bind()
+    if q.dim() != 3 or k.dim() != 3:
+        raise ValueError(f"q, k: expected [B, heads, 128], got shapes {tuple(q.shape)}, {tuple(k.shape)}")
     B, H, Hkv = q.shape[0], q.shape[1], k.shape[1]
+    f16 = torch.float16
+    _check("qkv", qkv, f16, (B, (H + 2 * Hkv) * 128))
+    _check("q", q, f16, (B, H, 128))
+    _check("k", k, f16, (B, Hkv, 128))
+    _check("v", v, f16, (B, Hkv, 128))
+    if cos_table.dim() != 2 or cos_table.shape[1] != 128:              # the kernel's rows are 128 wide (head_dim 128)
+        raise ValueError(f"cos_table: expected [rows, 128], got shape {tuple(cos_table.shape)}")
+    _check("cos_table", cos_table, f16, cos_table.shape)
+    _check("sin_table", sin_table, f16, cos_table.shape)
+    _lib.require_cuda(pos)
+    if pos.dtype != torch.int64 or pos.numel() != B or not pos.is_contiguous():
+        raise ValueError(f"pos: expected {B} contiguous int64 positions, got {pos.dtype} of shape {tuple(pos.shape)}")
     _lib.check(_lib.lib().kivi_rope_split_f16(qkv.data_ptr(), cos_table.data_ptr(), sin_table.data_ptr(), pos.data_ptr(),
                                               q.data_ptr(), k.data_ptr(), v.data_ptr(), B, H, Hkv, cos_table.shape[0],
                                               _lib.stream_ptr(qkv.device)), "kivi_rope_split_f16")
@@ -44,7 +77,11 @@ def rope_split(qkv, cos_table, sin_table, pos, q, k, v):
 
 def silu_mul(gate_up, out):
     _bind()
+    if out.dim() != 2:
+        raise ValueError(f"out: expected [rows, I], got shape {tuple(out.shape)}")
     rows, inter = out.shape
+    _check("out", out, torch.float16, (rows, inter))
+    _check("gate_up", gate_up, torch.float16, (rows, 2 * inter))
     _lib.check(_lib.lib().kivi_silu_mul_f16(gate_up.data_ptr(), out.data_ptr(), rows, inter,
                                             _lib.stream_ptr(out.device)), "kivi_silu_mul_f16")
     return out

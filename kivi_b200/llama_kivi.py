@@ -146,7 +146,12 @@ class LlamaRMSNorm(nn.Module):
         self.variance_epsilon = eps
 
     def forward(self, x):
-        return F.rms_norm(x, (x.shape[-1],), self.weight, self.variance_epsilon)
+        # HF LlamaRMSNorm: fp32 statistics, the normalised value rounded to x's dtype, THEN the weight product (rounded
+        # again).  F.rms_norm multiplies by the weight in fp32 and rounds once, which differs in ~1/4 of fp16 outputs;
+        # the decode step's add_rmsnorm kernel rounds like this chain.
+        h = x.float()
+        h = h * torch.rsqrt(h.pow(2).mean(-1, keepdim=True) + self.variance_epsilon)
+        return self.weight * h.to(x.dtype)
 
 
 def _rope_tables(head_dim, max_pos, theta, device):
