@@ -331,6 +331,39 @@ int kivi_silu_mul_f16(const void* gate_up, void* out, int rows, int intermediate
 int kivi_greedy_sample_exchange_f32(const void* logits, int batch, int vocab, void* next_local, void* ids_feedback,
                                     const void* peer_buffers, int rank, int world, const void* step, void* err, void* stream);
 
+/* Tensor-parallel residual-add + RMSNorm: the all-reduce after o_proj / down_proj fused into the norm that follows it.
+ * With the rows of the attention heads and of the MLP columns sharded over `world` ranks, rank p holds a partial sum
+ * partial_p [rows, hidden] fp16 of the projection.  Every rank computes the same bits:
+ *     x = fp16( sum_{p = 0 .. world-1} fp32(partial_p) )      (fp32 additions in rank order, starting from partial_0)
+ *     residual += x;  out = weight * fp16(residual * rsqrt(mean(residual^2) + eps))
+ * i.e. exactly kivi_add_rmsnorm_f16(x, residual, weight, out).
+ *
+ * peer_buffers: NULL (world must be 1: x is the whole sum and the call IS kivi_add_rmsnorm_f16), or a DEVICE array of
+ * `world` pointers, entry p = rank p's buffer -- one symmetric allocation per rank (peer-mapped over NVLink / NVSwitch),
+ * zero-initialised, 16-byte aligned:
+ *     half     partial[2][rows_max][hidden]    this rank's partial sums, double-buffered: call c uses slot c & 1
+ *     uint64   arrived[world]                  arrived[q] = the last call number rank q has announced here
+ * The caller writes its partial of call c into slot (c & 1) of ITS OWN buffer (the projection GEMM's output) before the call;
+ * x is ignored.  The call number is e = *epoch + call + 1 (epoch: device int64; call: the index of this call within a
+ * replay).  The kernel
+ *   1. stores e into arrived[rank] of every peer (red.release.sys max, so pre-set counters are harmless),
+ *   2. waits (ld.acquire.sys) until arrived[q] >= e for every q in its own buffer -- bounded: after ~ a second *err = 1 and it goes on
+ *      instead of hanging the GPU (the host raises),
+ *   3. reads slot (c & 1) of every peer's buffer and reduces.
+ * The caller advances *epoch by the number of calls per replay, which must be even (two per layer), once per replay and
+ * inside the same CUDA graph; consecutive calls then alternate slots across replays too.
+ * Why two slots are enough: a peer reads rank r's slot (c & 1) during call c.  Rank r overwrites that slot next for call c+2,
+ * with the GEMM that precedes call c+2 on its stream, i.e. after its call c+1 has returned -- and call c+1 returns only after
+ * every peer has arrived at c+1, which each peer does at the start of its call c+1, after its call c (and all of its reads
+ * of slot c & 1) has completed on its stream.  So no slot is written while a peer may still read it.
+ * A row is split over a cluster of `cluster` CTAs (1, 2, 4 or 8; 0 = the default, one CTA per row) whose reductions are
+ * arranged to give the same bits for every width.
+ * Requirements: rows >= 0, rows <= rows_max, hidden % 8 == 0, hidden <= 16384, 1 <= world <= 8, 0 <= rank < world,
+ * residual / weight / out 16-byte aligned; argument errors return KIVI_ERR_* before any launch.  Graph-capturable. */
+int kivi_allreduce_add_rmsnorm_f16(const void* x, void* residual, const void* weight, void* out, int rows, int hidden,
+                                   float eps, const void* peer_buffers, int rank, int world, int rows_max, int call,
+                                   const void* epoch, void* err, int cluster, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

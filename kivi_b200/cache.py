@@ -90,6 +90,7 @@ class KiviCache:
         self.n_layers, self.batch, self.num_heads, self.num_kv_heads = n_layers, batch, num_heads, num_kv_heads
         self.head_dim, self.k_bits, self.v_bits = head_dim, k_bits, v_bits
         self.group_size, self.residual_length, self.max_tokens = group_size, residual_length, max_tokens
+        self.tensor_parallel = False      # set by a tensor-parallel model: the heads are one rank's share of the model's heads
         sizes = (ctypes.c_int64 * 8)()
         _lib.check(_lib.lib().kivi_cache_sizes(batch, num_kv_heads, k_bits, v_bits, group_size, residual_length,
                                                max_tokens, sizes), "kivi_cache_sizes")
@@ -300,11 +301,17 @@ class KiviCache:
                                f"lengths {st[:6]} exceed the capacity the cache was created with")
         return st
 
+    def _whole_model_only(self, what: str):
+        if self.tensor_parallel:
+            raise NotImplementedError(f"KiviCache.{what}: the reference's 9-tuples hold every head of a layer; this cache "
+                                      "holds one tensor-parallel rank's heads")
+
     def import_tuple(self, layer: int, past, kv_start=None):
         """Load `layer` from the reference's per-layer 9-tuple (models/llama_kivi.py:454-455), the inverse of
         export(): a cache that was built by the reference's own hook (or by kivi_prefill_tuple /
         kivi_decode_attention_tuple) continues on the fused path.  All layers of a model share one `state`, so every
         layer must be imported from tuples of the same lengths.  kv_start: see set_kv_start."""
+        self._whole_model_only("import_tuple")
         kc, kfull, ks, km, vc, vfull, vs, vm, seen = past
         B, Hkv, D, g = self.batch, self.num_kv_heads, self.head_dim, self.group_size
         kf, vf = 32 // self.k_bits, 32 // self.v_bits
@@ -341,6 +348,7 @@ class KiviCache:
         """The reference's per-layer 9-tuple (models/llama_kivi.py:454-455):
         (Kq_code [B,Hkv,128,tk/fpi] | None, K_full [B,Hkv,r,128] | None, K_scale, K_mn,
          Vq_code [B,Hkv,tv,128/fpi] | None, V_full [B,Hkv,L,128], V_scale, V_mn, kv_seq_len)"""
+        self._whole_model_only("export")
         B, Hkv, D, g = self.batch, self.num_kv_heads, self.head_dim, self.group_size
         dev = self.device
         kf, vf = 32 // self.k_bits, 32 // self.v_bits

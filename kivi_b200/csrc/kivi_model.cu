@@ -4,6 +4,10 @@
 // (models/llama_kivi.py star-imports transformers.models.llama): every fp16 op rounds to fp16.
 #include "kivi_common.cuh"
 
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
+
 namespace kivi {
 
 // residual (fp16, in/out) += x;  out = weight * fp16( residual * rsqrt(mean(residual^2) + eps) )
@@ -170,11 +174,189 @@ greedy_exchange_kernel(const float* __restrict__ logits, int V, long long* __res
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Tensor-parallel residual-add + RMSNorm: the all-reduce of the o_proj / down_proj partial sums fused into the norm that
+// consumes them.  Every rank reads the `world` partials of this call straight from the peers' symmetric buffers (layout in
+// include/kivi_b200.h), sums them in fp32 in rank order, rounds to fp16 and continues exactly like add_rmsnorm_kernel<true>.
+//
+// A row is split over a cluster of C CTAs of 512 / C threads.  CTA c of the cluster plays threads [c * 512 / C, (c+1) * 512 / C)
+// of the one-CTA kernel: the same elements per thread, the same per-thread / per-warp partial sums of squares, and the 16
+// warp sums are added in the same order after a DSMEM gather -- so every C gives the bits of add_rmsnorm_kernel, and C only
+// decides how many SMs issue the N * hidden * 2 bytes of peer loads of a row.
+// ------------------------------------------------------------------------------------------------
+template <int C>
+__global__ void __launch_bounds__(512 / C, 1)
+allreduce_add_rmsnorm_kernel(const __half* const* __restrict__ peer, __half* __restrict__ residual, const __half* __restrict__ w,
+                             __half* __restrict__ out, int hidden, float eps, int rank, int world, long long slot_off,
+                             long long counters_off, const long long* __restrict__ epoch_ptr, int call, int* __restrict__ err)
+{
+    constexpr int kThreads = 512 / C, kWarps = kThreads / 32, kMaxIter = 4;
+    __shared__ float red[kWarps];
+    const int row = blockIdx.x / C, crank = blockIdx.x % C;
+    const int vt = crank * kThreads + threadIdx.x;                       // the thread of the one-CTA kernel this one plays
+    const unsigned long long epoch = (unsigned long long)(*epoch_ptr + call + 1);
+    if (blockIdx.x == 0 && threadIdx.x < world) {                        // this rank's partial of the call is written: arrive
+        unsigned long long* a = reinterpret_cast<unsigned long long*>(
+            reinterpret_cast<char*>(const_cast<__half*>(peer[threadIdx.x])) + counters_off) + rank;
+        asm volatile("red.release.sys.global.max.u64 [%0], %1;" :: "l"(a), "l"(epoch) : "memory");
+    }
+    if (threadIdx.x < world) {                                           // every rank's partial of the call is written
+        const unsigned long long* cnt = reinterpret_cast<const unsigned long long*>(
+            reinterpret_cast<const char*>(peer[rank]) + counters_off) + threadIdx.x;
+        long long spins = 0;
+        unsigned long long seen;
+        for (;;) {
+            asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(seen) : "l"(cnt) : "memory");
+            if (seen >= epoch) break;
+            if (++spins > (1ll << 24)) { *err = 1; break; }              // ~ a second: a peer is gone; report instead of hanging
+            __nanosleep(64);
+        }
+    }
+    __syncthreads();                                                     // the acquires above order every thread's reads below
+
+    const int nvec = hidden / 8;
+    const long long row_off = slot_off / 2 + (long long)row * hidden;    // in halves, from the start of a rank's buffer
+    __half* r = residual + (int64_t)row * hidden;
+    uint4 v[kMaxIter];
+    float ss = 0.f;
+    #pragma unroll
+    for (int it = 0; it < kMaxIter; ++it) {
+        const int i = vt + it * 512;
+        if (i < nvec) {
+            uint4 pv[8];                                                 // all peer loads in flight before the first add
+            #pragma unroll
+            for (int p = 0; p < 8; ++p)
+                if (p < world) pv[p] = __ldcg(reinterpret_cast<const uint4*>(peer[p] + row_off) + i);
+            float2 acc[4];
+            #pragma unroll
+            for (int e = 0; e < 4; ++e) acc[e] = __half22float2(reinterpret_cast<const __half2*>(&pv[0])[e]);
+            #pragma unroll
+            for (int p = 1; p < 8; ++p) {
+                if (p < world) {
+                    const __half2* ph = reinterpret_cast<const __half2*>(&pv[p]);
+                    #pragma unroll
+                    for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(ph[e]); acc[e].x += f.x; acc[e].y += f.y; }
+                }
+            }
+            uint4 u = *reinterpret_cast<const uint4*>(r + i * 8);
+            __half2* h = reinterpret_cast<__half2*>(&u);
+            #pragma unroll
+            for (int e = 0; e < 4; ++e) h[e] = __hadd2_rn(h[e], __floats2half2_rn(acc[e].x, acc[e].y));
+            *reinterpret_cast<uint4*>(r + i * 8) = u;
+            #pragma unroll
+            for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(h[e]); ss = fmaf(f.x, f.x, fmaf(f.y, f.y, ss)); }
+            v[it] = u;
+        }
+    }
+    ss = warp_sum(ss);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
+    float tot = 0.f;
+    if constexpr (C == 1) {
+        __syncthreads();
+        #pragma unroll
+        for (int i = 0; i < 16; ++i) tot += red[i];
+    } else {
+        cg::cluster_group cluster = cg::this_cluster();
+        cluster.sync();
+        #pragma unroll
+        for (int c = 0; c < C; ++c) {
+            const float* rr = cluster.map_shared_rank(red, c);
+            #pragma unroll
+            for (int i = 0; i < kWarps; ++i) tot += rr[i];
+        }
+        cluster.sync();                                                  // no CTA leaves while a peer CTA reads its red[]
+    }
+    const float rs = rsqrtf(tot / (float)hidden + eps);
+    #pragma unroll
+    for (int it = 0; it < kMaxIter; ++it) {
+        const int i = vt + it * 512;
+        if (i < nvec) {
+            const __half2* h = reinterpret_cast<const __half2*>(&v[it]);
+            const uint4 wv = __ldg(reinterpret_cast<const uint4*>(w) + i);
+            const __half2* wh = reinterpret_cast<const __half2*>(&wv);
+            uint4 o;
+            __half2* oh = reinterpret_cast<__half2*>(&o);
+            #pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(h[e]);
+                oh[e] = __hmul2_rn(wh[e], __floats2half2_rn(f.x * rs, f.y * rs));
+            }
+            *reinterpret_cast<uint4*>(out + (int64_t)row * hidden + i * 8) = o;
+        }
+    }
+}
+
 }  // namespace kivi
 
 using namespace kivi;
 
 static bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
+
+template <int C>
+static cudaError_t launch_allreduce_add_rmsnorm(int rows, cudaStream_t st, const __half* const* peer, __half* residual,
+                                                const __half* w, __half* out, int hidden, float eps, int rank, int world,
+                                                long long slot_off, long long counters_off, const long long* epoch, int call,
+                                                int* err)
+{
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(rows * C);
+    cfg.blockDim = dim3(512 / C);
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = C > 1 ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, allreduce_add_rmsnorm_kernel<C>, peer, residual, w, out, hidden, eps, rank, world,
+                              slot_off, counters_off, epoch, call, err);
+}
+
+
+extern "C" int kivi_allreduce_add_rmsnorm_f16(const void* x, void* residual, const void* weight, void* out,
+                                              int rows, int hidden, float eps,
+                                              const void* peer_buffers, int rank, int world, int rows_max, int call,
+                                              const void* epoch, void* err, int cluster, void* stream)
+{
+    if (!residual || !weight || !out) return KIVI_ERR_NULL;
+    if (rows < 0 || hidden <= 0 || hidden % 8 != 0 || hidden > 16384) return KIVI_ERR_SHAPE;
+    if (world < 1 || world > 8 || rank < 0 || rank >= world) return KIVI_ERR_SHAPE;
+    if (!peer_buffers) {                                                 // one rank: x is the whole sum
+        if (world != 1) return KIVI_ERR_NULL;
+        return kivi_add_rmsnorm_f16(x, residual, weight, out, rows, hidden, eps, stream);
+    }
+    if (!epoch || !err) return KIVI_ERR_NULL;
+    if (rows > rows_max || call < 0) return KIVI_ERR_SHAPE;
+    if (cluster != 0 && cluster != 1 && cluster != 2 && cluster != 4 && cluster != 8) return KIVI_ERR_SHAPE;
+    if (!aligned_to(residual, 16) || !aligned_to(weight, 16) || !aligned_to(out, 16) || !aligned_to(epoch, 8))
+        return KIVI_ERR_ALIGN;
+    if (rows == 0) return KIVI_OK;
+    const long long slot_bytes = (long long)rows_max * hidden * 2;
+    const long long slot_off = (long long)(call & 1) * slot_bytes, counters_off = 2 * slot_bytes;
+    // cluster == 0: one CTA per row, the fastest width at every rows / hidden / world measured (tools/tp_bench.py kernel,
+    // ranks emulated in one GPU's memory; over NVLink the widths have not been compared)
+    const int C = cluster ? cluster : 1;
+    cudaStream_t st = (cudaStream_t)stream;
+    auto peer = (const __half* const*)peer_buffers;
+    cudaError_t e;
+    switch (C) {
+        case 1: e = launch_allreduce_add_rmsnorm<1>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
+                                                    hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
+                                                    call, (int*)err); break;
+        case 2: e = launch_allreduce_add_rmsnorm<2>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
+                                                    hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
+                                                    call, (int*)err); break;
+        case 4: e = launch_allreduce_add_rmsnorm<4>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
+                                                    hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
+                                                    call, (int*)err); break;
+        default: e = launch_allreduce_add_rmsnorm<8>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
+                                                     hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
+                                                     call, (int*)err); break;
+    }
+    if (e != cudaSuccess) return (int)e;
+    return post_launch();
+}
 
 extern "C" int kivi_greedy_sample_exchange_f32(const void* logits, int batch, int vocab, void* next_local, void* ids_feedback,
                                                const void* peer_buffers, int rank, int world, const void* step, void* err,

@@ -5,6 +5,7 @@ contiguous ranges, each rank runs the whole model on its shard with NO per-layer
 only exchange is one all-gather of the final logits [B/N, vocab] at the sampling step (NCCL over
 NVLink 5 / NVSwitch on GPUs, gloo on CPU for the tests), followed by identical sampling on every rank.
 The reference has nothing here (device_map="auto" layer placement only).
+Tensor parallelism (kivi_b200.tp) adds one collective per sharded projection: `PeerAllReduce` below.
 """
 from __future__ import annotations
 
@@ -114,6 +115,47 @@ class PeerTokenExchange:
             raise RuntimeError("kivi_b200: the peer token exchange timed out waiting for another rank")
         par = int(self.step.item()) & 1
         return self.buf[par * self.world * self.batch: (par + 1) * self.world * self.batch]
+
+
+class PeerAllReduce:
+    """The per-layer all-reduce of tensor-parallel decoding (kivi_allreduce_add_rmsnorm_f16) WITHOUT a library collective:
+    every rank owns one symmetric buffer that its o_proj / down_proj GEMMs write their partial sums into, and the
+    residual-add + RMSNorm kernel reads all ranks' partials straight from the peers' buffers over NVLink.
+    Layout per rank (include/kivi_b200.h): half partial[2][rows_max][hidden] (call c uses slot c & 1) + uint64 arrived[world].
+    `epoch` is the device call counter (advanced by the calls of a step, inside the step's CUDA graph), `err` the time-out
+    word of the arrival waits.  With one rank the buffer is ordinary device memory and the kernel reads only it."""
+
+    def __init__(self, rows_max: int, hidden: int, device):
+        multi = dist.is_initialized() and dist.get_world_size() > 1
+        self.world, self.rank = (dist.get_world_size(), dist.get_rank()) if multi else (1, 0)
+        self.rows_max, self.hidden = rows_max, hidden
+        slot = rows_max * hidden                                          # halves per slot
+        n = (2 * slot * 2 + 8 * self.world + 7) // 8                      # int64 words
+        if multi:
+            import torch.distributed._symmetric_memory as symm
+            self.buf = symm.empty(n, dtype=torch.int64, device=device)
+            self.buf.zero_()
+            self.handle = symm.rendezvous(self.buf, dist.group.WORLD)
+            ptrs = [int(p) for p in self.handle.buffer_ptrs]
+        else:
+            self.buf = torch.zeros(n, dtype=torch.int64, device=device)
+            ptrs = [self.buf.data_ptr()]
+        self._slots = self.buf.view(torch.float16)[: 2 * slot].view(2, rows_max, hidden)
+        self.peer_ptrs = torch.tensor(ptrs, dtype=torch.int64, device=device)
+        self.epoch = torch.zeros(1, dtype=torch.int64, device=device)     # call number = epoch + call + 1
+        self.err = torch.zeros(1, dtype=torch.int32, device=device)
+        torch.cuda.synchronize(device)
+        if multi:
+            dist.barrier()                                                # every buffer is zeroed before anyone arrives
+
+    def slot(self, call: int, rows: int) -> torch.Tensor:
+        """[rows, hidden] fp16 view of this rank's partial-sum slot of call number `call` (what the GEMM writes)."""
+        return self._slots[call & 1, :rows]
+
+    def check(self):
+        """Raise if a reduction timed out waiting for another rank (synchronises: reads the device error word)."""
+        if int(self.err.item()) != 0:
+            raise RuntimeError("kivi_b200: the tensor-parallel all-reduce timed out waiting for another rank")
 
 
 def barrier():

@@ -21,6 +21,8 @@ def _bind():
     _lib.bind("kivi_rope_split_f16", i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp])
     _lib.bind("kivi_silu_mul_f16", i32, [vp, vp, i32, i32, vp])
     _lib.bind("kivi_greedy_sample_exchange_f32", i32, [vp, i32, i32, vp, vp, vp, i32, i32, vp, vp, vp])
+    _lib.bind("kivi_allreduce_add_rmsnorm_f16", i32,
+              [vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, i32, i32, i32, i32, vp, vp, i32, vp])
     _B = True
 
 
@@ -49,6 +51,33 @@ def add_rmsnorm(x, residual, weight, out, eps: float):
     _lib.check(_lib.lib().kivi_add_rmsnorm_f16(x.data_ptr() if x is not None else None, residual.data_ptr(),
                                                weight.data_ptr(), out.data_ptr(), rows, hidden, eps,
                                                _lib.stream_ptr(residual.device)), "kivi_add_rmsnorm_f16")
+    return out
+
+
+def allreduce_add_rmsnorm(residual, weight, out, eps: float, ar, call: int = 0, x=None, cluster: int = 0):
+    """Tensor-parallel add_rmsnorm: residual += fp16(sum over ranks of fp32 partials, in rank order); out = RMSNorm(residual).
+    ar: kivi_b200.dist.PeerAllReduce (or an object with its fields); this rank's partial of call number `call` must already be
+    in ar.slot(call, rows).  ar None: one rank, `x` is the whole sum (exactly add_rmsnorm).  cluster: CTAs per row (1, 2, 4,
+    8; 0 = the library's default, one) -- the result does not depend on it."""
+    _bind()
+    if residual.dim() != 2:
+        raise ValueError(f"residual: expected [rows, hidden], got shape {tuple(residual.shape)}")
+    rows, hidden = residual.shape
+    f16 = torch.float16
+    for name, t, shape in (("residual", residual, (rows, hidden)), ("weight", weight, (hidden,)), ("out", out, (rows, hidden)),
+                           ("x", x, (rows, hidden))):
+        if t is not None:
+            _check(name, t, f16, shape)
+    if ar is not None:
+        if ar.hidden != hidden or rows > ar.rows_max:
+            raise ValueError(f"the all-reduce buffer holds [{ar.rows_max}, {ar.hidden}] rows, got [{rows}, {hidden}]")
+        _lib.require_cuda(ar.peer_ptrs, ar.epoch, ar.err)
+    _lib.check(_lib.lib().kivi_allreduce_add_rmsnorm_f16(
+        x.data_ptr() if x is not None else None, residual.data_ptr(), weight.data_ptr(), out.data_ptr(), rows, hidden, eps,
+        ar.peer_ptrs.data_ptr() if ar is not None else None, ar.rank if ar is not None else 0,
+        ar.world if ar is not None else 1, ar.rows_max if ar is not None else rows, call,
+        ar.epoch.data_ptr() if ar is not None else None, ar.err.data_ptr() if ar is not None else None, cluster,
+        _lib.stream_ptr(residual.device)), "kivi_allreduce_add_rmsnorm_f16")
     return out
 
 

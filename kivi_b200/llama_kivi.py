@@ -28,6 +28,7 @@ import torch.nn.functional as F
 from .cache import KiviCache, kv_start_from_mask
 from .matmul import cuda_bmm_fA_qB_outer
 from .new_pack import triton_quantize_and_pack_along_last_dim
+from .tp import check_divisible, shard_of, shard_state_dict, shard_tensor, sum_partials  # noqa: F401 (re-export)
 
 
 def repeat_kv(hidden_states: torch.Tensor, n_rep: int) -> torch.Tensor:
@@ -130,6 +131,10 @@ def default_config(name: str = "llama-2-7b", **kw):
                            num_key_value_heads=8, vocab_size=128256, rope_theta=500000.0, rms_norm_eps=1e-5),
         "mistral-7b": dict(hidden_size=4096, intermediate_size=14336, num_hidden_layers=32, num_attention_heads=32,
                            num_key_value_heads=8, vocab_size=32000, rope_theta=1000000.0, rms_norm_eps=1e-5),
+        "llama-2-13b": dict(hidden_size=5120, intermediate_size=13824, num_hidden_layers=40, num_attention_heads=40,
+                            num_key_value_heads=40, vocab_size=32000, rope_theta=10000.0, rms_norm_eps=1e-5),
+        "llama-2-70b": dict(hidden_size=8192, intermediate_size=28672, num_hidden_layers=80, num_attention_heads=64,
+                            num_key_value_heads=8, vocab_size=32000, rope_theta=10000.0, rms_norm_eps=1e-5),
         "tiny": dict(hidden_size=256, intermediate_size=512, num_hidden_layers=2, num_attention_heads=2,
                      num_key_value_heads=2, vocab_size=512, rope_theta=10000.0, rms_norm_eps=1e-5),
     }
@@ -169,14 +174,14 @@ def _rotate_half(x):
 class LlamaFlashAttention_KIVI(nn.Module):
     """Attention layer of the reference (models/llama_kivi.py:264-466), KIVI ops on libkivi_b200."""
 
-    def __init__(self, config, layer_idx: int = 0):
+    def __init__(self, config, layer_idx: int = 0, tp_world: int = 1):
         super().__init__()
         self.config = config
         self.layer_idx = layer_idx
         self.hidden_size = config.hidden_size
-        self.num_heads = config.num_attention_heads
-        self.head_dim = self.hidden_size // self.num_heads
-        self.num_key_value_heads = config.num_key_value_heads
+        self.head_dim = self.hidden_size // config.num_attention_heads
+        self.num_heads = config.num_attention_heads // tp_world              # this rank's heads (kivi_b200.tp)
+        self.num_key_value_heads = config.num_key_value_heads // tp_world
         self.num_key_value_groups = self.num_heads // self.num_key_value_heads
         self.k_bits, self.v_bits = config.k_bits, config.v_bits            # models/llama_kivi.py:34-38
         self.group_size, self.residual_length = config.group_size, config.residual_length
@@ -217,20 +222,20 @@ class LlamaFlashAttention_KIVI(nn.Module):
             cache, layer, seq = past_key_value
             attn_output = self._prompt_attention(q, k, v, attention_mask)
             cache.refill(layer, seq, k, v)
-            attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.hidden_size)
+            attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.num_heads * self.head_dim)
             return self.o_proj(attn_output), None, past_key_value
         if fused:
             cache, layer = past_key_value
             if q_len > 1:                                                   # prefill (:401-452)
                 attn_output = self._prompt_attention(q, k, v, attention_mask)
                 cache.prefill(layer, k, v)
-                attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.hidden_size)
+                attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.num_heads * self.head_dim)
             else:                                                           # decode (:314-399), one launch
                 out = cache.decode_attention(layer, q.reshape(bsz, self.num_heads, self.head_dim).contiguous(),
                                              k.reshape(bsz, self.num_key_value_heads, self.head_dim).contiguous(),
                                              v.reshape(bsz, self.num_key_value_heads, self.head_dim).contiguous(),
                                              mask=attention_mask)
-                attn_output = out.view(bsz, 1, self.hidden_size)
+                attn_output = out.view(bsz, 1, self.num_heads * self.head_dim)
             return self.o_proj(attn_output), None, past_key_value
         if past_key_value is not None:                                      # reference 9-tuple, decode
             attn_output, past = kivi_decode_attention_tuple(q, k, v, past_key_value, self.group_size, self.k_bits,
@@ -247,37 +252,44 @@ LlamaAttention_KIVI = LlamaFlashAttention_KIVI      # models/llama_kivi.py:19 (u
 
 
 class LlamaMLP(nn.Module):
-    def __init__(self, config):
+    def __init__(self, config, tp_world: int = 1):
         super().__init__()
-        self.gate_proj = nn.Linear(config.hidden_size, config.intermediate_size, bias=False)
-        self.up_proj = nn.Linear(config.hidden_size, config.intermediate_size, bias=False)
-        self.down_proj = nn.Linear(config.intermediate_size, config.hidden_size, bias=False)
+        inter = config.intermediate_size // tp_world                          # this rank's channels (kivi_b200.tp)
+        self.gate_proj = nn.Linear(config.hidden_size, inter, bias=False)
+        self.up_proj = nn.Linear(config.hidden_size, inter, bias=False)
+        self.down_proj = nn.Linear(inter, config.hidden_size, bias=False)
 
     def forward(self, x):
         return self.down_proj(F.silu(self.gate_proj(x)) * self.up_proj(x))
 
 
 class LlamaDecoderLayer_KIVI(nn.Module):
-    def __init__(self, config, layer_idx):
+    def __init__(self, config, layer_idx, tp_world: int = 1):
         super().__init__()
-        self.self_attn = LlamaFlashAttention_KIVI(config, layer_idx)
-        self.mlp = LlamaMLP(config)
+        self.self_attn = LlamaFlashAttention_KIVI(config, layer_idx, tp_world)
+        self.mlp = LlamaMLP(config, tp_world)
         self.input_layernorm = LlamaRMSNorm(config.hidden_size, config.rms_norm_eps)
         self.post_attention_layernorm = LlamaRMSNorm(config.hidden_size, config.rms_norm_eps)
+        self.tp_world = tp_world
 
     def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None):
         residual = hidden_states
         h, _, past = self.self_attn(self.input_layernorm(hidden_states), cos, sin, past_key_value, attention_mask)
+        if self.tp_world > 1:                                                 # partial sums of the sharded projections
+            h = sum_partials(h)
         hidden_states = residual + h
-        hidden_states = hidden_states + self.mlp(self.post_attention_layernorm(hidden_states))
+        h = self.mlp(self.post_attention_layernorm(hidden_states))
+        if self.tp_world > 1:
+            h = sum_partials(h)
+        hidden_states = hidden_states + h
         return hidden_states, past
 
 
 class LlamaModel_KIVI(nn.Module):
-    def __init__(self, config):
+    def __init__(self, config, tp_world: int = 1):
         super().__init__()
         self.embed_tokens = nn.Embedding(config.vocab_size, config.hidden_size)
-        self.layers = nn.ModuleList([LlamaDecoderLayer_KIVI(config, i) for i in range(config.num_hidden_layers)])
+        self.layers = nn.ModuleList([LlamaDecoderLayer_KIVI(config, i, tp_world) for i in range(config.num_hidden_layers)])
         self.norm = LlamaRMSNorm(config.hidden_size, config.rms_norm_eps)
 
 
@@ -346,13 +358,25 @@ def _additive_mask(attention_mask, q_len: int, total: int, dtype, device):
 class LlamaForCausalLM_KIVI(nn.Module):
     """models/llama_kivi.py:785.  `forward` keeps the reference's contract (HF argument names, per-layer 9-tuples as
     past_key_values, fp32 logits, `prepare_inputs_for_generation`, `_reorder_cache`); `decode_step` / `generate` use
-    the fused cache path (pre-allocated KiviCache, the step captured in a CUDA graph)."""
+    the fused cache path (pre-allocated KiviCache, the step captured in a CUDA graph).
 
-    def __init__(self, config):
+    tensor_parallel=True: one rank of a model sharded over the GPUs of a box (kivi_b200.tp; rank and world from
+    kivi_b200.dist.init(), i.e. torchrun's environment).  The modules are built at this rank's shapes, the cache holds its
+    heads, and the decode step reduces the o_proj / down_proj partial sums with kivi_allreduce_add_rmsnorm_f16 inside its
+    CUDA graph.  generate / decode_step / prefill / insert / serve run on every rank with the same inputs and give every
+    rank the same tokens; forward() (9-tuples), 9-tuple import / export and enable_token_allgather are rejected."""
+
+    def __init__(self, config, tensor_parallel: bool = False):
         super().__init__()
         self.config = config
         self.vocab_size = config.vocab_size
-        self.model = LlamaModel_KIVI(config)
+        self.tensor_parallel = tensor_parallel
+        self.tp_rank, self.tp_world = 0, 1
+        if tensor_parallel:
+            from . import dist as kdist
+            self.tp_rank, self.tp_world, _ = kdist.init()
+            check_divisible(config, self.tp_world)
+        self.model = LlamaModel_KIVI(config, self.tp_world)
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False)
         self._rope = None
         self.cache: KiviCache | None = None
@@ -362,16 +386,20 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._dist_tokens = None            # [world * B] ids gathered inside the step (greedy sampling, world > 1)
         self._dist_in_graph = True
         self._exchange = None               # kivi_b200.dist.PeerTokenExchange: ids stored into the peers' buffers by the sampling kernel
+        self._allreduce = None              # kivi_b200.dist.PeerAllReduce of the tensor-parallel decode step
 
     # ------------------------------------------------------------------ HF-style construction
     @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, config=None, torch_dtype=torch.float16, device_map=None,
-                        **unused):
+                        tensor_parallel: bool = False, **unused):
         """Load a LOCAL Hugging Face Llama / Mistral checkpoint directory (config.json + *.safetensors or
         pytorch_model*.bin; there is no network here) into the KIVI model, as the reference's
         LlamaForCausalLM_KIVI.from_pretrained(config=...) does (example.py:22-28, mem_spd_test.py:24-31).  `config` is
         the user's config object carrying k_bits / v_bits / group_size / residual_length (models/llama_kivi.py:34-38);
-        without one, config.json is read and the KIVI attributes default to K2V2 g32 R128."""
+        without one, config.json is read and the KIVI attributes default to K2V2 g32 R128.
+        tensor_parallel=True: this rank's shard only (kivi_b200.tp): safetensors files are read slice by slice
+        (safe_open(...).get_slice), .bin files are sharded after loading; the modules are built without initialising the
+        full-size weights."""
         import glob
         import json
         import os
@@ -385,25 +413,40 @@ class LlamaForCausalLM_KIVI(nn.Module):
         for name, dflt in (("k_bits", 2), ("v_bits", 2), ("group_size", 32), ("residual_length", 128), ("use_flash", True)):
             if not hasattr(config, name):
                 setattr(config, name, dflt)
-        model = cls(config)
+        if tensor_parallel:
+            from . import dist as kdist
+            kdist.init()                                                  # the process group, outside the meta context
+            with torch.device("meta"):                                   # parameters come from the checkpoint (assign)
+                model = cls(config, tensor_parallel=True)
+            rank, world = model.tp_rank, model.tp_world
+        else:
+            model = cls(config)
         state = {}
         files = sorted(glob.glob(os.path.join(path, "*.safetensors")))
         if files:
-            from safetensors.torch import load_file
-            for fn in files:
-                state.update(load_file(fn))
+            if tensor_parallel:
+                from safetensors import safe_open
+                for fn in files:
+                    with safe_open(fn, framework="pt") as f:
+                        for k in f.keys():
+                            state[k] = shard_tensor(f.get_slice(k), shard_of(k, config, rank, world))
+            else:
+                from safetensors.torch import load_file
+                for fn in files:
+                    state.update(load_file(fn))
         else:
             for fn in sorted(glob.glob(os.path.join(path, "pytorch_model*.bin"))):
-                state.update(torch.load(fn, map_location="cpu", weights_only=True))
+                part = torch.load(fn, map_location="cpu", weights_only=True)
+                state.update(shard_state_dict(part, config, rank, world) if tensor_parallel else part)
         if not state:
             raise FileNotFoundError(f"{path}: no *.safetensors / pytorch_model*.bin weights found")
         if "lm_head.weight" not in state and getattr(config, "tie_word_embeddings", False):
             state["lm_head.weight"] = state["model.embed_tokens.weight"]
         state = {k: v for k, v in state.items() if not k.endswith("rotary_emb.inv_freq")}
-        model.load_state_dict(state, strict=True)
+        model.load_state_dict(state, strict=True, assign=tensor_parallel)
         if torch_dtype is not None:
             model = model.to(torch_dtype)
-        if device_map is not None:          # "auto" / "cuda" / {"": device}: one replica on the current GPU (dp, not pipeline)
+        if device_map is not None:          # "auto" / "cuda" / {"": device}: this rank's model on the current GPU (dp or tp)
             model = model.cuda()
         return model.eval()
 
@@ -449,6 +492,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
         9-tuples (:696-698, :911-916); prefill when past_key_values is None.  attention_mask: HF padding mask
         [B, kv_len] or an additive [B, 1, q_len, kv_len].  The result unpacks as (logits, past_key_values) and has the
         attributes of CausalLMOutputWithPast; with return_dict=True (or config.use_return_dict) it IS one."""
+        if self.tensor_parallel:
+            raise NotImplementedError("forward() returns the reference's per-layer 9-tuples, which hold every head; a "
+                                      "tensor-parallel rank holds its share: use generate / decode_step / serve")
         B, q_len = input_ids.shape
         if past_key_values is not None and len(past_key_values) == 0:
             past_key_values = None
@@ -551,10 +597,17 @@ class LlamaForCausalLM_KIVI(nn.Module):
         cfg = self.config
         dev = self.lm_head.weight.device
         self.cache, self._graph = None, None                 # release the previous cache before the new one is allocated
-        self.cache = KiviCache(cfg.num_hidden_layers, batch, cfg.num_attention_heads, cfg.num_key_value_heads,
-                               cfg.hidden_size // cfg.num_attention_heads, cfg.k_bits, cfg.v_bits, cfg.group_size,
+        a = self.model.layers[0].self_attn                  # this rank's heads
+        self.cache = KiviCache(cfg.num_hidden_layers, batch, a.num_heads, a.num_key_value_heads,
+                               a.head_dim, cfg.k_bits, cfg.v_bits, cfg.group_size,
                                cfg.residual_length, max_tokens, device=dev,
                                overlap_prologue=True)       # the attention call follows the layer's RoPE kernel
+        if self.tensor_parallel:
+            self.cache.tensor_parallel = True
+            if self._allreduce is None or self._allreduce.rows_max != batch:
+                from . import dist as kdist
+                self._allreduce = None
+                self._allreduce = kdist.PeerAllReduce(batch, cfg.hidden_size, dev)
         self._graph, self._graph_ragged = None, False
         self._pos = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._ids = torch.zeros((batch, 1), dtype=torch.long, device=dev)
@@ -565,6 +618,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def import_cache(self, past_key_values, max_tokens: int | None = None):
         """Continue on the fused path from the reference's per-layer 9-tuples (models/llama_kivi.py:454-455)."""
+        if self.tensor_parallel:
+            raise NotImplementedError("import_cache: the reference's 9-tuples hold every head; a tensor-parallel rank "
+                                      "holds its share")
         seen = past_key_values[0][-1]
         B = past_key_values[0][5].shape[0]
         if self.cache is None or self.cache.batch != B or max(max_tokens or 0, seen + 1) > self.cache.max_tokens:
@@ -639,6 +695,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._pos.fill_(n)
 
     def _step_body(self):
+        if self.tensor_parallel and not self._fast_ok():
+            raise NotImplementedError("tensor-parallel decoding needs head_dim 128, bias-free projections and fp16 weights")
         if self._fast_ok():
             self._step_body_fast()
         else:
@@ -664,6 +722,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         mode "p2p": the sampling kernel itself stores the ids into every peer's symmetric buffer (PeerTokenExchange; one
         fused compute + collective kernel inside the step's CUDA graph).  mode "nccl": an NCCL all-gather of the ids, inside
         the graph (in_graph) or right after the replay.  Call before the first decode_step (the step is captured once)."""
+        if self.tensor_parallel:
+            raise NotImplementedError("data-parallel replicas of a tensor-parallel model are not supported")
         self._exchange, self._dist_tokens = None, None
         if world_size > 1 and mode == "p2p":
             from . import dist as kdist
@@ -692,7 +752,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if self._fast is not None and self._fast.B == self.cache.batch:
             return self._fast
         cfg, dev, B = self.config, self.cache.device, self.cache.batch
-        H, Hkv, hid, inter = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.hidden_size, cfg.intermediate_size
+        a0 = self.model.layers[0].self_attn                                  # this rank's shapes (all of them at world 1)
+        H, Hkv, hid = a0.num_heads, a0.num_key_value_heads, cfg.hidden_size
+        inter = self.model.layers[0].mlp.gate_proj.weight.shape[0]
         f = self._fast if self._fast is not None else SimpleNamespace(wqkv=None)
         f.B = B
         if f.wqkv is None:
@@ -723,6 +785,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
     def _step_body_fast(self):
         """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split,
         fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels."""
+        if self.tensor_parallel:
+            return self._step_body_tp()
         from . import glue
         f = self._ensure_fast()
         cfg, cache = self.config, self.cache
@@ -744,6 +808,43 @@ class LlamaForCausalLM_KIVI(nn.Module):
             glue.add_rmsnorm(f.d, f.res, nxt, f.h, eps)
         torch.mm(f.h, self.lm_head.weight.t(), out=f.logits16)
         self._logits.copy_(f.logits16)                                       # logits.float() (:881)
+
+    def _step_body_tp(self):
+        """The decode step of one tensor-parallel rank: the same launches on this rank's heads and channels, but o_proj and
+        down_proj write their partial sums into the PeerAllReduce slots, and the two residual-add + RMSNorm kernels of a
+        layer become kivi_allreduce_add_rmsnorm_f16 (calls 2i and 2i + 1 of the step), which add up every rank's partials.
+        The embedding's RMSNorm and lm_head are replicated: every rank computes the same logits."""
+        from . import glue
+        f, ar = self._ensure_fast(), self._allreduce
+        cfg, cache = self.config, self.cache
+        cos_t, sin_t = self._tables(cache.device)
+        eps = cfg.rms_norm_eps
+        layers = self.model.layers
+        f.res.copy_(self.model.embed_tokens(self._ids)[:, 0])
+        glue.add_rmsnorm(None, f.res, layers[0].input_layernorm.weight, f.h, eps)
+        for i, l in enumerate(layers):
+            torch.mm(f.h, f.wqkv[i], out=f.qkv)
+            glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
+            cache.decode_attention(i, f.q, f.k, f.v, out=f.attn)
+            torch.mm(f.attn.view(f.B, -1), f.wo[i], out=ar.slot(2 * i, f.B))
+            glue.allreduce_add_rmsnorm(f.res, l.post_attention_layernorm.weight, f.h, eps, ar, call=2 * i)
+            torch.mm(f.h, f.wgu[i], out=f.gu)
+            glue.silu_mul(f.gu, f.act)
+            torch.mm(f.act, l.mlp.down_proj.weight.t(), out=ar.slot(2 * i + 1, f.B))
+            nxt = layers[i + 1].input_layernorm.weight if i + 1 < len(layers) else self.model.norm.weight
+            glue.allreduce_add_rmsnorm(f.res, nxt, f.h, eps, ar, call=2 * i + 1)
+        ar.epoch.add_(2 * len(layers))                                       # the next step's calls continue the count
+        torch.mm(f.h, self.lm_head.weight.t(), out=f.logits16)
+        self._logits.copy_(f.logits16)
+
+    def first_tokens(self, logits):
+        """Greedy ids of prompt logits (prefill / insert) -- under tensor parallelism rank 0's, broadcast, so the ranks can
+        never start from different tokens."""
+        tok = logits.argmax(-1)
+        if self.tensor_parallel and self.tp_world > 1:
+            import torch.distributed as dist
+            dist.broadcast(tok, src=0)
+        return tok
 
     def cache_advance_device(self):
         from . import _lib
@@ -796,6 +897,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if self._dist_tokens is not None and not self._dist_in_graph:
             from . import dist as kdist
             kdist.gather_tokens(self.next_tokens, out=self._dist_tokens)
+        if self._allreduce is not None:
+            self._allreduce.check()
         self.cache._mirror_advance()
         return self._logits
 
@@ -819,7 +922,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.init_cache(B, n + max_new_tokens)
         logits = self.prefill(input_ids, attention_mask)
         out = [input_ids]
-        tok = logits.argmax(-1, keepdim=True)
+        tok = self.first_tokens(logits).view(B, 1)
         for _ in range(max_new_tokens - 1):
             out.append(tok)
             self.decode_step(tok, use_graph=use_graph)

@@ -97,7 +97,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
         ids, mask = ids.to(dev), mask.to(dev)
         logits = model.prefill(ids, attention_mask=mask)
         cache.set_kv_start(kv_start_from_mask(mask))                      # ragged from the start: one step graph
-        first = logits.argmax(-1)
+        first = model.first_tokens(logits)
         model._ids.copy_(first.view(batch, 1))
         first = first.tolist()
         stats["prefills"] += 1
@@ -124,7 +124,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
                         stats["shifts"] += 1
                         stats["shifted_tokens"] += plan[0]
                     i = queue.popleft()
-                    tok = int(model.insert(slot, p.to(dev)).argmax())
+                    tok = int(model.first_tokens(model.insert(slot, p.to(dev))))
                     model._ids[slot] = tok
                     owner[slot] = i
                     stats["inserts"] += 1
