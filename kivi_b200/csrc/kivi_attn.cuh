@@ -161,10 +161,17 @@ constexpr float kRcpSqrtD = 1.0f / 11.313708f;   // ATen: x * (1.0f / float(math
 // with every fp32 rounding of the contraction).  Inputs outside those regimes take exactly the arithmetic they always took:
 //   q.K^T: a head whose max|q| is below 2^-3 enters scaled into [2^Q, 2^(Q+1)) (q_prescale), Q = 0 for 2-bit K, 2 for 4-bit
 //          K; other heads enter as they are.  A finite K scale is at most 65504 / (2^bits - 1), so hi = fp16(q*s) cannot
-//          overflow for a prescaled head.
-//   p.V:   probabilities enter x 2^6.  A packed block whose largest V scale m is below 2^-4 (pv_boost) takes them
+//          overflow for a prescaled head.  Every packed K block is then checked against the unit's prescaled max|q| = 2^qe
+//          (qk_guard): where qe + floor(log2 m), m the block's largest finite K scale, leaves [-4, 14] (some q*s could
+//          overflow, or even the largest products are below 2^-4), the block's scales are rescaled in place by 2^-a so that
+//          every product is below 2^15 and the largest at least 2^11; the zero term takes 2^-a in fp32, the epilogue 2^a.
+//   p.V:   probabilities enter x 2^6.  A packed block whose largest finite V scale m is below 2^-4 (pv_boost) takes them
 //          x 2^(6 + e + b) instead, e = floor(log2 S) of the softmax denominator S, b = min(-4 - floor(log2 m), 9): max p <= 1 / S,
-//          so the scaled probabilities stay below 2^(6 + b) <= 2^15 and p*s below 8, at any context length.
+//          so the scaled probabilities stay below 2^(6 + b) <= 2^15 and p*s below 8, at any context length.  A block whose
+//          m is below 2^-13 (where b would pass its cap) or 2^10 and above (where p * 2^6 * s can overflow) first has its
+//          scales rescaled in place by 2^-v (pv_vshift), into [2^-13, 2^-12) or [2^8, 2^9); the zero term and the epilogue
+//          undo it as in q.K^T.
+//   The block maxima skip non-finite scales: an inf scale stays non-finite and does not set the factor of its block.
 constexpr float kProbScale = 64.f, kProbScaleInv = 1.f / 64.f;
 constexpr float kQPrescaleBelow = 0.125f;
 
@@ -180,6 +187,14 @@ __device__ __forceinline__ float2 q_prescale(float mx) {
 __device__ __forceinline__ int pv_boost(float m) {
     if (!(m > 0.f) || !(m < 0.0625f)) return 0;
     return min(-4 - ((int)((__float_as_uint(m) >> 23) & 0xff) - 127), 9);     // >= 1: floor(log2 m) <= -5
+}
+// floor(log2 |x|) of a normal fp32 x (-127 for 0)
+__device__ __forceinline__ int exp2_floor(float x) { return (int)((__float_as_uint(x) >> 23) & 0xff) - 127; }
+// v of a packed V block whose largest finite |scale| is m: its scales are taken x 2^-v in place, bringing m into [2^8, 2^9)
+// for m >= 2^10 and into [2^-13, 2^-12) (pv_boost 9) for 0 < m < 2^-13; 0 otherwise
+__device__ __forceinline__ int pv_vshift(float m) {
+    const int e = exp2_floor(m);
+    return m >= 1024.f ? e - 8 : (m > 0.f && e < -13) ? e + 13 : 0;
 }
 // exponent of the extra probability scale of a boosted block: e + b, e = floor(log2 S) in [0, 15] (S >= 1: the largest
 // logit contributes exp(0) = 1; NaN -> 15)
@@ -290,6 +305,11 @@ __device__ __forceinline__ float fast_exp(float x) {
 
 __device__ __forceinline__ uint32_t h2_as_u32(const __half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
 __device__ __forceinline__ __half2 u32_as_h2(const uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
+// |h| of both halves, 0 for the non-finite ones (an inf scale must not set the factor of its block's finite groups)
+__device__ __forceinline__ __half2 finite_abs2(uint32_t w) {
+    const __half2 a = __habs2(u32_as_h2(w));
+    return u32_as_h2(h2_as_u32(a) & __hlt2_mask(a, __float2half2_rn(INFINITY)));
+}
 
 // One B-fragment register: column part 0 -> hi = fp16(x*s); part 1 -> lo = x*s - hi, exact while it is not below fp16's
 // smallest step (the callers prescale x where it would not be: q_prescale, pv_boost).
@@ -306,6 +326,56 @@ __device__ __forceinline__ uint32_t b_prep(uint32_t x2, uint32_t s2, __half2 mse
     const __half2 nh = __hmul2(__hmul2(x, s), msel);         // nh = hi * (part ? -1 : 0);  b = fma(x, s, nh)
     return h2_as_u32(__hfma2(x, s, nh));
 #endif
+}
+
+// Multiply the finite scales of the meta units that `keep(idx)` selects by 2^-a in place (idx = lane + 32 i: the (chunk,
+// group, t) units, {z, s, z, s}); the others get scale 0.  Exact: powers of two, the largest scale stays below 2^15; a
+// scale taken down into the fp16 subnormals loses its low bits (those of scales below 2^(a - 14)).  The z rows are untouched.
+template <int NG, class KF>
+__device__ __forceinline__ void rescale_meta(uint4* mt, int a, int lane, KF&& keep) {
+    const float f = __uint_as_float((uint32_t)(127 - a) << 23);
+    auto sc = [&](uint32_t w, bool k0, bool k1) {
+        const float2 x = __half22float2(u32_as_h2(w));
+        return h2_as_u32(__floats2half2_rn(k0 ? x.x * f : 0.f, k1 ? x.y * f : 0.f));
+    };
+    #pragma unroll
+    for (int i = 0; i < NG; ++i) {
+        const int idx = lane + 32 * i;
+        uint4 w = mt[idx];
+        w.y = sc(w.y, keep(idx, 0), keep(idx, 1)); w.w = sc(w.w, keep(idx, 8), keep(idx, 9));
+        mt[idx] = w;
+    }
+    __syncwarp();
+}
+
+// q.K^T block guard.  qexp = floor(log2) of the unit's prescaled max|q| over its heads (-127: q = 0), m = the block's
+// largest finite K scale over the token groups below nvalid (later groups hold no data; their logits are dropped).
+// Unflagged while e = qexp + floor(log2 m) is in [-4, 14]: every |q*s| < 2^(e+2) stays at most 65504 after rounding, and
+// the largest products are at least 2^-4.  A flagged block gets a = max(e - 13, floor(log2 m) - 14): every product below
+// 2^15 and (qexp >= -3 for an unprescaled head) the largest at least 2^11.  Its scales are rescaled in place by 2^-a
+// (rescale_meta).  For a > 0 a scale s loses low bits where s * 2^-a < 2^-14, i.e. below 2^(a - 14) <= m * 2^(qexp - 27):
+// 2^20 below m at qexp = 7, only 2^12 below it for max|q| near 2^15; those groups' residuals lo move 2^a closer to the
+// fp16 denormals as well.
+// Returns a (0: unflagged).  Runs on every packed K block: NG shared loads, 5 shuffles, ~20 instructions per lane.
+template <int BITS, int GS>
+__device__ __forceinline__ int qk_guard(uint8_t* st, int qexp, int nvalid, int lane) {
+    constexpr int NG = 128 / GS;
+    uint4* mt = reinterpret_cast<uint4*>(st + kHalfChunks * Lay<BITS>::kChunkBytes);
+    auto valid = [&](int idx, int) { return ((idx >> 2) % NG) * GS < nvalid; };
+    __half2 m2 = __float2half2_rn(0.f);
+    #pragma unroll
+    for (int i = 0; i < NG; ++i) {
+        const uint4 w = mt[lane + 32 * i];
+        if (valid(lane + 32 * i, 0)) m2 = __hmax2(m2, __hmax2(finite_abs2(w.y), finite_abs2(w.w)));
+    }
+    float m = fmaxf(__low2float(m2), __high2float(m2));
+    #pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    const int fm = exp2_floor(m), e = qexp + fm;
+    if (!(m > 0.f) || qexp == -127 || (e >= -4 && e <= 14)) return 0;
+    const int a = max(e - 13, fm - 14);
+    rescale_meta<NG>(mt, a, lane, valid);
+    return a;
 }
 
 // exact power of two 2^(24 - P) that undoes the denormal scaling of the fields of MMA mm
@@ -969,7 +1039,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
 
         // ---- this warp's copy of q: half2 pairs in B-fragment order (prescaled: q_prescale), fp32 in channel order (as is);
         // qpost_blk / qpost_win undo the prescale of the head of this lane's packed-block / window-item outputs
-        float qpost_blk = 1.f, qpost_win = 1.f;
+        float qpost_blk = 1.f, qpost_win = 1.f, qmx = 0.f;
         __syncwarp();
         #pragma unroll
         for (int h = 0; h < G; ++h) {
@@ -987,7 +1057,9 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
             q2[h * 32 + lane] = make_uint2(sc(qf[h].x), sc(qf[h].y));
             if (h == h_l) qpost_blk = ps.y;
             if (h == (lane >> 2)) qpost_win = ps.y;
+            qmx = fmaxf(qmx, mx * ps.x);
         }
+        const int qexp = exp2_floor(qmx);                                    // floor(log2) of the prescaled max|q| of the unit
         __syncwarp();
         if (left > n_here) fetch_q(unit + 1);                                // the range continues into the next unit
 
@@ -1011,9 +1083,12 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     #pragma unroll
                     for (int e = 0; e < 4; ++e) zc[e] = 0.f;
                 }
+                static_assert(kParts == 1, "the scale guard of a block (qk_guard) is chosen from the whole block's scales");
+                int kshift = 0;                                              // qk_guard of the block (warp-uniform)
                 #pragma unroll 1
                 for (int half = 0; half < kParts; ++half) {
                     pp.wait();
+                    kshift = qk_guard<KB, GS>(pp.cons(), qexp, s.tk - j * kBlockTokens, lane);
                     mma_half<KB, G, GS, kParts == 1>(pp.cons(), half * kHalfChunks, [&](int cc, int h, uint32_t& xa, uint32_t& xb) {
                         const uint2 v = q2[(h * 8 + cc) * 4 + t4];
                         xa = v.x; xb = v.y;
@@ -1024,6 +1099,13 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
+                float post = qpost_blk;
+                if (kshift) {                                                // the scales entered x 2^-kshift, the zero term as is
+                    const float dn = __uint_as_float((uint32_t)(127 - kshift) << 23);
+                    #pragma unroll
+                    for (int grp = 0; grp < NG; ++grp) zsel[grp] *= dn;
+                    post *= __uint_as_float((uint32_t)(127 + kshift) << 23);
+                }
                 const int64_t rowi = uq0 + h_l;
                 __half* row = p.w.lg + rowi * p.w.ld + j * kBlockTokens;
                 const int nvalid = s.tk - j * kBlockTokens;                  // < 128 only in the last block when R < 128
@@ -1035,13 +1117,13 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 #pragma unroll
                 for (int e = 0; e < Slots<G, GS>::k; ++e) x[e] = -INFINITY;
                 if (!slow && !padded && nvalid >= kBlockTokens) {
-                    finalize<KB, G, GS>(acc, zsel, lane, qpost_blk, [&](int slot, int o, float v) {
+                    finalize<KB, G, GS>(acc, zsel, lane, post, [&](int slot, int o, float v) {
                         const __half hv = scale_logit(v);
                         row[o] = hv;
                         x[slot] = __half2float(hv);
                     });
                 } else {
-                    finalize<KB, G, GS>(acc, zsel, lane, qpost_blk, [&](int slot, int o, float v) {
+                    finalize<KB, G, GS>(acc, zsel, lane, post, [&](int slot, int o, float v) {
                         if (o < nvalid) {
                             __half hv = scale_logit(v);                      // fp16 scaled (+ mask): the softmax input
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + j * kBlockTokens + o);
@@ -1549,7 +1631,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     pp.wait();
                     uint8_t* st = pp.cons();
                     __half* prob = reinterpret_cast<__half*>(st + kHalfBytes);   // [G][kPartTokens] logits -> scaled probabilities
-                    {   // the block's largest |V scale|: lane reads the (chunk, group, t) meta units lane, lane + 32, ...
+                    {   // the block's largest finite |V scale|: lane reads the (chunk, group, t) meta units lane, lane + 32, ...
                         const uint4* mt = reinterpret_cast<const uint4*>(st + kHalfChunks * Lay<VB>::kChunkBytes);
                         const __half h0 = __float2half_rn(0.f);
                         __half2 m2 = __half2half2(h0);
@@ -1557,7 +1639,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                         for (int i = 0; i < NG; ++i) {
                             const int idx = lane + 32 * i;               // {z, s} of tokens 16 c + 2 t + {0, 1} and + {8, 9}
                             const uint4 w = mt[idx];
-                            __half2 sa = __habs2(u32_as_h2(w.y)), sb = __habs2(u32_as_h2(w.w));
+                            __half2 sa = finite_abs2(w.y), sb = finite_abs2(w.w);
                             if (nt < kPartTokens) {                      // the end of the store: later slots hold no data
                                 const int tok = 16 * ((idx >> 2) / NG) + 2 * (idx & 3);
                                 sa = __halves2half2(tok < nt ? __low2half(sa) : h0, tok + 1 < nt ? __high2half(sa) : h0);
@@ -1568,8 +1650,15 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                         float m = fmaxf(__low2float(m2), __high2float(m2));
                         #pragma unroll
                         for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                        boost = pv_boost(m);
-                        if (lane == 0) *reinterpret_cast<volatile int*>(obuf) = boost;   // obuf: unused by packed blocks
+                        const int vshift = pv_vshift(m);
+                        boost = pv_boost(m * __uint_as_float((uint32_t)(127 - vshift) << 23));
+                        if (vshift)                                          // the end of the store: later slots hold no data
+                            rescale_meta<NG>(const_cast<uint4*>(mt), vshift, lane, [&](int idx, int d) {
+                                return nt >= kPartTokens || 16 * ((idx >> 2) / NG) + 2 * (idx & 3) + d < nt; });
+                        if (lane == 0) {                                     // obuf: unused by packed blocks
+                            reinterpret_cast<volatile int*>(obuf)[0] = boost;
+                            reinterpret_cast<volatile int*>(obuf)[1] = vshift;
+                        }
                     }
                     #pragma unroll
                     for (int h = 0; h < G; ++h) {
@@ -1608,15 +1697,19 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
-                const int boost_b = *reinterpret_cast<volatile const int*>(obuf);   // parked across the MMAs (register pressure)
+                const int boost_b = reinterpret_cast<volatile const int*>(obuf)[0];   // parked across the MMAs (register pressure)
+                const int vshift_b = reinterpret_cast<volatile const int*>(obuf)[1];
                 __syncwarp();
-                if (!boost_b) {
+                if (!(boost_b | vshift_b)) {
                     finalize<VB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int, float v) { run[slot] += v; });
                 } else {                                                     // back to the x 2^6 of the running sums
-                    float post = 0.f;
+                    float post = 0.f;                                        // x 2^(v - e - b); the zero term entered without 2^-v
                     #pragma unroll
                     for (int h = 0; h < G; ++h)
-                        if (h == h_l) post = __uint_as_float((uint32_t)(127 - pv_extra_exp(S[h], boost_b)) << 23);
+                        if (h == h_l) post = __uint_as_float((uint32_t)(127 + vshift_b - (boost_b ? pv_extra_exp(S[h], boost_b) : 0)) << 23);
+                    const float zdn = __uint_as_float((uint32_t)(127 - vshift_b) << 23);
+                    #pragma unroll
+                    for (int grp = 0; grp < NG; ++grp) zsel[grp] *= zdn;
                     finalize<VB, G, GS>(acc, zsel, lane, post, [&](int slot, int, float v) { run[slot] += v; });
                 }
             } else if (j < s.bpu - 1) {                                      // ---- fp16 V window item (tensor cores)

@@ -69,6 +69,11 @@ def test_prefill_matches_oracle(n, kb, vb, g, R):
     assert to_np(cache.state)[:6].tolist() == [cache.tk, cache.r, cache.tv, cache.L, cache.vhead, cache.kv_len]
 
 
+def _step16(x):
+    """Bound of one fp16 rounding step of x: 2^-10 |x|, and the subnormal step 2^-24 below 2^-14."""
+    return np.maximum(2.0 ** -10 * np.abs(np.asarray(x, np.float64)), 2.0 ** -24)
+
+
 def _stage_checks(cache_tuple_before, q, k_new, v_new, g, kb, vb, R, got_out, got_s, got_p, mask=None):
     """cache_tuple_before: oracle 9-tuple BEFORE the step (numpy)."""
     Kq, Kfull, Ks, Kz, Vq, Vfull, Vs, Vz, kv_len = cache_tuple_before
@@ -105,6 +110,8 @@ def _stage_checks(cache_tuple_before, q, k_new, v_new, g, kb, vb, R, got_out, go
     for cand in (logits, np.nextafter(logits, np.float16(-np.inf)), np.nextafter(logits, np.float16(np.inf))):
         ok |= (gs == _sc(cand))
     ok |= np.abs(gs.astype(np.float64) - exp_s.astype(np.float64)) <= 1e-6 * l1 / 11.3
+    if mask is not None:      # masked positions are not part of the kernel's result (fp16(s + finfo.min) depends on s)
+        ok |= np.broadcast_to(mask == np.finfo(np.float16).min, ok.shape)
     assert ok.all(), f"scaled logits: {(~ok).sum()} / {ok.size} differ by more than one fp16 ulp of the kernel output"
     # ---- stage 2: softmax of the kernel's own scaled logits
     exp_p = ref.scale_softmax(np.ascontiguousarray(got_s[..., :T]), 1)
@@ -122,10 +129,12 @@ def _stage_checks(cache_tuple_before, q, k_new, v_new, g, kb, vb, R, got_out, go
         out_q = ref.bmm_fA_qB_outer(g, pq, Vq, Vs, Vz, vb)
         exp_out = ref.add_f16(out_q, out_r)
         l1o = l1o + l1_mass_ref_layout(pq, Vs, Vz, 2 ** vb - 1)
-        # the two fp16 partial sums may each flip by one ulp before the fp16 add
-        l1o = l1o + (2.0 ** -10 / 1e-6) * (np.abs(out_q.astype(np.float64)) + np.abs(out_r.astype(np.float64)))
+        # the two fp16 partial sums may each flip by one ulp before the fp16 add (one step is 2^-24 in the subnormals)
+        l1o = l1o + (1 / 1e-6) * (_step16(out_q) + _step16(out_r))
     else:
         exp_out = out_r
+    # rtol covers one rounding step of a normal fp16 output (2^-10 relative at most); a subnormal output's step is 2^-24
+    l1o = l1o + np.where(np.abs(exp_out.astype(np.float64)) < 2.0 ** -14, 2.0 ** -24 / 1e-6, 0.0)
     assert_gemv_close(got_out, exp_out, l1o, "attention output (own probs)")
 
 
