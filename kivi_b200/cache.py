@@ -280,10 +280,15 @@ class KiviCache:
         return out
 
     def advance(self):
+        self._enqueue_advance()
+        self._mirror_advance()
+
+    def _enqueue_advance(self):
+        """The device half of advance(): one launch, capturable in a CUDA graph whose every replay is followed by
+        _mirror_advance()."""
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().kivi_cache_advance(ctypes.byref(self._structs[0]), _lib.stream_ptr(self.device)),
                        "kivi_cache_advance")
-        self._mirror_advance()
 
     def read_state(self):
         """The device-side `state` words (synchronises the stream); raises if a decode kernel flagged a capacity

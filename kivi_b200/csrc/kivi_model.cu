@@ -10,32 +10,37 @@ namespace cg = cooperative_groups;
 
 namespace kivi {
 
-// residual (fp16, in/out) += x;  out = weight * fp16( residual * rsqrt(mean(residual^2) + eps) )
-// (LlamaRMSNorm.forward: fp32 statistics, cast to fp16, then multiply by the fp16 weight)
-// One CTA per row, every thread keeps its 8-element slices in registers between the two passes.
-template <bool ADD>
-__global__ void __launch_bounds__(512)
-add_rmsnorm_kernel(const __half* __restrict__ x, __half* __restrict__ residual, const __half* __restrict__ w,
-                   __half* __restrict__ out, int hidden, float eps)
+constexpr int kNormThreads = 512, kNormMaxIter = 4;
+constexpr int kNormMaxHidden = kNormMaxIter * kNormThreads * 8;           // 16384: every 8-element slice held in registers
+
+// One row of residual-add + RMSNorm, the body of add_rmsnorm_kernel and allreduce_add_rmsnorm_kernel:
+//   residual (fp16, in/out) += addend;  out = weight * fp16( residual * rsqrt(mean(residual^2) + eps) )
+// (LlamaRMSNorm.forward: fp32 statistics, cast to fp16, then multiply by the fp16 weight).
+// The row has 512 threads, spread over a cluster of C CTAs of 512 / C; thread vt owns the 8-element slices vt, vt + 512, ...
+// and keeps them in registers between the two passes.  The per-thread and per-warp sums of squares and the order in which
+// the 16 warp sums are added do not depend on C, so neither do the bits.
+// ADD: addend(i) returns slice i of the addend as 4 __half2 (a uint4); without ADD the residual is only normalised.
+template <int C, bool ADD, class Addend>
+__device__ __forceinline__ void add_rmsnorm_row(Addend addend, __half* __restrict__ r, const __half* __restrict__ w,
+                                                __half* __restrict__ out, int hidden, float eps, int vt)
 {
-    constexpr int kMaxIter = 4;                          // hidden <= 4 * 512 * 8 = 16384
-    __shared__ float red[16];
-    const int row = blockIdx.x;
-    __half* r = residual + (int64_t)row * hidden;
+    constexpr int kWarps = kNormThreads / C / 32;
+    __shared__ float red[kWarps];
     const int nvec = hidden / 8;
-    uint4 v[kMaxIter];
+    uint4 v[kNormMaxIter];
     float ss = 0.f;
     #pragma unroll
-    for (int it = 0; it < kMaxIter; ++it) {
-        const int i = threadIdx.x + it * 512;
+    for (int it = 0; it < kNormMaxIter; ++it) {
+        const int i = vt + it * kNormThreads;
         if (i < nvec) {
+            uint4 a;
+            if (ADD) a = addend(i);                                      // issued first: the peer loads of the all-reduce
             uint4 u = *reinterpret_cast<const uint4*>(r + i * 8);
             __half2* h = reinterpret_cast<__half2*>(&u);
             if (ADD) {
-                const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + (int64_t)row * hidden) + i);
-                const __half2* xh = reinterpret_cast<const __half2*>(&xv);
+                const __half2* ah = reinterpret_cast<const __half2*>(&a);
                 #pragma unroll
-                for (int e = 0; e < 4; ++e) h[e] = __hadd2_rn(h[e], xh[e]);
+                for (int e = 0; e < 4; ++e) h[e] = __hadd2_rn(h[e], ah[e]);
                 *reinterpret_cast<uint4*>(r + i * 8) = u;
             }
             #pragma unroll
@@ -45,14 +50,26 @@ add_rmsnorm_kernel(const __half* __restrict__ x, __half* __restrict__ residual, 
     }
     ss = warp_sum(ss);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
-    __syncthreads();
     float tot = 0.f;
-    #pragma unroll
-    for (int i = 0; i < 16; ++i) tot += red[i];
+    if constexpr (C == 1) {
+        __syncthreads();
+        #pragma unroll
+        for (int i = 0; i < kWarps; ++i) tot += red[i];
+    } else {
+        cg::cluster_group cluster = cg::this_cluster();
+        cluster.sync();
+        #pragma unroll
+        for (int c = 0; c < C; ++c) {
+            const float* rr = cluster.map_shared_rank(red, c);
+            #pragma unroll
+            for (int i = 0; i < kWarps; ++i) tot += rr[i];
+        }
+        cluster.sync();                                                  // no CTA leaves while a peer CTA reads its red[]
+    }
     const float rs = rsqrtf(tot / (float)hidden + eps);
     #pragma unroll
-    for (int it = 0; it < kMaxIter; ++it) {
-        const int i = threadIdx.x + it * 512;
+    for (int it = 0; it < kNormMaxIter; ++it) {
+        const int i = vt + it * kNormThreads;
         if (i < nvec) {
             const __half2* h = reinterpret_cast<const __half2*>(&v[it]);
             const uint4 wv = __ldg(reinterpret_cast<const uint4*>(w) + i);
@@ -64,9 +81,21 @@ add_rmsnorm_kernel(const __half* __restrict__ x, __half* __restrict__ residual, 
                 const float2 f = __half22float2(h[e]);
                 oh[e] = __hmul2_rn(wh[e], __floats2half2_rn(f.x * rs, f.y * rs));
             }
-            *reinterpret_cast<uint4*>(out + (int64_t)row * hidden + i * 8) = o;
+            *reinterpret_cast<uint4*>(out + i * 8) = o;
         }
     }
+}
+
+// One CTA per row; ADD: the addend is x (fp16, [rows, hidden]).
+template <bool ADD>
+__global__ void __launch_bounds__(kNormThreads)
+add_rmsnorm_kernel(const __half* __restrict__ x, __half* __restrict__ residual, const __half* __restrict__ w,
+                   __half* __restrict__ out, int hidden, float eps)
+{
+    const int row = blockIdx.x;
+    const int64_t row_off = (int64_t)row * hidden;
+    add_rmsnorm_row<1, ADD>([&](int i) { return __ldg(reinterpret_cast<const uint4*>(x + row_off) + i); },
+                            residual + row_off, w, out + row_off, hidden, eps, threadIdx.x);
 }
 
 // qkv [B, (H + 2*Hkv) * 128] -> q [B,H,128], k [B,Hkv,128] (both rotated), v [B,Hkv,128]
@@ -110,6 +139,13 @@ silu_mul_kernel(const __half* __restrict__ gu, __half* __restrict__ out, int I)
     *reinterpret_cast<__half2*>(out + (int64_t)row * I + i) = __hmul2_rn(a, u);
 }
 
+// Whether the candidate (ov, oi) replaces (best, bi) when two argmax results merge: the larger value, the lower index among
+// equal values, and a NaN beats every number (the lower index among NaNs), like torch.argmax.
+__device__ __forceinline__ bool argmax_takes(float ov, int oi, float best, int bi)
+{
+    return (ov != ov) ? (!(best != best) || oi < bi) : (!(best != best) && (ov > best || (ov == best && oi < bi)));
+}
+
 // ------------------------------------------------------------------------------------------------
 // Greedy sampling fused with its collective.  One block per sequence: argmax over the vocabulary (first index among equal
 // maxima, like torch.argmax), then thread 0 stores the id into this rank's slot of EVERY rank's token buffer -- plain stores
@@ -138,8 +174,7 @@ greedy_exchange_kernel(const float* __restrict__ logits, int V, long long* __res
     for (int o = 16; o >= 1; o >>= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        const bool take = (ov != ov) ? (!(best != best) || oi < bi) : (!(best != best) && (ov > best || (ov == best && oi < bi)));
-        if (take) { best = ov; bi = oi; }
+        if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
     if ((tid & 31) == 0) { smax[tid >> 5] = best; sidx[tid >> 5] = bi; }
     __syncthreads();
@@ -147,8 +182,7 @@ greedy_exchange_kernel(const float* __restrict__ logits, int V, long long* __res
         for (int w = 1; w < 8; ++w) {
             const float ov = smax[w];
             const int oi = sidx[w];
-            const bool take = (ov != ov) ? (!(best != best) || oi < bi) : (!(best != best) && (ov > best || (ov == best && oi < bi)));
-            if (take) { best = ov; bi = oi; }
+            if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
         }
         const long long tok = bi;
         next_local[b] = tok;
@@ -177,23 +211,20 @@ greedy_exchange_kernel(const float* __restrict__ logits, int V, long long* __res
 // ------------------------------------------------------------------------------------------------
 // Tensor-parallel residual-add + RMSNorm: the all-reduce of the o_proj / down_proj partial sums fused into the norm that
 // consumes them.  Every rank reads the `world` partials of this call straight from the peers' symmetric buffers (layout in
-// include/kivi_b200.h), sums them in fp32 in rank order, rounds to fp16 and continues exactly like add_rmsnorm_kernel<true>.
+// include/kivi_b200.h), sums them in fp32 in rank order, rounds to fp16 and runs add_rmsnorm_row on that addend, the body of
+// add_rmsnorm_kernel<true>: every rank gets the bits add_rmsnorm gives for the rank-order sum.
 //
-// A row is split over a cluster of C CTAs of 512 / C threads.  CTA c of the cluster plays threads [c * 512 / C, (c+1) * 512 / C)
-// of the one-CTA kernel: the same elements per thread, the same per-thread / per-warp partial sums of squares, and the 16
-// warp sums are added in the same order after a DSMEM gather -- so every C gives the bits of add_rmsnorm_kernel, and C only
-// decides how many SMs issue the N * hidden * 2 bytes of peer loads of a row.
+// A row is split over a cluster of C CTAs of 512 / C threads: CTA c of the cluster plays threads [c * 512 / C, (c+1) * 512 / C)
+// of the one-CTA kernel, so C only decides how many SMs issue the N * hidden * 2 bytes of peer loads of a row.
 // ------------------------------------------------------------------------------------------------
 template <int C>
-__global__ void __launch_bounds__(512 / C, 1)
+__global__ void __launch_bounds__(kNormThreads / C, 1)
 allreduce_add_rmsnorm_kernel(const __half* const* __restrict__ peer, __half* __restrict__ residual, const __half* __restrict__ w,
                              __half* __restrict__ out, int hidden, float eps, int rank, int world, long long slot_off,
                              long long counters_off, const long long* __restrict__ epoch_ptr, int call, int* __restrict__ err)
 {
-    constexpr int kThreads = 512 / C, kWarps = kThreads / 32, kMaxIter = 4;
-    __shared__ float red[kWarps];
     const int row = blockIdx.x / C, crank = blockIdx.x % C;
-    const int vt = crank * kThreads + threadIdx.x;                       // the thread of the one-CTA kernel this one plays
+    const int vt = crank * (kNormThreads / C) + threadIdx.x;            // the thread of the one-CTA kernel this one plays
     const unsigned long long epoch = (unsigned long long)(*epoch_ptr + call + 1);
     if (blockIdx.x == 0 && threadIdx.x < world) {                        // this rank's partial of the call is written: arrive
         unsigned long long* a = reinterpret_cast<unsigned long long*>(
@@ -214,76 +245,29 @@ allreduce_add_rmsnorm_kernel(const __half* const* __restrict__ peer, __half* __r
     }
     __syncthreads();                                                     // the acquires above order every thread's reads below
 
-    const int nvec = hidden / 8;
-    const long long row_off = slot_off / 2 + (long long)row * hidden;    // in halves, from the start of a rank's buffer
-    __half* r = residual + (int64_t)row * hidden;
-    uint4 v[kMaxIter];
-    float ss = 0.f;
-    #pragma unroll
-    for (int it = 0; it < kMaxIter; ++it) {
-        const int i = vt + it * 512;
-        if (i < nvec) {
-            uint4 pv[8];                                                 // all peer loads in flight before the first add
-            #pragma unroll
-            for (int p = 0; p < 8; ++p)
-                if (p < world) pv[p] = __ldcg(reinterpret_cast<const uint4*>(peer[p] + row_off) + i);
-            float2 acc[4];
-            #pragma unroll
-            for (int e = 0; e < 4; ++e) acc[e] = __half22float2(reinterpret_cast<const __half2*>(&pv[0])[e]);
-            #pragma unroll
-            for (int p = 1; p < 8; ++p) {
-                if (p < world) {
-                    const __half2* ph = reinterpret_cast<const __half2*>(&pv[p]);
-                    #pragma unroll
-                    for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(ph[e]); acc[e].x += f.x; acc[e].y += f.y; }
-                }
-            }
-            uint4 u = *reinterpret_cast<const uint4*>(r + i * 8);
-            __half2* h = reinterpret_cast<__half2*>(&u);
-            #pragma unroll
-            for (int e = 0; e < 4; ++e) h[e] = __hadd2_rn(h[e], __floats2half2_rn(acc[e].x, acc[e].y));
-            *reinterpret_cast<uint4*>(r + i * 8) = u;
-            #pragma unroll
-            for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(h[e]); ss = fmaf(f.x, f.x, fmaf(f.y, f.y, ss)); }
-            v[it] = u;
-        }
-    }
-    ss = warp_sum(ss);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
-    float tot = 0.f;
-    if constexpr (C == 1) {
-        __syncthreads();
+    const long long slice_off = slot_off / 2 + (long long)row * hidden;  // in halves, from the start of a rank's buffer
+    const int64_t row_off = (int64_t)row * hidden;
+    add_rmsnorm_row<C, true>([&](int i) {
+        uint4 pv[8];                                                     // all peer loads in flight before the first add
         #pragma unroll
-        for (int i = 0; i < 16; ++i) tot += red[i];
-    } else {
-        cg::cluster_group cluster = cg::this_cluster();
-        cluster.sync();
+        for (int p = 0; p < 8; ++p)
+            if (p < world) pv[p] = __ldcg(reinterpret_cast<const uint4*>(peer[p] + slice_off) + i);
+        float2 acc[4];
         #pragma unroll
-        for (int c = 0; c < C; ++c) {
-            const float* rr = cluster.map_shared_rank(red, c);
-            #pragma unroll
-            for (int i = 0; i < kWarps; ++i) tot += rr[i];
-        }
-        cluster.sync();                                                  // no CTA leaves while a peer CTA reads its red[]
-    }
-    const float rs = rsqrtf(tot / (float)hidden + eps);
-    #pragma unroll
-    for (int it = 0; it < kMaxIter; ++it) {
-        const int i = vt + it * 512;
-        if (i < nvec) {
-            const __half2* h = reinterpret_cast<const __half2*>(&v[it]);
-            const uint4 wv = __ldg(reinterpret_cast<const uint4*>(w) + i);
-            const __half2* wh = reinterpret_cast<const __half2*>(&wv);
-            uint4 o;
-            __half2* oh = reinterpret_cast<__half2*>(&o);
-            #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h[e]);
-                oh[e] = __hmul2_rn(wh[e], __floats2half2_rn(f.x * rs, f.y * rs));
+        for (int e = 0; e < 4; ++e) acc[e] = __half22float2(reinterpret_cast<const __half2*>(&pv[0])[e]);
+        #pragma unroll
+        for (int p = 1; p < 8; ++p) {
+            if (p < world) {
+                const __half2* ph = reinterpret_cast<const __half2*>(&pv[p]);
+                #pragma unroll
+                for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(ph[e]); acc[e].x += f.x; acc[e].y += f.y; }
             }
-            *reinterpret_cast<uint4*>(out + (int64_t)row * hidden + i * 8) = o;
         }
-    }
+        uint4 a;
+        #pragma unroll
+        for (int e = 0; e < 4; ++e) reinterpret_cast<__half2*>(&a)[e] = __floats2half2_rn(acc[e].x, acc[e].y);
+        return a;
+    }, residual + row_off, w, out + row_off, hidden, eps, vt);
 }
 
 }  // namespace kivi
@@ -292,35 +276,20 @@ using namespace kivi;
 
 static bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
 
-template <int C>
-static cudaError_t launch_allreduce_add_rmsnorm(int rows, cudaStream_t st, const __half* const* peer, __half* residual,
-                                                const __half* w, __half* out, int hidden, float eps, int rank, int world,
-                                                long long slot_off, long long counters_off, const long long* epoch, int call,
-                                                int* err)
+// the checks both residual-add + RMSNorm entry points begin with
+static int check_rmsnorm_args(const void* residual, const void* weight, const void* out, int rows, int hidden)
 {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(rows * C);
-    cfg.blockDim = dim3(512 / C);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = C > 1 ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, allreduce_add_rmsnorm_kernel<C>, peer, residual, w, out, hidden, eps, rank, world,
-                              slot_off, counters_off, epoch, call, err);
+    if (!residual || !weight || !out) return KIVI_ERR_NULL;
+    if (rows < 0 || hidden <= 0 || hidden % 8 != 0 || hidden > kNormMaxHidden) return KIVI_ERR_SHAPE;
+    return KIVI_OK;
 }
-
 
 extern "C" int kivi_allreduce_add_rmsnorm_f16(const void* x, void* residual, const void* weight, void* out,
                                               int rows, int hidden, float eps,
                                               const void* peer_buffers, int rank, int world, int rows_max, int call,
                                               const void* epoch, void* err, int cluster, void* stream)
 {
-    if (!residual || !weight || !out) return KIVI_ERR_NULL;
-    if (rows < 0 || hidden <= 0 || hidden % 8 != 0 || hidden > 16384) return KIVI_ERR_SHAPE;
+    if (int e = check_rmsnorm_args(residual, weight, out, rows, hidden)) return e;
     if (world < 1 || world > 8 || rank < 0 || rank >= world) return KIVI_ERR_SHAPE;
     if (!peer_buffers) {                                                 // one rank: x is the whole sum
         if (world != 1) return KIVI_ERR_NULL;
@@ -337,23 +306,22 @@ extern "C" int kivi_allreduce_add_rmsnorm_f16(const void* x, void* residual, con
     // cluster == 0: one CTA per row, the fastest width at every rows / hidden / world measured (tools/tp_bench.py kernel,
     // ranks emulated in one GPU's memory; over NVLink the widths have not been compared)
     const int C = cluster ? cluster : 1;
-    cudaStream_t st = (cudaStream_t)stream;
-    auto peer = (const __half* const*)peer_buffers;
-    cudaError_t e;
-    switch (C) {
-        case 1: e = launch_allreduce_add_rmsnorm<1>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
-                                                    hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
-                                                    call, (int*)err); break;
-        case 2: e = launch_allreduce_add_rmsnorm<2>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
-                                                    hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
-                                                    call, (int*)err); break;
-        case 4: e = launch_allreduce_add_rmsnorm<4>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
-                                                    hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
-                                                    call, (int*)err); break;
-        default: e = launch_allreduce_add_rmsnorm<8>(rows, st, peer, (__half*)residual, (const __half*)weight, (__half*)out,
-                                                     hidden, eps, rank, world, slot_off, counters_off, (const long long*)epoch,
-                                                     call, (int*)err); break;
-    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(rows * C);
+    cfg.blockDim = dim3(kNormThreads / C);
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = C;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = C > 1 ? 1 : 0;
+    auto kernel = C == 1 ? allreduce_add_rmsnorm_kernel<1> : C == 2 ? allreduce_add_rmsnorm_kernel<2>
+                : C == 4 ? allreduce_add_rmsnorm_kernel<4> : allreduce_add_rmsnorm_kernel<8>;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, (const __half* const*)peer_buffers, (__half*)residual,
+                                             (const __half*)weight, (__half*)out, hidden, eps, rank, world, slot_off,
+                                             counters_off, (const long long*)epoch, call, (int*)err);
     if (e != cudaSuccess) return (int)e;
     return post_launch();
 }
@@ -374,8 +342,7 @@ extern "C" int kivi_greedy_sample_exchange_f32(const void* logits, int batch, in
 extern "C" int kivi_add_rmsnorm_f16(const void* x, void* residual, const void* weight, void* out,
                                     int rows, int hidden, float eps, void* stream)
 {
-    if (!residual || !weight || !out) return KIVI_ERR_NULL;
-    if (rows < 0 || hidden <= 0 || hidden % 8 != 0 || hidden > 16384) return KIVI_ERR_SHAPE;
+    if (int e = check_rmsnorm_args(residual, weight, out, rows, hidden)) return e;
     // the kernel moves 8 halves per uint4 access: a view that starts off a 16-byte boundary would fault
     if ((x && !aligned_to(x, 16)) || !aligned_to(residual, 16) || !aligned_to(weight, 16) || !aligned_to(out, 16))
         return KIVI_ERR_ALIGN;

@@ -89,6 +89,20 @@ def gather_tokens(local_tokens: torch.Tensor, out: torch.Tensor | None = None) -
     return out
 
 
+def _symmetric_buffer(words: int, device):
+    """This rank's `words` int64 of one symmetric allocation (torch.distributed._symmetric_memory: peer-mapped over NVLink /
+    NVSwitch), zeroed on every rank before any returns, so no rank's kernel signals into a buffer that is still being zeroed.
+    Returns (buffer, rendezvous handle, int64 device tensor of every rank's buffer address in rank order)."""
+    import torch.distributed._symmetric_memory as symm
+    buf = symm.empty(words, dtype=torch.int64, device=device)
+    buf.zero_()
+    handle = symm.rendezvous(buf, dist.group.WORLD)
+    ptrs = torch.tensor([int(p) for p in handle.buffer_ptrs], dtype=torch.int64, device=device)
+    torch.cuda.synchronize(device)
+    dist.barrier()
+    return buf, handle, ptrs
+
+
 class PeerTokenExchange:
     """The token exchange of greedy data-parallel decoding WITHOUT a library collective: every rank owns one symmetric buffer
     (torch.distributed._symmetric_memory: peer-mapped over NVLink / NVSwitch), and the sampling kernel
@@ -97,17 +111,10 @@ class PeerTokenExchange:
     Layout per rank: int64 tokens[2][world * B] (double-buffered by step parity) + uint64 arrived[world]."""
 
     def __init__(self, batch: int, device):
-        import torch.distributed._symmetric_memory as symm
         self.world, self.rank, self.batch = dist.get_world_size(), dist.get_rank(), batch
-        n = 2 * self.world * batch + self.world
-        self.buf = symm.empty(n, dtype=torch.int64, device=device)
-        self.buf.zero_()
-        self.handle = symm.rendezvous(self.buf, dist.group.WORLD)
-        self.peer_ptrs = torch.tensor([int(p) for p in self.handle.buffer_ptrs], dtype=torch.int64, device=device)
+        self.buf, self.handle, self.peer_ptrs = _symmetric_buffer(2 * self.world * batch + self.world, device)
         self.step = torch.zeros(1, dtype=torch.int32, device=device)      # incremented inside the step, before the kernel
         self.err = torch.zeros(1, dtype=torch.int32, device=device)
-        torch.cuda.synchronize(device)
-        dist.barrier()                                                    # every rank's buffer is zeroed before anyone signals
 
     def tokens(self) -> torch.Tensor:
         """[world * B] ids of the last completed step (synchronises: reads the device step counter)."""
@@ -132,21 +139,13 @@ class PeerAllReduce:
         slot = rows_max * hidden                                          # halves per slot
         n = (2 * slot * 2 + 8 * self.world + 7) // 8                      # int64 words
         if multi:
-            import torch.distributed._symmetric_memory as symm
-            self.buf = symm.empty(n, dtype=torch.int64, device=device)
-            self.buf.zero_()
-            self.handle = symm.rendezvous(self.buf, dist.group.WORLD)
-            ptrs = [int(p) for p in self.handle.buffer_ptrs]
+            self.buf, self.handle, self.peer_ptrs = _symmetric_buffer(n, device)
         else:
             self.buf = torch.zeros(n, dtype=torch.int64, device=device)
-            ptrs = [self.buf.data_ptr()]
+            self.peer_ptrs = torch.tensor([self.buf.data_ptr()], dtype=torch.int64, device=device)
         self._slots = self.buf.view(torch.float16)[: 2 * slot].view(2, rows_max, hidden)
-        self.peer_ptrs = torch.tensor(ptrs, dtype=torch.int64, device=device)
         self.epoch = torch.zeros(1, dtype=torch.int64, device=device)     # call number = epoch + call + 1
         self.err = torch.zeros(1, dtype=torch.int32, device=device)
-        torch.cuda.synchronize(device)
-        if multi:
-            dist.barrier()                                                # every buffer is zeroed before anyone arrives
 
     def slot(self, call: int, rows: int) -> torch.Tensor:
         """[rows, hidden] fp16 view of this rank's partial-sum slot of call number `call` (what the GEMM writes)."""

@@ -37,17 +37,22 @@ def _check(name, t, dtype, shape):
         raise ValueError(f"{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
 
 
-def add_rmsnorm(x, residual, weight, out, eps: float):
-    """residual += x (x may be None); out = weight * fp16(residual * rsqrt(mean(residual^2) + eps))."""
-    _bind()
+def _check_norm(residual, weight, out, x):
+    """The operands of a residual-add + RMSNorm (x may be None); returns (rows, hidden)."""
     if residual.dim() != 2:
         raise ValueError(f"residual: expected [rows, hidden], got shape {tuple(residual.shape)}")
     rows, hidden = residual.shape
-    f16 = torch.float16
     for name, t, shape in (("residual", residual, (rows, hidden)), ("weight", weight, (hidden,)), ("out", out, (rows, hidden)),
                            ("x", x, (rows, hidden))):
         if t is not None:
-            _check(name, t, f16, shape)
+            _check(name, t, torch.float16, shape)
+    return rows, hidden
+
+
+def add_rmsnorm(x, residual, weight, out, eps: float):
+    """residual += x (x may be None); out = weight * fp16(residual * rsqrt(mean(residual^2) + eps))."""
+    _bind()
+    rows, hidden = _check_norm(residual, weight, out, x)
     _lib.check(_lib.lib().kivi_add_rmsnorm_f16(x.data_ptr() if x is not None else None, residual.data_ptr(),
                                                weight.data_ptr(), out.data_ptr(), rows, hidden, eps,
                                                _lib.stream_ptr(residual.device)), "kivi_add_rmsnorm_f16")
@@ -60,14 +65,7 @@ def allreduce_add_rmsnorm(residual, weight, out, eps: float, ar, call: int = 0, 
     in ar.slot(call, rows).  ar None: one rank, `x` is the whole sum (exactly add_rmsnorm).  cluster: CTAs per row (1, 2, 4,
     8; 0 = the library's default, one) -- the result does not depend on it."""
     _bind()
-    if residual.dim() != 2:
-        raise ValueError(f"residual: expected [rows, hidden], got shape {tuple(residual.shape)}")
-    rows, hidden = residual.shape
-    f16 = torch.float16
-    for name, t, shape in (("residual", residual, (rows, hidden)), ("weight", weight, (hidden,)), ("out", out, (rows, hidden)),
-                           ("x", x, (rows, hidden))):
-        if t is not None:
-            _check(name, t, f16, shape)
+    rows, hidden = _check_norm(residual, weight, out, x)
     if ar is not None:
         if ar.hidden != hidden or rows > ar.rows_max:
             raise ValueError(f"the all-reduce buffer holds [{ar.rows_max}, {ar.hidden}] rows, got [{rows}, {hidden}]")

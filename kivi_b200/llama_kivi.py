@@ -703,7 +703,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             pasts = [(self.cache, i) for i in range(len(self.model.layers))]
             h, _ = self._run_layers(self._ids, self._pos, pasts)
             self._logits.copy_(self.lm_head(h[:, 0]).float())
-        self.cache_advance_device()
+        self.cache._enqueue_advance()                        # decode_step advances the host mirror after each replay
         self._pos.add_(1)
         # greedy sampling inside the step (and inside its CUDA graph): the argmax of a sequence needs only that
         # sequence's logits, so with data-parallel replicas the exchange is the sampled ids, 8 B per sequence
@@ -784,34 +784,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def _step_body_fast(self):
         """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split,
-        fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels."""
-        if self.tensor_parallel:
-            return self._step_body_tp()
-        from . import glue
-        f = self._ensure_fast()
-        cfg, cache = self.config, self.cache
-        cos_t, sin_t = self._tables(cache.device)
-        eps = cfg.rms_norm_eps
-        layers = self.model.layers
-        f.res.copy_(self.model.embed_tokens(self._ids)[:, 0])
-        glue.add_rmsnorm(None, f.res, layers[0].input_layernorm.weight, f.h, eps)
-        for i, l in enumerate(layers):
-            torch.mm(f.h, f.wqkv[i], out=f.qkv)
-            glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
-            cache.decode_attention(i, f.q, f.k, f.v, out=f.attn)
-            torch.mm(f.attn.view(f.B, -1), f.wo[i], out=f.o)
-            glue.add_rmsnorm(f.o, f.res, l.post_attention_layernorm.weight, f.h, eps)
-            torch.mm(f.h, f.wgu[i], out=f.gu)
-            glue.silu_mul(f.gu, f.act)
-            torch.mm(f.act, l.mlp.down_proj.weight.t(), out=f.d)
-            nxt = layers[i + 1].input_layernorm.weight if i + 1 < len(layers) else self.model.norm.weight
-            glue.add_rmsnorm(f.d, f.res, nxt, f.h, eps)
-        torch.mm(f.h, self.lm_head.weight.t(), out=f.logits16)
-        self._logits.copy_(f.logits16)                                       # logits.float() (:881)
-
-    def _step_body_tp(self):
-        """The decode step of one tensor-parallel rank: the same launches on this rank's heads and channels, but o_proj and
-        down_proj write their partial sums into the PeerAllReduce slots, and the two residual-add + RMSNorm kernels of a
+        fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels.
+        Tensor-parallel (self._allreduce is a PeerAllReduce): the same launches on this rank's heads and channels, but o_proj
+        and down_proj write their partial sums into the PeerAllReduce slots, and the two residual-add + RMSNorm kernels of a
         layer become kivi_allreduce_add_rmsnorm_f16 (calls 2i and 2i + 1 of the step), which add up every rank's partials.
         The embedding's RMSNorm and lm_head are replicated: every rank computes the same logits."""
         from . import glue
@@ -820,22 +795,33 @@ class LlamaForCausalLM_KIVI(nn.Module):
         cos_t, sin_t = self._tables(cache.device)
         eps = cfg.rms_norm_eps
         layers = self.model.layers
+
+        def partial(call):                      # where o_proj (call 2i of the step) or down_proj (2i + 1) writes
+            return (f.o, f.d)[call & 1] if ar is None else ar.slot(call, f.B)
+
+        def add_rmsnorm(call, weight):          # f.res += the sum of the call's partials; f.h = RMSNorm(f.res) * weight
+            if ar is None:
+                glue.add_rmsnorm(partial(call), f.res, weight, f.h, eps)
+            else:
+                glue.allreduce_add_rmsnorm(f.res, weight, f.h, eps, ar, call=call)
+
         f.res.copy_(self.model.embed_tokens(self._ids)[:, 0])
         glue.add_rmsnorm(None, f.res, layers[0].input_layernorm.weight, f.h, eps)
         for i, l in enumerate(layers):
             torch.mm(f.h, f.wqkv[i], out=f.qkv)
             glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
             cache.decode_attention(i, f.q, f.k, f.v, out=f.attn)
-            torch.mm(f.attn.view(f.B, -1), f.wo[i], out=ar.slot(2 * i, f.B))
-            glue.allreduce_add_rmsnorm(f.res, l.post_attention_layernorm.weight, f.h, eps, ar, call=2 * i)
+            torch.mm(f.attn.view(f.B, -1), f.wo[i], out=partial(2 * i))
+            add_rmsnorm(2 * i, l.post_attention_layernorm.weight)
             torch.mm(f.h, f.wgu[i], out=f.gu)
             glue.silu_mul(f.gu, f.act)
-            torch.mm(f.act, l.mlp.down_proj.weight.t(), out=ar.slot(2 * i + 1, f.B))
+            torch.mm(f.act, l.mlp.down_proj.weight.t(), out=partial(2 * i + 1))
             nxt = layers[i + 1].input_layernorm.weight if i + 1 < len(layers) else self.model.norm.weight
-            glue.allreduce_add_rmsnorm(f.res, nxt, f.h, eps, ar, call=2 * i + 1)
-        ar.epoch.add_(2 * len(layers))                                       # the next step's calls continue the count
+            add_rmsnorm(2 * i + 1, nxt)
+        if ar is not None:
+            ar.epoch.add_(2 * len(layers))                                   # the next step's calls continue the count
         torch.mm(f.h, self.lm_head.weight.t(), out=f.logits16)
-        self._logits.copy_(f.logits16)
+        self._logits.copy_(f.logits16)                                       # logits.float() (:881)
 
     def first_tokens(self, logits):
         """Greedy ids of prompt logits (prefill / insert) -- under tensor parallelism rank 0's, broadcast, so the ranks can
@@ -845,13 +831,6 @@ class LlamaForCausalLM_KIVI(nn.Module):
             import torch.distributed as dist
             dist.broadcast(tok, src=0)
         return tok
-
-    def cache_advance_device(self):
-        from . import _lib
-        import ctypes
-        with torch.cuda.device(self.cache.device):
-            _lib.check(_lib.lib().kivi_cache_advance(ctypes.byref(self.cache._structs[0]),
-                                                     _lib.stream_ptr(self.cache.device)), "kivi_cache_advance")
 
     @torch.no_grad()
     def decode_step(self, input_ids=None, use_graph: bool = True):
