@@ -331,6 +331,35 @@ int kivi_silu_mul_f16(const void* gate_up, void* out, int rows, int intermediate
 int kivi_greedy_sample_exchange_f32(const void* logits, int batch, int vocab, void* next_local, void* ids_feedback,
                                     const void* peer_buffers, int rank, int world, const void* step, void* err, void* stream);
 
+/* Sampling: next_local[b] = one draw from row b of logits (fp32 [batch, vocab]) after temperature, top-k and top-p, applied in
+ * the order of HF's logits warpers.  One launch, no sort, no scratch buffer.  All per-row parameters are DEVICE arrays [batch],
+ * read by the kernel, so a captured call keeps working when the caller changes a row's parameters between replays.
+ *   temperature[b] == 0 : the row is greedy: exactly the id of kivi_greedy_sample_exchange_f32 (first index among equal maxima, a
+ *                         NaN wins); draw[b] does not change.  (A negative or NaN temperature is the caller's error.  The values live on the
+ *                         device, so neither this entry point nor its ctypes wrapper can see them without a synchronisation;
+ *                         kivi_b200's set_sampling / generate / serve validate them on the host before they are uploaded.
+ *                         The kernel takes such a row as greedy rather than dividing by it.)
+ *   otherwise             x_v = logits[b, v] / temperature[b] in fp32; a NaN logit counts as -inf.
+ *   top_k[b] = k        : k <= 0 or k >= vocab: off.  Else keep every v with x_v >= the k-th largest x of the row (ties at the
+ *                         threshold are all kept, as TopKLogitsWarper does).
+ *   top_p[b] = p        : p >= 1: off.  Else, over the softmax of what top-k kept, keep the smallest set of highest-probability
+ *                         tokens whose mass reaches p; p <= 0 keeps the maximum only.  Tokens of EQUAL logit stand or fall
+ *                         together (TopPLogitsWarper drops part of a tie by sort order; here the whole tie is kept).
+ *   draw                : u = (Philox4x32-10(key = seed[b], counter = (draw[b], 0)).x >> 8) * 2^-24, in [0, 1).  The id is the
+ *                         first kept token, in ASCENDING TOKEN-ID order, whose cumulative kept mass exceeds u * S (S = the kept
+ *                         mass) -- not torch.multinomial's order, and a pure function of (row, parameters, seed[b], draw[b]):
+ *                         the batch size, the row's index and the run do not matter.  Then draw[b] += 1.
+ * Tokens at -inf are never kept and never counted; at least one token is kept.  A row with a +inf among its scaled logits, or
+ * with no finite logit, gets the greedy id and does not consume a draw.
+ * Masses are exp(x_v - max_v x_v) rounded to multiples of 2^-40 and summed, compared and walked as integers; a token whose mass
+ * rounds to 0 can be kept but cannot be drawn.
+ * ids_feedback (may be NULL) receives the same ids (the next step's input buffer), next_local / ids_feedback are int64 [batch].
+ * dbg_u / dbg_kept (NULL, or [batch]; tests): u and the number of kept tokens (0 and 1 for a row that took the greedy id).
+ * Requirements: batch >= 0, 1 <= vocab <= 2^22; argument errors return KIVI_ERR_* before any launch.  Graph-capturable. */
+int kivi_sample_f32(const void* logits, int batch, int vocab, const float* temperature, const int32_t* top_k, const float* top_p,
+                    const uint64_t* seed, uint64_t* draw, void* next_local, void* ids_feedback, float* dbg_u, int32_t* dbg_kept,
+                    void* stream);
+
 /* Tensor-parallel residual-add + RMSNorm: the all-reduce after o_proj / down_proj fused into the norm that follows it.
  * With the rows of the attention heads and of the MLP columns sharded over `world` ranks, rank p holds a partial sum
  * partial_p [rows, hidden] fp16 of the projection.  Every rank computes the same bits:

@@ -6,6 +6,8 @@
 
 #include <cooperative_groups.h>
 
+#include <type_traits>
+
 namespace cg = cooperative_groups;
 
 namespace kivi {
@@ -209,6 +211,327 @@ greedy_exchange_kernel(const float* __restrict__ logits, int V, long long* __res
 }
 
 // ------------------------------------------------------------------------------------------------
+// Sampling (temperature -> top-k -> top-p -> one draw), semantics in include/kivi_b200.h.  One CTA per row, no sort: both
+// thresholds are selections by histogram (sample_select), exact in the order-preserving 32-bit key of the scaled logit.
+// Every sum the result depends on is an integer sum -- token counts, and exp(x - max) as 40-bit fixed point in a
+// uint64 -- so neither the order of the shared-memory atomics nor the row's place in the batch can change a bit of it.
+// STAGED: the scaled row is kept in shared memory after the first pass; otherwise every pass re-reads it (from L2).
+// ------------------------------------------------------------------------------------------------
+constexpr int kSampleThreads = 1024, kSampleWarps = kSampleThreads / 32;
+constexpr int kSampleBins = 2048;                                        // two bins per thread
+constexpr int kSampleStageMax = 50 * 1024;                               // tokens: 200 KB of the SM's 227 KB, the rest is below
+constexpr int kSampleCand = 2048;                                        // listed tokens of a selection's chosen bucket
+constexpr uint32_t kSampleKeyFinite = 0x00800000u;                       // the smallest key above that of -inf
+constexpr int kSampleMaxVocab = 1 << 22;                                 // 2^22 masses of at most 2^40 fit a uint64
+
+struct SampleShared {
+    unsigned long long hist[kSampleBins];
+    unsigned long long warp_sum[kSampleWarps];                           // block reductions; the segment masses of the walk
+    int warp_cnt[kSampleWarps];
+    float warp_max[kSampleWarps], warp_xmax[kSampleWarps];
+    int warp_idx[kSampleWarps];
+    int cand[kSampleCand];
+    int cand_n;
+    unsigned long long pick_above;
+    uint32_t pick_digit;
+    float xmax;
+    int greedy_id;
+};
+
+// x ascending <=> key ascending, for x without NaN and without -0
+__device__ __forceinline__ uint32_t sample_key(float x)
+{
+    const uint32_t b = __float_as_uint(x);
+    return b ^ ((b >> 31) ? 0xffffffffu : 0x80000000u);
+}
+
+// logit / temperature; a NaN becomes -inf (never sampled) and -0 becomes +0 (equal logits have equal keys)
+__device__ __forceinline__ float sample_scaled(float logit, float temperature)
+{
+    const float x = logit / temperature;
+    return (x != x) ? -INFINITY : (x == 0.f ? 0.f : x);
+}
+
+// exp(x - max) in units of 2^-40: at most 2^40, and 0 for x = -inf
+__device__ __forceinline__ unsigned long long sample_mass(float x, float xmax)
+{
+    return __float2ull_rn(expf(x - xmax) * 1099511627776.f);
+}
+
+// first word of Philox4x32-10 with key (key.lo, key.hi) and counter (counter.lo, counter.hi, 0, 0)
+__device__ __forceinline__ uint32_t philox4x32_10(unsigned long long key, unsigned long long counter)
+{
+    uint32_t c0 = (uint32_t)counter, c1 = (uint32_t)(counter >> 32), c2 = 0, c3 = 0;
+    uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
+    #pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t h0 = __umulhi(0xD2511F53u, c0), l0 = 0xD2511F53u * c0;
+        const uint32_t h1 = __umulhi(0xCD9E8D57u, c2), l1 = 0xCD9E8D57u * c2;
+        const uint32_t n0 = h1 ^ c1 ^ k0, n2 = h0 ^ c3 ^ k1;
+        c0 = n0; c1 = l1; c2 = n2; c3 = l0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    return c0;
+}
+
+// Bin of a scaled logit in the first level of a selection: linear in x, 1/64 wide, over the 32 units below the row's maximum
+// (2047 = the maximum's bin, 0 = everything lower, -inf included).  Monotone in x, so it orders tokens as their keys do, and
+// unlike the key's leading bits (sign, exponent) it spreads a row of logits over many bins.
+__device__ __forceinline__ int sample_bucket(float x, float xmax)
+{
+    const float d = (xmax - x) * 64.f;
+    return d < 2047.f ? 2047 - (int)d : 0;
+}
+
+// The bin d with  above + hist[d+1 ..] < target <= above + hist[d ..]  into s.pick_digit, and the weight above it into
+// s.pick_above: a suffix sum over the bins, two per thread.  Called by all threads, after a barrier that follows the last add.
+// The callers' targets never exceed above + the histogram's total, so exactly one thread writes the pick: it is written
+// between this function's two barriers and read after the second, and nothing else ever writes it.
+template <class Bin>
+__device__ __forceinline__ void sample_find_bin(unsigned long long above, unsigned long long target, SampleShared& s)
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const Bin* hist = reinterpret_cast<const Bin*>(s.hist);
+    const unsigned long long h0 = hist[2 * tid], h1 = hist[2 * tid + 1];
+    unsigned long long v = h0 + h1;
+    #pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_down_sync(0xffffffffu, v, o);
+        if (lane + o < 32) v += y;
+    }
+    if (lane == 0) s.warp_sum[warp] = v;
+    __syncthreads();
+    unsigned long long a = above + v - (h0 + h1);                        // weight above bin 2 * tid + 1
+    for (int w = warp + 1; w < kSampleWarps; ++w) a += s.warp_sum[w];
+    if (a < target && target <= a + h1) { s.pick_digit = 2 * tid + 1; s.pick_above = a; }
+    else if (a + h1 < target && target <= a + h1 + h0) { s.pick_digit = 2 * tid; s.pick_above = a + h1; }
+    __syncthreads();
+}
+
+// The largest key t for which the tokens with key >= max(t, floor) weigh at least `target`; a token weighs its mass (MASS,
+// uint64 bins) or 1 (uint32 bins: native shared-memory adds).  x(i) is the scaled logit of token i.  Four levels of 2048
+// bins: sample_bucket, then the 11 + 11 + 10 bits of the key among the tokens of the chosen bucket.
+// Level 0 reads the row and adds with plain atomics, except into bin 0, which a cold or masked row fills: those lanes add
+// once per warp.  Level 1 reads the row again and lists the chosen bucket's tokens in s.cand (in any order: every sum over
+// them is an integer sum); levels 2 and 3 read that list -- a few dozen tokens -- or the row once more when the bucket
+// holds more than the list does.  From level 1 on the tokens share the key's leading bits, so lanes that hit the same bin
+// add once.
+template <bool MASS, class X>
+__device__ __noinline__ uint32_t sample_select(X x, int V, uint32_t floor, float xmax, unsigned long long target,
+                                               SampleShared& s)
+{
+    using Bin = typename std::conditional<MASS, unsigned long long, uint32_t>::type;
+    Bin* hist = reinterpret_cast<Bin*>(s.hist);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint32_t prefix = 0;
+    int bucket = 0;
+    unsigned long long above = 0;                                        // weight of the tokens above the current bin's range
+    #pragma unroll 1
+    for (int level = 0; level < 4; ++level) {
+        const int shift = level == 1 ? 21 : level == 2 ? 10 : 0;
+        const uint32_t digits = level == 3 ? 1023u : 2047u;
+        const uint32_t known = level <= 1 ? 0u : level == 2 ? 0xffe00000u : 0xfffffc00u;
+        hist[2 * tid] = 0;
+        hist[2 * tid + 1] = 0;
+        if (level == 0 && tid == 0) s.cand_n = 0;
+        const bool listed = level >= 2 && s.cand_n <= kSampleCand;       // written during level 1, two barriers ago
+        const int n = listed ? s.cand_n : V;
+        __syncthreads();
+        for (int base = warp * 32; base < n; base += kSampleThreads) {
+            const int j = base + lane;
+            float xi = 0.f;
+            uint32_t key = 0;
+            int bk = -1, i = j;
+            bool active = j < n;
+            if (active) {
+                if (listed) i = s.cand[j];
+                xi = x(i);
+                key = sample_key(xi);
+                if (!listed) bk = sample_bucket(xi, xmax);
+                active = (listed || (key >= floor && (level == 0 || bk == bucket))) && (key & known) == prefix;
+            }
+            if (level == 0) {
+                Bin w = 1;
+                if (MASS && active) w = sample_mass(xi, xmax);
+                const uint32_t low = __ballot_sync(0xffffffffu, active && bk == 0);
+                if (active && bk == 0) {
+                    if (MASS) w = ((unsigned long long)__reduce_add_sync(low, (uint32_t)((unsigned long long)w >> 20)) << 20)
+                                  + __reduce_add_sync(low, (uint32_t)w & 0xfffffu);
+                    else w = __popc(low);
+                    if (lane == __ffs(low) - 1) atomicAdd(&hist[0], w);
+                } else if (active) {
+                    atomicAdd(&hist[bk], w);
+                }
+                continue;
+            }
+            const uint32_t live = __ballot_sync(0xffffffffu, active);
+            if (!live) continue;
+            if (level == 1) {                                            // list the bucket: one counter add per warp
+                int at = 0;
+                if (lane == __ffs(live) - 1) at = atomicAdd(&s.cand_n, __popc(live));
+                at = __shfl_sync(0xffffffffu, at, __ffs(live) - 1) + __popc(live & ((1u << lane) - 1));
+                if (active && at < kSampleCand) s.cand[at] = i;
+            }
+            const uint32_t bin = active ? ((key >> shift) & digits) : 0xffffffffu;
+            const uint32_t peers = __match_any_sync(0xffffffffu, bin);
+            if (active) {
+                Bin w;
+                if (MASS) {
+                    const unsigned long long q = sample_mass(xi, xmax);
+                    w = ((unsigned long long)__reduce_add_sync(peers, (uint32_t)(q >> 20)) << 20)
+                        + __reduce_add_sync(peers, (uint32_t)q & 0xfffffu);
+                } else {
+                    w = __popc(peers);
+                }
+                if (lane == __ffs(peers) - 1) atomicAdd(&hist[bin], w);
+            }
+        }
+        __syncthreads();
+        sample_find_bin<Bin>(above, target, s);
+        if (level == 0) bucket = s.pick_digit;
+        else prefix |= s.pick_digit << shift;
+        above = s.pick_above;
+    }
+    return prefix;
+}
+
+// Mass and number of the tokens with key >= floor, per warp segment: warp w owns the tokens [w * seg, (w + 1) * seg).
+// Returns the total mass; s.warp_sum / s.warp_cnt hold the segments'.
+template <class X>
+__device__ __noinline__ unsigned long long sample_segments(X x, int V, int seg, uint32_t floor, float xmax, SampleShared& s)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long m = 0;
+    int n = 0;
+    const int end = min(V, (warp + 1) * seg);
+    for (int i = warp * seg + lane; i < end; i += 32) {
+        const float xi = x(i);
+        if (sample_key(xi) >= floor) { m += sample_mass(xi, xmax); ++n; }
+    }
+    #pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); n += __shfl_xor_sync(0xffffffffu, n, o); }
+    __syncthreads();                                                     // the previous reader of warp_sum is done
+    if (lane == 0) { s.warp_sum[warp] = m; s.warp_cnt[warp] = n; }
+    __syncthreads();
+    unsigned long long tot = 0;
+    for (int w = 0; w < kSampleWarps; ++w) tot += s.warp_sum[w];
+    return tot;
+}
+
+template <bool STAGED>
+__global__ void __launch_bounds__(kSampleThreads, 1)
+sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__ temperature, const int* __restrict__ top_k,
+              const float* __restrict__ top_p, const unsigned long long* __restrict__ seed, unsigned long long* __restrict__ draw,
+              long long* __restrict__ next_local, long long* __restrict__ ids_feedback, float* __restrict__ dbg_u,
+              int* __restrict__ dbg_kept)
+{
+    extern __shared__ float sx[];                                        // STAGED: the scaled row
+    __shared__ SampleShared s;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float* row = logits + (long long)b * V;
+    const float T = temperature[b];
+    const bool sampled = T > 0.f;
+
+    // pass 0: the greedy id (the rule of greedy_exchange_kernel) and the maximum of the scaled row
+    float best = -INFINITY, xmax = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = tid; i < V; i += kSampleThreads) {
+        const float v = __ldg(row + i);
+        if (argmax_takes(v, i, best, bi)) { best = v; bi = i; }
+        if (sampled) {
+            const float xi = sample_scaled(v, T);
+            if (STAGED) sx[i] = xi;
+            xmax = fmaxf(xmax, xi);
+        }
+    }
+    #pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
+        xmax = fmaxf(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
+    }
+    if (lane == 0) { s.warp_max[warp] = best; s.warp_idx[warp] = bi; s.warp_xmax[warp] = xmax; }
+    __syncthreads();
+    if (tid == 0) {
+        for (int w = 1; w < kSampleWarps; ++w) {
+            const float ov = s.warp_max[w];
+            const int oi = s.warp_idx[w];
+            if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
+            xmax = fmaxf(xmax, s.warp_xmax[w]);
+        }
+        s.greedy_id = bi;
+        s.xmax = xmax;
+    }
+    __syncthreads();
+    xmax = s.xmax;
+    if (!sampled || !(xmax > -INFINITY) || xmax == INFINITY) {           // greedy row; no finite logit; a +inf
+        if (tid == 0) {
+            const long long tok = s.greedy_id;
+            next_local[b] = tok;
+            if (ids_feedback) ids_feedback[b] = tok;
+            if (dbg_u) dbg_u[b] = 0.f;
+            if (dbg_kept) dbg_kept[b] = 1;
+        }
+        return;
+    }
+    auto x = [&](int i) { return STAGED ? sx[i] : sample_scaled(__ldg(row + i), T); };
+
+    uint32_t floor = kSampleKeyFinite;                                   // kept: key >= floor
+    const int k = top_k[b];
+    if (k > 0 && k < V) floor = max(floor, sample_select<false>(x, V, 0u, xmax, (unsigned long long)k, s));
+    const int seg = cdiv(cdiv(V, kSampleWarps), 32) * 32;
+    unsigned long long S = sample_segments(x, V, seg, floor, xmax, s);
+    const float p = top_p[b];
+    if (!(p >= 1.f)) {
+        unsigned long long target = 1;                                   // p <= 0: the maximum (mass 2^40) only
+        if (p > 0.f) {
+            const double t = ceil((double)p * (double)S);
+            target = t >= (double)S ? S : max((unsigned long long)t, 1ull);
+        }
+        floor = max(floor, sample_select<true>(x, V, floor, xmax, target, s));
+        S = sample_segments(x, V, seg, floor, xmax, s);
+    }
+
+    // the draw: the first kept token, in token-id order, whose cumulative mass exceeds floor(u * S)
+    const unsigned long long d = draw[b];
+    const unsigned long long n24 = philox4x32_10(seed[b], d) >> 8;
+    const unsigned long long want = (__umul64hi(n24, S) << 40) | ((n24 * S) >> 24);
+    unsigned long long run = 0;
+    int ws = 0, kept = 0;
+    for (int w = 0; w < kSampleWarps; ++w) kept += s.warp_cnt[w];
+    while (ws < kSampleWarps - 1 && run + s.warp_sum[ws] <= want) run += s.warp_sum[ws++];
+    if (warp != ws) return;
+    const int end = min(V, (ws + 1) * seg);
+    for (int base = ws * seg; base < end; base += 32) {
+        const int i = base + lane;
+        unsigned long long q = 0;
+        if (i < end) {
+            const float xi = x(i);
+            if (sample_key(xi) >= floor) q = sample_mass(xi, xmax);
+        }
+        #pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, q, o);
+            if (lane >= o) q += y;
+        }
+        const uint32_t over = __ballot_sync(0xffffffffu, run + q > want);
+        if (over) {
+            if (lane == 0) {
+                const long long tok = base + __ffs(over) - 1;
+                next_local[b] = tok;
+                if (ids_feedback) ids_feedback[b] = tok;
+                draw[b] = d + 1;
+                if (dbg_u) dbg_u[b] = (float)n24 * 5.9604644775390625e-8f;
+                if (dbg_kept) dbg_kept[b] = kept;
+            }
+            return;
+        }
+        run += __shfl_sync(0xffffffffu, q, 31);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Tensor-parallel residual-add + RMSNorm: the all-reduce of the o_proj / down_proj partial sums fused into the norm that
 // consumes them.  Every rank reads the `world` partials of this call straight from the peers' symmetric buffers (layout in
 // include/kivi_b200.h), sums them in fp32 in rank order, rounds to fp16 and runs add_rmsnorm_row on that addend, the body of
@@ -336,6 +659,30 @@ extern "C" int kivi_greedy_sample_exchange_f32(const void* logits, int batch, in
     greedy_exchange_kernel<<<batch, 256, 0, (cudaStream_t)stream>>>(
         (const float*)logits, vocab, (long long*)next_local, (long long*)ids_feedback, (long long* const*)peer_buffers,
         batch, rank, world, (const int*)step, (int*)err);
+    return post_launch();
+}
+
+extern "C" int kivi_sample_f32(const void* logits, int batch, int vocab, const float* temperature, const int32_t* top_k,
+                               const float* top_p, const uint64_t* seed, uint64_t* draw, void* next_local, void* ids_feedback,
+                               float* dbg_u, int32_t* dbg_kept, void* stream)
+{
+    if (!logits || !temperature || !top_k || !top_p || !seed || !draw || !next_local) return KIVI_ERR_NULL;
+    if (batch < 0 || vocab < 1 || vocab > kSampleMaxVocab) return KIVI_ERR_SHAPE;
+    if (batch == 0) return KIVI_OK;
+    DeviceInfo info;
+    if (int e = device_info(&info)) return e;
+    // a row that fits beside the histogram is staged in shared memory (Llama-2's 32000 tokens); a longer one (Llama-3's
+    // 128256) is re-read from L2 by every pass
+    const int row_bytes = vocab * (int)sizeof(float);
+    const bool staged = vocab <= kSampleStageMax && row_bytes + (int)sizeof(SampleShared) <= info.max_smem_optin;
+    if (staged) {
+        static std::atomic<unsigned long long> done{0};
+        if (int e = ensure_dynamic_smem(sample_kernel<true>, kSampleStageMax * (int)sizeof(float), info.ordinal, done)) return e;
+    }
+    auto kernel = staged ? sample_kernel<true> : sample_kernel<false>;
+    kernel<<<batch, kSampleThreads, staged ? row_bytes : 0, (cudaStream_t)stream>>>(
+        (const float*)logits, vocab, temperature, top_k, top_p, (const unsigned long long*)seed, (unsigned long long*)draw,
+        (long long*)next_local, (long long*)ids_feedback, dbg_u, dbg_kept);
     return post_launch();
 }
 

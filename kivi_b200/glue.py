@@ -1,5 +1,5 @@
 """ctypes wrappers of the decode-step glue kernels (csrc/kivi_model.cu): residual-add + RMSNorm,
-RoPE + q/k/v split, SiLU*mul.  fp16 CUDA tensors only; each wrapper checks device, dtype, contiguity and shapes
+RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), greedy and sampled next-token selection (fp32 logits); each wrapper checks device, dtype, contiguity and shapes
 before the call (ValueError, or RuntimeError for a CPU tensor)."""
 from __future__ import annotations
 
@@ -21,6 +21,7 @@ def _bind():
     _lib.bind("kivi_rope_split_f16", i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp])
     _lib.bind("kivi_silu_mul_f16", i32, [vp, vp, i32, i32, vp])
     _lib.bind("kivi_greedy_sample_exchange_f32", i32, [vp, i32, i32, vp, vp, vp, i32, i32, vp, vp, vp])
+    _lib.bind("kivi_sample_f32", i32, [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
     _lib.bind("kivi_allreduce_add_rmsnorm_f16", i32,
               [vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, i32, i32, i32, i32, vp, vp, i32, vp])
     _B = True
@@ -126,4 +127,33 @@ def greedy_sample(logits, next_local, ids_feedback=None, exchange=None):
         ex.peer_ptrs.data_ptr() if ex is not None else None, ex.rank if ex is not None else 0, ex.world if ex is not None else 1,
         ex.step.data_ptr() if ex is not None else None, ex.err.data_ptr() if ex is not None else None,
         _lib.stream_ptr(logits.device)), "kivi_greedy_sample_exchange_f32")
+    return next_local
+
+
+def sample(logits, temperature, top_k, top_p, seed, draw, next_local, ids_feedback=None, dbg_u=None, dbg_kept=None):
+    """next_local[b] = one draw from logits[b] (fp32 [B, vocab]) after temperature[b] (fp32), top_k[b] (int32) and top_p[b]
+    (fp32), with the uniform number Philox4x32-10(seed[b], draw[b]) (int64 tensors holding the uint64 bits); draw[b] += 1.
+    temperature[b] == 0 is the greedy id and leaves draw[b] alone.  All operands are device tensors of B elements: the kernel
+    reads them, so a captured call follows later changes.  include/kivi_b200.h (kivi_sample_f32) has the exact rules.
+    The parameter VALUES are not checked here (that would read the device and break a capture): callers validate them on the
+    host before uploading, as llama_kivi.sampling_rows does; the kernel takes a row whose temperature is not > 0 as greedy.
+    dbg_u (fp32) / dbg_kept (int32): optional outputs, the uniform number and the size of the kept set."""
+    _bind()
+    if logits.dim() != 2:
+        raise ValueError(f"logits: expected [B, vocab], got shape {tuple(logits.shape)}")
+    B, V = logits.shape
+    _check("logits", logits, torch.float32, (B, V))
+    for name, t, dtype in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32),
+                           ("top_p", top_p, torch.float32), ("seed", seed, torch.int64), ("draw", draw, torch.int64),
+                           ("next_local", next_local, torch.int64), ("ids_feedback", ids_feedback, torch.int64),
+                           ("dbg_u", dbg_u, torch.float32), ("dbg_kept", dbg_kept, torch.int32)):
+        if t is not None:
+            _check(name, t, dtype, (B,))
+            if t.device != logits.device:
+                raise ValueError(f"{name}: on {t.device}, logits on {logits.device}")
+    ptr = lambda t: t.data_ptr() if t is not None else None             # noqa: E731
+    _lib.check(_lib.lib().kivi_sample_f32(
+        logits.data_ptr(), B, V, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), seed.data_ptr(), draw.data_ptr(),
+        next_local.data_ptr(), ptr(ids_feedback), ptr(dbg_u), ptr(dbg_kept), _lib.stream_ptr(logits.device)),
+        "kivi_sample_f32")
     return next_local

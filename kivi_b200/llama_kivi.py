@@ -337,6 +337,10 @@ class _Output(tuple):
     past_key_values = property(lambda self: self[1])
 
 
+_P2P_SAMPLING = ("sampling with enable_token_allgather(mode='p2p'): the fused argmax + peer-store exchange is greedy only; "
+                 "use mode='nccl', which gathers the sampled ids")
+
+
 def _additive_mask(attention_mask, q_len: int, total: int, dtype, device):
     """HF padding mask [B, total] (1 = attend) -> additive [B, 1, q_len, total] with the causal structure, or None
     when nothing is masked; a 4-D additive mask passes through (what the reference's hook receives, :364-372)."""
@@ -353,6 +357,45 @@ def _additive_mask(attention_mask, q_len: int, total: int, dtype, device):
     else:
         keep = keep.expand(-1, 1, 1, total)
     return torch.zeros(keep.shape, dtype=dtype, device=device).masked_fill(~keep, torch.finfo(dtype).min)
+
+
+def sampling_rows(n: int, temperature=1.0, top_k=50, top_p=1.0, seed=0):
+    """The sampling parameters of n batch rows as four lists (temperature, top_k, top_p, seed), from scalars or length-n
+    sequences.  An int seed gives row b the Philox key seed + b (mod 2^64); a sequence gives row b its own key.
+    temperature >= 0 (0 = greedy), top_k an int (<= 0 = off), 0 <= top_p <= 1; anything else is a ValueError."""
+    import math
+
+    def rows(name, v, conv):
+        vals = list(v) if isinstance(v, (list, tuple)) or (torch.is_tensor(v) and v.dim() > 0) else [v] * n
+        if len(vals) != n:
+            raise ValueError(f"{name}: expected a scalar or {n} values, got {len(vals)}")
+        try:
+            return [conv(x) for x in vals]
+        except (TypeError, OverflowError) as e:
+            raise ValueError(f"{name}: {e}") from None
+
+    def integer(x):
+        if isinstance(x, bool) or int(x) != x:
+            raise ValueError(f"expected an integer, got {x!r}")
+        return int(x)
+
+    t, p = rows("temperature", temperature, float), rows("top_p", top_p, float)
+    k = rows("top_k", top_k, integer)
+    if isinstance(seed, (list, tuple)) or (torch.is_tensor(seed) and seed.dim() > 0):
+        sd = rows("seed", seed, integer)
+    else:
+        sd = [integer(seed) + b for b in range(n)]
+    for b in range(n):
+        if not (math.isfinite(t[b]) and t[b] >= 0.0):
+            raise ValueError(f"temperature: expected a finite value >= 0 (0 = greedy), got {t[b]}")
+        if not 0.0 <= p[b] <= 1.0:
+            raise ValueError(f"top_p: expected a value in [0, 1], got {p[b]}")
+        if not -2 ** 31 <= k[b] < 2 ** 31:
+            raise ValueError(f"top_k: {k[b]} is not an int32")
+        if sd[b] < 0:
+            raise ValueError(f"seed: expected a non-negative integer, got {sd[b]}")
+        sd[b] %= 2 ** 64
+    return t, k, p, sd
 
 
 class LlamaForCausalLM_KIVI(nn.Module):
@@ -387,6 +430,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._dist_in_graph = True
         self._exchange = None               # kivi_b200.dist.PeerTokenExchange: ids stored into the peers' buffers by the sampling kernel
         self._allreduce = None              # kivi_b200.dist.PeerAllReduce of the tensor-parallel decode step
+        self._sampling = False              # the step's last kernel samples (set_sampling) instead of taking the argmax
 
     # ------------------------------------------------------------------ HF-style construction
     @classmethod
@@ -612,7 +656,15 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._pos = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._ids = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._logits = torch.zeros((batch, cfg.vocab_size), dtype=torch.float32, device=dev)
-        self.next_tokens = torch.zeros((batch,), dtype=torch.long, device=dev)   # greedy argmax of the step (in-graph)
+        self.next_tokens = torch.zeros((batch,), dtype=torch.long, device=dev)   # the step's argmax or sample (in-graph)
+        # per-slot sampling parameters, read by the sampling kernel on the device (seed / draw: uint64 bits); greedy until
+        # set_sampling()
+        self._sampling = False
+        self._samp = SimpleNamespace(temperature=torch.zeros(batch, dtype=torch.float32, device=dev),
+                                     top_k=torch.zeros(batch, dtype=torch.int32, device=dev),
+                                     top_p=torch.ones(batch, dtype=torch.float32, device=dev),
+                                     seed=torch.zeros(batch, dtype=torch.long, device=dev),
+                                     draw=torch.zeros(batch, dtype=torch.long, device=dev))
         self._tables(dev)                                    # rows for every position the cache can reach
         return self.cache
 
@@ -708,11 +760,16 @@ class LlamaForCausalLM_KIVI(nn.Module):
         # greedy sampling inside the step (and inside its CUDA graph): the argmax of a sequence needs only that
         # sequence's logits, so with data-parallel replicas the exchange is the sampled ids, 8 B per sequence
         from . import glue
-        if self._exchange is not None:
-            self._exchange.step.add_(1)                      # the step number the peers' arrival counters are compared with
-        # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight into
-        # every peer's buffer over NVLink + arrival counters
-        glue.greedy_sample(self._logits, self.next_tokens, self._ids.view(-1), self._exchange)
+        if self._sampling:
+            # in the argmax kernel's place, one kernel as well: a draw per sequence from its own parameters, seed and counter
+            s = self._samp
+            glue.sample(self._logits, s.temperature, s.top_k, s.top_p, s.seed, s.draw, self.next_tokens, self._ids.view(-1))
+        else:
+            if self._exchange is not None:
+                self._exchange.step.add_(1)                  # the step number the peers' arrival counters are compared with
+            # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight
+            # into every peer's buffer over NVLink + arrival counters
+            glue.greedy_sample(self._logits, self.next_tokens, self._ids.view(-1), self._exchange)
         if self._dist_tokens is not None and self._dist_in_graph:
             from . import dist as kdist
             kdist.gather_tokens(self.next_tokens, out=self._dist_tokens)
@@ -726,12 +783,66 @@ class LlamaForCausalLM_KIVI(nn.Module):
             raise NotImplementedError("data-parallel replicas of a tensor-parallel model are not supported")
         self._exchange, self._dist_tokens = None, None
         if world_size > 1 and mode == "p2p":
+            if self._sampling:
+                raise NotImplementedError(_P2P_SAMPLING)
             from . import dist as kdist
             self._exchange = kdist.PeerTokenExchange(self.cache.batch, self.cache.device)
         elif world_size > 1:
             self._dist_tokens = torch.zeros(world_size * self.cache.batch, dtype=torch.long, device=self.cache.device)
         self._dist_in_graph = in_graph
         self._graph = None
+
+    # ------------------------------------------------------------------ sampling
+    def set_sampling(self, temperature=1.0, top_k=50, top_p=1.0, seed=0):
+        """Sample the next token of every decode step on the device (kivi_sample_f32, the step's last kernel, inside its
+        CUDA graph): temperature, then top-k, then top-p, then one draw.  Scalars, or one value per batch row; row b draws
+        from the Philox stream of key seed + b (an int seed) or seed[b], starting at draw 0.  temperature 0 makes a row
+        greedy.  set_sampling(None) returns the whole step to the greedy kernel.  The captured step is dropped when the
+        mode changes, not when only parameters do.  Under tensor parallelism every rank calls this with the same arguments."""
+        assert self.cache is not None, "call init_cache() first"
+        on = temperature is not None
+        if on:
+            if self._exchange is not None:
+                raise NotImplementedError(_P2P_SAMPLING)
+            t, k, p, sd = sampling_rows(self.cache.batch, temperature, top_k, top_p, seed)
+            s, dev = self._samp, self.cache.device
+            s.temperature.copy_(torch.tensor(t, dtype=torch.float32).to(dev))
+            s.top_k.copy_(torch.tensor(k, dtype=torch.int32).to(dev))
+            s.top_p.copy_(torch.tensor(p, dtype=torch.float32).to(dev))
+            s.seed.copy_(torch.tensor([x - 2 ** 64 if x >= 2 ** 63 else x for x in sd], dtype=torch.long).to(dev))
+            s.draw.zero_()
+        if on != self._sampling:
+            self._sampling, self._graph = on, None
+
+    def set_slot_sampling(self, seq: int, temperature=1.0, top_k=50, top_p=1.0, seed=0):
+        """The sampling parameters of batch row `seq` alone (a slot given to a new request), its draw counter back to 0; the
+        row's key is `seed` itself.  The captured step reads them on the device: no recapture."""
+        if not self._sampling:
+            raise RuntimeError("set_slot_sampling: the step is greedy; call set_sampling() first")
+        if not 0 <= seq < self.cache.batch:
+            raise ValueError(f"seq {seq} outside the batch of {self.cache.batch}")
+        t, k, p, sd = sampling_rows(1, temperature, top_k, top_p, seed)
+        s = self._samp
+        s.temperature[seq], s.top_k[seq], s.top_p[seq] = t[0], k[0], p[0]
+        s.seed[seq] = sd[0] - 2 ** 64 if sd[0] >= 2 ** 63 else sd[0]
+        s.draw[seq] = 0
+
+    def sample_first(self, logits, seq: int | None = None):
+        """first_tokens() under sampling: the prompt's last-position logits ([B, vocab] of prefill, or [vocab] of
+        insert(seq)) go through the step's own sampling kernel with the rows' parameters and consume their next draw
+        (draw 0 after set_sampling / set_slot_sampling).  Rank 0's ids under tensor parallelism, like first_tokens."""
+        from . import glue
+        if not self._sampling:
+            raise RuntimeError("sample_first: the step is greedy; call set_sampling() first")
+        s = self._samp
+        rows = slice(None) if seq is None else slice(seq, seq + 1)
+        logits = logits.reshape(-1, logits.shape[-1]).float().contiguous()
+        tok = torch.empty(logits.shape[0], dtype=torch.long, device=logits.device)
+        glue.sample(logits, s.temperature[rows], s.top_k[rows], s.top_p[rows], s.seed[rows], s.draw[rows], tok)
+        if self.tensor_parallel and self.tp_world > 1:
+            import torch.distributed as dist
+            dist.broadcast(tok, src=0)
+        return tok if seq is None else tok[0]
 
     @property
     def all_tokens(self):
@@ -835,9 +946,10 @@ class LlamaForCausalLM_KIVI(nn.Module):
     @torch.no_grad()
     def decode_step(self, input_ids=None, use_graph: bool = True):
         """One decode step for the whole batch: input_ids [B, 1] (device) -> logits [B, vocab] fp32 (device,
-        a static buffer); `next_tokens` [B] holds their argmax (and `all_tokens` every rank's, see
-        enable_token_allgather).  The step (32 x [norm, qkv, rope, fused KIVI attention, o_proj, MLP], lm_head,
-        cache advance, greedy argmax, token all-gather) is captured once in a CUDA graph and replayed."""
+        a static buffer); `next_tokens` [B] holds their argmax, or after set_sampling() one sampled id per sequence (and
+        `all_tokens` every rank's, see enable_token_allgather).  The step (32 x [norm, qkv, rope, fused KIVI attention,
+        o_proj, MLP], lm_head, cache advance, argmax or sampling, token all-gather) is captured once in a CUDA graph and
+        replayed."""
         assert self.cache is not None
         if self.cache.kv_len + 1 > self.cache.max_tokens:
             raise ValueError("KIVI cache capacity exceeded")
@@ -852,6 +964,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 # warm-up on a side stream (cuBLAS workspaces, lazy module loading, NCCL channels), then capture
                 state = self.cache.state.clone()
                 pos, ids0 = self._pos.clone(), self._ids.clone()
+                draw = self._samp.draw.clone() if self._sampling else None
                 s = torch.cuda.Stream()
                 s.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(s):
@@ -864,6 +977,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 self.cache.state.copy_(state)
                 self._pos.copy_(pos)
                 self._ids.copy_(ids0)
+                if draw is not None:
+                    self._samp.draw.copy_(draw)                              # the warm-up step consumed a draw per row
                 from . import _lib
                 n0 = _lib.launch_count()
                 g = torch.cuda.CUDAGraph()
@@ -883,13 +998,17 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     @torch.no_grad()
     def generate(self, input_ids=None, max_new_tokens: int | None = None, use_graph: bool = True, attention_mask=None,
-                 max_length: int | None = None, do_sample: bool = False, **unused):
-        """Greedy decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
-        max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Sampling is outside
-        the hot path: do_sample is rejected.  attention_mask: an HF padding mask of a LEFT-padded batch (prefill(); the
-        decode steps skip each sequence's padding); right padding raises ValueError."""
+                 max_length: int | None = None, do_sample: bool = False, temperature=1.0, top_k=50, top_p=1.0, seed=0,
+                 **unused):
+        """Decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
+        max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Greedy by default;
+        do_sample=True samples every token, the first included, on the device with temperature / top_k / top_p (HF's
+        defaults; scalars or one value per sequence, set_sampling) from the Philox streams of `seed`: the same seed gives
+        the same ids, with or without the CUDA graph.  generate() sets the step's mode (set_sampling) to what this call asks
+        for and leaves it so: a later decode_step() samples after do_sample=True and takes the argmax after do_sample=False.  attention_mask: an HF padding mask of a LEFT-padded batch
+        (prefill(); the decode steps skip each sequence's padding); right padding raises ValueError."""
         if do_sample:
-            raise NotImplementedError("kivi_b200.generate decodes greedily; sample from decode_step() logits instead")
+            sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
         if attention_mask is not None:
             kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
         B, n = input_ids.shape
@@ -899,9 +1018,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
             max_new_tokens = max_length - n
         if self.cache is None or self.cache.batch != B or self.cache.max_tokens < n + max_new_tokens:
             self.init_cache(B, n + max_new_tokens)
+        # generate() owns the step's mode; it changes (and the captured step is dropped) only when do_sample does
+        if do_sample:
+            self.set_sampling(temperature, top_k, top_p, seed)
+        else:
+            self.set_sampling(None)
         logits = self.prefill(input_ids, attention_mask)
         out = [input_ids]
-        tok = self.first_tokens(logits).view(B, 1)
+        tok = (self.sample_first(logits) if do_sample else self.first_tokens(logits)).view(B, 1)
         for _ in range(max_new_tokens - 1):
             out.append(tok)
             self.decode_step(tok, use_graph=use_graph)

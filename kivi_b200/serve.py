@@ -5,7 +5,8 @@ All sequences share one length T (one `state` for the whole batch).  A new promp
 right-aligned, at positions [T - n, T), with kv_start = T - n (LlamaForCausalLM_KIVI.insert -> KiviCache.refill); a
 finished slot is released (kv_start beyond every length: it reads no cached byte).  T grows by one per step; positions
 that no live sequence sees any more are dropped from the front in multiples of max(128, R) (KiviCache.shift), so the
-timeline stays inside the cache.  Decoding is greedy, as everywhere in this package.
+timeline stays inside the cache.  A request decodes greedily, or samples with its own temperature / top-k / top-p / seed:
+the sampling kernel of the step reads each slot's parameters on the device, so both kinds share a batch and one step graph.
 """
 from __future__ import annotations
 
@@ -14,6 +15,33 @@ from collections import deque
 import torch
 
 from .cache import kv_start_from_mask
+from .llama_kivi import sampling_rows
+
+GREEDY = dict(temperature=0.0, top_k=0, top_p=1.0, seed=0)            # the slot parameters of a request without params
+
+
+def parse_requests(requests):
+    """requests: (prompt ids, max_new_tokens) or (prompt ids, max_new_tokens, params) with params a dict of temperature,
+    top_k, top_p, seed (missing keys: 1.0, 50, 1.0, 0, as generate(do_sample=True); the seed is the request's Philox key).
+    Returns ([(prompt int64 1-D on the host, max_new_tokens)], [params or None]); ValueError for an empty prompt, a budget
+    below 1, an unknown key or a value outside its range."""
+    reqs, params = [], []
+    for i, r in enumerate(requests):
+        if len(r) not in (2, 3):
+            raise ValueError(f"request {i}: expected (prompt, max_new_tokens) or (prompt, max_new_tokens, params)")
+        p = torch.as_tensor(r[0]).reshape(-1).to(torch.long).cpu()
+        if p.numel() < 1 or int(r[1]) < 1:
+            raise ValueError("every request needs at least one prompt token and max_new_tokens >= 1")
+        reqs.append((p, int(r[1])))
+        par = r[2] if len(r) == 3 else None
+        if par is not None:
+            unknown = set(par) - {"temperature", "top_k", "top_p", "seed"}
+            if unknown:
+                raise ValueError(f"request {i}: unknown sampling parameters {sorted(unknown)}")
+            sampling_rows(1, **par)                                       # ValueError for a value outside its range
+            par = dict(par)
+        params.append(par)
+    return reqs, params
 
 
 def plan_admission(T: int, tv: int, max_tokens: int, quantum: int, live_starts, prompt_len: int, new_tokens: int,
@@ -40,22 +68,21 @@ def plan_admission(T: int, tv: int, max_tokens: int, quantum: int, live_starts, 
 @torch.no_grad()
 def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None = None, use_graph: bool = True,
           stats: dict | None = None):
-    """Greedy decoding of a stream of requests with `batch` slots on one cache of `max_tokens` positions.
-    requests: a list of (prompt ids 1-D, max_new_tokens).  Yields (index into requests, new token ids [k] int64 on the
-    host) as each request finishes: after max_new_tokens tokens, or after eos_token_id (included, as in HF).
+    """Decoding of a stream of requests with `batch` slots on one cache of `max_tokens` positions.
+    requests: a list of (prompt ids 1-D, max_new_tokens), greedy, or (prompt ids, max_new_tokens, params), sampled on the
+    device with params = a dict of temperature, top_k, top_p, seed (parse_requests).  A sampled request's tokens depend on
+    its own prompt, parameters and seed only, not on its slot or on the other requests.  When no request has params the
+    step is the greedy one throughout.  serve() sets the model's mode (set_sampling) for its requests and leaves it so.
+    Yields (index into requests, new token ids [k] int64 on the host) as each request finishes: after max_new_tokens tokens, or after eos_token_id (included, as in HF).
     The first `batch` requests start with one left-padded prefill, padded to the longest prompt of the whole list, so every
     later prompt fits under the shared length.  Each step is one decode_step (its CUDA graph is captured once: the batch
     is ragged from the start) and one device-to-host read of the sampled ids; finished slots are released and refilled
     from the queue in order.  stats: an optional dict that receives counters (steps, slot_steps = live slots summed over
     the steps, inserts, shifts, shifted_tokens, prefills)."""
-    reqs = []
-    for p, m in requests:
-        p = torch.as_tensor(p).reshape(-1).to(torch.long).cpu()
-        if p.numel() < 1 or int(m) < 1:
-            raise ValueError("every request needs at least one prompt token and max_new_tokens >= 1")
-        reqs.append((p, int(m)))
+    reqs, params = parse_requests(requests)
     if not reqs:
         return
+    sampling = any(par is not None for par in params)
     longest = max(p.numel() for p, _ in reqs)
     for i, (p, m) in enumerate(reqs):
         if longest + m > max_tokens:
@@ -70,6 +97,21 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
         cache = model.init_cache(batch, max_tokens)
     quantum = max(128, cache.residual_length)
     dev = cache.device
+    # serve() owns the step's mode: sampling with every slot greedy until a sampled request takes it, or the greedy step
+    if sampling:
+        model.set_sampling(**GREEDY)
+    else:
+        model.set_sampling(None)
+
+    def first_token(logits, slot=None, rows=None):
+        """The first token(s) from prompt logits: of slot `slot` (insert) or of the whole batch, whose row b holds request
+        rows[b] (prefill); a slot gets its request's parameters and a fresh draw counter here."""
+        if not sampling:
+            return model.first_tokens(logits)
+        for b, i in enumerate(rows) if slot is None else [(slot, rows)]:
+            model.set_slot_sampling(b, **(GREEDY if params[i] is None else params[i]))
+        return model.sample_first(logits, slot)
+
     queue = deque(range(len(reqs)))
     owner = [None] * batch                  # request index decoding in each slot
     outs = [[] for _ in range(batch)]
@@ -97,7 +139,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
         ids, mask = ids.to(dev), mask.to(dev)
         logits = model.prefill(ids, attention_mask=mask)
         cache.set_kv_start(kv_start_from_mask(mask))                      # ragged from the start: one step graph
-        first = model.first_tokens(logits)
+        first = first_token(logits, rows=rows)
         model._ids.copy_(first.view(batch, 1))
         first = first.tolist()
         stats["prefills"] += 1
@@ -124,7 +166,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
                         stats["shifts"] += 1
                         stats["shifted_tokens"] += plan[0]
                     i = queue.popleft()
-                    tok = int(model.first_tokens(model.insert(slot, p.to(dev))))
+                    tok = int(first_token(model.insert(slot, p.to(dev)), slot, i))
                     model._ids[slot] = tok
                     owner[slot] = i
                     stats["inserts"] += 1
