@@ -159,8 +159,56 @@ class LlamaRMSNorm(nn.Module):
         return self.weight * h.to(x.dtype)
 
 
-def _rope_tables(head_dim, max_pos, theta, device):
+ROPE_TYPES = ("default", "linear", "llama3")
+
+
+def rope_settings(config):
+    """The RoPE settings of a config object or a config.json dict -> (theta, scaling).  transformers 5.x writes them as
+    `rope_parameters` {"rope_theta", "rope_type", ...}; 4.x as a top-level `rope_theta` plus `rope_scaling` (None, or a dict
+    naming its type under "type" or "rope_type").  scaling is None for plain RoPE, else the parameters with "rope_type"
+    set.  Raises NotImplementedError for a RoPE type outside ROPE_TYPES and for a partial rotary embedding."""
+    get = config.get if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+    params = dict(get("rope_parameters") or get("rope_scaling") or {})
+    theta = float(params.get("rope_theta", get("rope_theta", 10000.0)))
+    kind = params.get("rope_type", params.get("type", "default"))
+    if kind not in ROPE_TYPES:
+        raise NotImplementedError(f"RoPE type {kind!r} is not supported (supported: {', '.join(ROPE_TYPES)})")
+    partial = params.get("partial_rotary_factor", get("partial_rotary_factor"))
+    if partial is not None and float(partial) != 1.0:
+        raise NotImplementedError(f"partial_rotary_factor {partial}: only a rotary embedding over the whole head is supported")
+    if kind == "default":
+        return theta, None
+    need = ("factor",) if kind == "linear" else ("factor", "low_freq_factor", "high_freq_factor")
+    missing = [k for k in need if k not in params]
+    if missing:
+        raise ValueError(f"RoPE type {kind!r} needs {', '.join(missing)}")
+    scaling = {k: float(params[k]) for k in need}
+    scaling["rope_type"] = kind
+    if kind == "llama3":        # transformers falls back to max_position_embeddings as well
+        scaling["original_max_position_embeddings"] = params.get("original_max_position_embeddings",
+                                                                 get("max_position_embeddings"))
+    return theta, scaling
+
+
+def _rope_tables(head_dim, max_pos, theta, device, scaling=None):
+    """fp16 cos / sin [max_pos, head_dim].  The inverse frequencies follow transformers' RoPE initialisers (default, linear,
+    llama3) op for op in fp32, so the tables are the ones its rotary embedding produces."""
     inv_freq = 1.0 / (theta ** (torch.arange(0, head_dim, 2, dtype=torch.float32, device=device) / head_dim))
+    kind = "default" if scaling is None else scaling["rope_type"]
+    if kind == "linear":
+        inv_freq = inv_freq / scaling["factor"]
+    elif kind == "llama3":
+        factor, low, high = scaling["factor"], scaling["low_freq_factor"], scaling["high_freq_factor"]
+        old_context_len = scaling["original_max_position_embeddings"]
+        low_freq_wavelen, high_freq_wavelen = old_context_len / low, old_context_len / high
+        wavelen = 2 * math.pi / inv_freq
+        inv_freq_llama = torch.where(wavelen > low_freq_wavelen, inv_freq / factor, inv_freq)
+        smooth_factor = (old_context_len / wavelen - low) / (high - low)
+        smoothed_inv_freq = (1 - smooth_factor) * inv_freq_llama / factor + smooth_factor * inv_freq_llama
+        is_medium_freq = ~(wavelen < high_freq_wavelen) * ~(wavelen > low_freq_wavelen)
+        inv_freq = torch.where(is_medium_freq, smoothed_inv_freq, inv_freq_llama)
+    elif kind != "default":
+        raise NotImplementedError(f"RoPE type {kind!r} is not supported (supported: {', '.join(ROPE_TYPES)})")
     freqs = torch.outer(torch.arange(max_pos, dtype=torch.float32, device=device), inv_freq)
     emb = torch.cat((freqs, freqs), dim=-1)
     return emb.cos().half(), emb.sin().half()
@@ -411,6 +459,11 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def __init__(self, config, tensor_parallel: bool = False):
         super().__init__()
+        head_dim = getattr(config, "head_dim", None)            # transformers configs carry it explicitly
+        if head_dim is not None and (head_dim != config.hidden_size // config.num_attention_heads or head_dim != 128):
+            raise NotImplementedError(f"head_dim {head_dim} (hidden_size {config.hidden_size}, {config.num_attention_heads} "
+                                      "heads): only head_dim = hidden_size / num_attention_heads = 128 is supported")
+        rope_settings(config)                                   # an unsupported RoPE type is refused here, not at the first forward
         self.config = config
         self.vocab_size = config.vocab_size
         self.tensor_parallel = tensor_parallel
@@ -513,7 +566,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
             rows = max(rows, self.cache.max_tokens + 1)   # a cache longer than the config's context still has its rows
         if self._rope is None or self._rope[0].device != device or self._rope[0].shape[0] < rows:
             hd = self.config.hidden_size // self.config.num_attention_heads
-            self._rope = _rope_tables(hd, rows, self.config.rope_theta, device)
+            theta, scaling = rope_settings(self.config)
+            self._rope = _rope_tables(hd, rows, theta, device, scaling)
         return self._rope
 
     def _run_layers(self, input_ids, positions, pasts, attention_mask=None):
