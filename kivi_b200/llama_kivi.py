@@ -4,13 +4,13 @@
   (models/llama_kivi.py:314-399) on the reference's own 9-tuple cache, op for op, with every KIVI op
   routed to libkivi_b200 (cuda_bmm_fA_qB_outer without re-layout copies, fused pack kernel).
 * `kivi_prefill_tuple`           -- the prefill split + pack (:425-455) producing that 9-tuple.
-* `LlamaFlashAttention_KIVI`     -- attention module: same projections / RoPE / cache policy; the fast
-  path keeps the cache in a pre-allocated `KiviCache` and runs ONE fused CUDA launch per layer per
-  step (kivi_decode.cu); `past_key_value` may also be the legacy 9-tuple (then the tuple path runs).
+* `LlamaFlashAttention_KIVI`     -- attention module: same projections / RoPE / cache policy on the
+  reference's 9-tuple; a prompt pass may instead hand its rotated K/V to the pre-allocated `KiviCache`
+  (`store_kv`).
 * `LlamaForCausalLM_KIVI`        -- decoder-only LM with HF Llama parameter names (state dicts of
   LlamaForCausalLM / MistralForCausalLM load unchanged), config attrs k_bits, v_bits, group_size,
   residual_length (models/llama_kivi.py:34-38).  Host code is PyTorch (linears = cuBLAS); the decode
-  step is captured in a CUDA graph.
+  step runs on the `KiviCache` (fused attention, kivi_decode.cu) and is captured in a CUDA graph.
 
 The reference's forks star-import transformers 4.43 internals and do not import under the installed
 transformers 5.5 (SURVEY 8c); this module depends on torch only and accepts any config object with the
@@ -256,43 +256,26 @@ class LlamaFlashAttention_KIVI(nn.Module):
             return F.scaled_dot_product_attention(q, kk, vv, is_causal=True)
         return F.scaled_dot_product_attention(q, kk, vv, attn_mask=attention_mask.to(q.dtype))
 
-    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None):
+    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None):
         """hidden_states [B, q_len, hidden]; cos/sin broadcastable to [B, 1, q_len, D].
-        past_key_value: None (prefill, returns a 9-tuple), a 9-tuple (reference semantics), or a
-        (KiviCache, layer) pair (fused path; prefill fills it, decode is one launch), or a (KiviCache, layer, seq) triple:
-        the B = 1 prompt of a new sequence, written into slot `seq` of a live cache (KiviCache.refill).
+        past_key_value: None (a prompt pass, returns a 9-tuple) or the reference's 9-tuple (decode, returns the next one).
+        store_kv: with a prompt pass, a callable store_kv(layer, k, v) that takes the rotated K and V [B, Hkv, q_len, D] in
+        place of the 9-tuple (the fused cache: KiviCache.prefill, or a refill of one slot); the pass then returns None.
         attention_mask: None or additive [B, 1, q_len, kv_len] (models/llama_kivi.py:364-372)."""
         bsz, q_len, _ = hidden_states.shape
         q, k, v = self._qkv(hidden_states, cos, sin)
-        fused = isinstance(past_key_value, tuple) and len(past_key_value) in (2, 3) and \
-            isinstance(past_key_value[0], KiviCache)
-        if fused and len(past_key_value) == 3:                              # a new sequence into one slot
-            cache, layer, seq = past_key_value
-            attn_output = self._prompt_attention(q, k, v, attention_mask)
-            cache.refill(layer, seq, k, v)
-            attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.num_heads * self.head_dim)
-            return self.o_proj(attn_output), None, past_key_value
-        if fused:
-            cache, layer = past_key_value
-            if q_len > 1:                                                   # prefill (:401-452)
-                attn_output = self._prompt_attention(q, k, v, attention_mask)
-                cache.prefill(layer, k, v)
-                attn_output = attn_output.transpose(1, 2).reshape(bsz, q_len, self.num_heads * self.head_dim)
-            else:                                                           # decode (:314-399), one launch
-                out = cache.decode_attention(layer, q.reshape(bsz, self.num_heads, self.head_dim).contiguous(),
-                                             k.reshape(bsz, self.num_key_value_heads, self.head_dim).contiguous(),
-                                             v.reshape(bsz, self.num_key_value_heads, self.head_dim).contiguous(),
-                                             mask=attention_mask)
-                attn_output = out.view(bsz, 1, self.num_heads * self.head_dim)
-            return self.o_proj(attn_output), None, past_key_value
         if past_key_value is not None:                                      # reference 9-tuple, decode
             attn_output, past = kivi_decode_attention_tuple(q, k, v, past_key_value, self.group_size, self.k_bits,
                                                             self.v_bits, self.residual_length, attention_mask)
             attn_output = attn_output.transpose(1, 2).contiguous()
-        else:                                                               # prefill -> 9-tuple
+        else:                                                               # prompt (:401-455)
             attn_output = self._prompt_attention(q, k, v, attention_mask).transpose(1, 2)
-            past = kivi_prefill_tuple(k, v, self.group_size, self.k_bits, self.v_bits, self.residual_length)
-        attn_output = attn_output.reshape(bsz, q_len, self.hidden_size)
+            if store_kv is None:
+                past = kivi_prefill_tuple(k, v, self.group_size, self.k_bits, self.v_bits, self.residual_length)
+            else:
+                store_kv(self.layer_idx, k, v)
+                past = None
+        attn_output = attn_output.reshape(bsz, q_len, self.num_heads * self.head_dim)
         return self.o_proj(attn_output), None, past
 
 
@@ -320,9 +303,10 @@ class LlamaDecoderLayer_KIVI(nn.Module):
         self.post_attention_layernorm = LlamaRMSNorm(config.hidden_size, config.rms_norm_eps)
         self.tp_world = tp_world
 
-    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None):
+    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None):
         residual = hidden_states
-        h, _, past = self.self_attn(self.input_layernorm(hidden_states), cos, sin, past_key_value, attention_mask)
+        h, _, past = self.self_attn(self.input_layernorm(hidden_states), cos, sin, past_key_value, attention_mask,
+                                    store_kv)
         if self.tp_world > 1:                                                 # partial sums of the sharded projections
             h = sum_partials(h)
         hidden_states = residual + h
@@ -570,14 +554,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self._rope = _rope_tables(hd, rows, theta, device, scaling)
         return self._rope
 
-    def _run_layers(self, input_ids, positions, pasts, attention_mask=None):
+    def _run_layers(self, input_ids, positions, pasts, attention_mask=None, store_kv=None):
         cos_t, sin_t = self._tables(input_ids.device)
         cos = cos_t.index_select(0, positions.reshape(-1)).view(positions.shape[0], 1, positions.shape[1], -1)
         sin = sin_t.index_select(0, positions.reshape(-1)).view(positions.shape[0], 1, positions.shape[1], -1)
         h = self.model.embed_tokens(input_ids)
         new_pasts = []
         for i, layer in enumerate(self.model.layers):
-            h, past = layer(h, cos, sin, pasts[i] if pasts is not None else None, attention_mask)
+            h, past = layer(h, cos, sin, pasts[i] if pasts is not None else None, attention_mask, store_kv)
             new_pasts.append(past)
         h = self.model.norm(h)
         return h, new_pasts
@@ -624,8 +608,10 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def _fused_forward_ok(self, input_ids, past_key_values, attention_mask, position_ids, start):
         """forward() may run on the pre-allocated cache when nothing asks for what only the tuple path offers: CUDA fp16
-        weights, equal-length sequences (no padding mask), default positions, and -- with a past -- one new token."""
-        if not self.fused_forward or not input_ids.is_cuda or not self._fast_ok():
+        weights, head_dim 128, equal-length sequences (no padding mask), default positions, and -- with a past -- one new
+        token."""
+        if not (self.fused_forward and input_ids.is_cuda and self.lm_head.weight.dtype == torch.float16
+                and self.model.layers[0].self_attn.head_dim == 128):
             return False
         B, q_len = input_ids.shape
         if attention_mask is not None and (attention_mask.dim() != 2 or not bool(attention_mask.to(torch.bool).all())):
@@ -650,10 +636,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if past_key_values is None:                                          # prefill into the blocked cache
             if self.cache is None or self.cache.batch != B or self.cache.max_tokens < q_len + 1:
                 self.init_cache(B, q_len + reserve)
-            positions = torch.arange(q_len, device=input_ids.device).unsqueeze(0).expand(B, -1)
-            h, _ = self._run_layers(input_ids, positions, [(self.cache, i) for i in range(n_layers)])
-            self._pos.fill_(q_len)
-            logits = self.lm_head(h).float()
+            logits = self.lm_head(self._prompt_pass(input_ids)).float()
         else:
             if not isinstance(past_key_values[0], KiviPast):                 # a cache grown elsewhere (reference hook): one re-layout
                 self.import_cache(past_key_values, max_tokens=start + reserve)
@@ -692,8 +675,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     # ------------------------------------------------------------------ fused cache path
     def init_cache(self, batch: int, max_tokens: int):
+        """Allocate the fused KIVI cache for `batch` sequences of up to `max_tokens` tokens.  The fused path runs fp16
+        weights only (ValueError otherwise: convert the model with .half())."""
         cfg = self.config
-        dev = self.lm_head.weight.device
+        dev, dtype = self.lm_head.weight.device, self.lm_head.weight.dtype
+        if dtype != torch.float16:
+            raise ValueError(f"the fused KIVI cache path needs fp16 weights, the model's are {dtype}: call .half() first")
         self.cache, self._graph = None, None                 # release the previous cache before the new one is allocated
         a = self.model.layers[0].self_attn                  # this rank's heads
         self.cache = KiviCache(cfg.num_hidden_layers, batch, a.num_heads, a.num_key_value_heads,
@@ -741,10 +728,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
         """Run the prompt, fill the cache (models/llama_kivi.py:401-452), return last-position logits.
         attention_mask: None or an HF padding mask [B, n] of a LEFT-padded batch (ValueError otherwise).  The prompt
         attention then takes the additive mask of the tuple path, positions follow HF (cumsum - 1, pad positions 1), and
-        the decode steps skip each sequence's padding (KiviCache.set_kv_start).  An all-ones mask is no mask."""
+        the decode steps skip each sequence's padding (KiviCache.set_kv_start).  An all-ones mask is no mask.  Every
+        prompt, a one-token one included, replaces what the cache held."""
         assert self.cache is not None, "call init_cache() first"
+        return self.lm_head(self._prompt_pass(input_ids, attention_mask)[:, -1]).float()
+
+    def _prompt_pass(self, input_ids, attention_mask=None):
+        """prefill() up to the final norm: the hidden states [B, n, hidden] of every position."""
         B, n = input_ids.shape
-        pasts = [(self.cache, i) for i in range(len(self.model.layers))]
         starts = None
         if attention_mask is not None:
             starts = kv_start_from_mask(attention_mask)
@@ -752,18 +743,18 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 starts = None
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
-            h, _ = self._run_layers(input_ids, positions, pasts)
+            h, _ = self._run_layers(input_ids, positions, None, store_kv=self.cache.prefill)
             self._pos.fill_(n)
         else:
             am = attention_mask.to(input_ids.device)
             positions = am.long().cumsum(-1) - 1                            # prepare_inputs_for_generation (:908-948)
             positions.masked_fill_(am == 0, 1)
             mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device)
-            h, _ = self._run_layers(input_ids, positions, pasts, mask)
+            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=self.cache.prefill)
             starts = starts.to(self._pos.device)
             self._pos.copy_((n - starts).to(torch.long).view(B, 1))
             self.cache.set_kv_start(starts)
-        return self.lm_head(h[:, -1]).float()
+        return h
 
     @torch.no_grad()
     def insert(self, seq: int, prompt_ids):
@@ -777,7 +768,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if not 1 <= n <= T:
             raise ValueError(f"a prompt of {n} tokens does not fit the shared length {T} (1 <= n <= length)")
         positions = torch.arange(n, device=ids.device).unsqueeze(0)
-        h, _ = self._run_layers(ids, positions, [(self.cache, i, seq) for i in range(len(self.model.layers))])
+        h, _ = self._run_layers(ids, positions, None, store_kv=lambda layer, k, v: self.cache.refill(layer, seq, k, v))
         self._pos[seq] = n
         self.cache.set_seq_start(seq, T - n)
         return self.lm_head(h[0, -1]).float()
@@ -799,34 +790,6 @@ class LlamaForCausalLM_KIVI(nn.Module):
             v = torch.randn((c.batch, c.num_kv_heads, n, c.head_dim), generator=gen, device=c.device, dtype=torch.float16)
             c.prefill(l, k, v)
         self._pos.fill_(n)
-
-    def _step_body(self):
-        if self.tensor_parallel and not self._fast_ok():
-            raise NotImplementedError("tensor-parallel decoding needs head_dim 128, bias-free projections and fp16 weights")
-        if self._fast_ok():
-            self._step_body_fast()
-        else:
-            pasts = [(self.cache, i) for i in range(len(self.model.layers))]
-            h, _ = self._run_layers(self._ids, self._pos, pasts)
-            self._logits.copy_(self.lm_head(h[:, 0]).float())
-        self.cache._enqueue_advance()                        # decode_step advances the host mirror after each replay
-        self._pos.add_(1)
-        # greedy sampling inside the step (and inside its CUDA graph): the argmax of a sequence needs only that
-        # sequence's logits, so with data-parallel replicas the exchange is the sampled ids, 8 B per sequence
-        from . import glue
-        if self._sampling:
-            # in the argmax kernel's place, one kernel as well: a draw per sequence from its own parameters, seed and counter
-            s = self._samp
-            glue.sample(self._logits, s.temperature, s.top_k, s.top_p, s.seed, s.draw, self.next_tokens, self._ids.view(-1))
-        else:
-            if self._exchange is not None:
-                self._exchange.step.add_(1)                  # the step number the peers' arrival counters are compared with
-            # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight
-            # into every peer's buffer over NVLink + arrival counters
-            glue.greedy_sample(self._logits, self.next_tokens, self._ids.view(-1), self._exchange)
-        if self._dist_tokens is not None and self._dist_in_graph:
-            from . import dist as kdist
-            kdist.gather_tokens(self.next_tokens, out=self._dist_tokens)
 
     def enable_token_allgather(self, world_size: int, in_graph: bool = True, mode: str = "nccl"):
         """Data-parallel replicas (kivi_b200.dist): every rank's sampled ids end up in `all_tokens` [world_size * B].
@@ -904,16 +867,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
             return self._exchange.tokens()
         return self.next_tokens if self._dist_tokens is None else self._dist_tokens
 
-    def _fast_ok(self):
-        a = self.model.layers[0].self_attn
-        return a.head_dim == 128 and a.q_proj.bias is None and self.lm_head.weight.dtype == torch.float16
-
     def _ensure_fast(self):
-        """Fused q|k|v, o and gate|up weights in [in, out] layout + static activation buffers for the 9-launch-per-layer
-        step.  At M = B rows cuBLAS streams the weights faster from this layout (tools/gemm_probe.py compares the two
-        layouts; down is layout-neutral).  The fused buffers OWN the storage:
-        the nn.Linear parameters become transposed views of them, so there is one copy of every weight (the reference's
-        mem_spd_test reports peak memory) and load_state_dict / in-place edits reach the decode path."""
+        """Fused q|k|v, o and gate|up weights in [in, out] layout, the fused q|k|v bias (None without attention biases)
+        + static activation buffers for the 9-launch-per-layer step.  At M = B rows cuBLAS streams the weights faster from
+        this layout (tools/gemm_probe.py compares the two layouts; down is layout-neutral).  The fused buffers OWN the
+        storage: the nn.Linear parameters become (transposed) views of them, so there is one copy of every weight (the
+        reference's mem_spd_test reports peak memory) and load_state_dict / in-place edits reach the decode path."""
         if self._fast is not None and self._fast.B == self.cache.batch:
             return self._fast
         cfg, dev, B = self.config, self.cache.device, self.cache.batch
@@ -925,7 +884,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if f.wqkv is None:
             def view_param(buf, lo, hi):
                 return nn.Parameter(buf.t()[lo:hi], requires_grad=False)
-            f.wqkv, f.wgu, f.wo = [], [], []
+            f.wqkv, f.bqkv, f.wgu, f.wo = [], [], [], []
             for l in self.model.layers:
                 a, m = l.self_attn, l.mlp
                 nq, nk = a.q_proj.weight.shape[0], a.k_proj.weight.shape[0]
@@ -933,6 +892,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 a.q_proj.weight, a.k_proj.weight = view_param(w, 0, nq), view_param(w, nq, nq + nk)
                 a.v_proj.weight = view_param(w, nq + nk, w.shape[1])
                 f.wqkv.append(w)
+                b = None
+                if a.q_proj.bias is not None:
+                    b = torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias])
+                    a.q_proj.bias, a.k_proj.bias = view_param(b, 0, nq), view_param(b, nq, nq + nk)
+                    a.v_proj.bias = view_param(b, nq + nk, b.shape[0])
+                f.bqkv.append(b)
                 w = torch.cat([m.gate_proj.weight, m.up_proj.weight], 0).t().contiguous()
                 m.gate_proj.weight, m.up_proj.weight = view_param(w, 0, inter), view_param(w, inter, 2 * inter)
                 f.wgu.append(w)
@@ -947,9 +912,10 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._fast = f
         return f
 
-    def _step_body_fast(self):
+    def _step_body(self):
         """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split,
-        fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels.
+        fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels; then lm_head, the cache advance and the argmax
+        or sampling kernel.  A model with attention biases adds them in the q|k|v and o GEMMs (addmm).
         Tensor-parallel (self._allreduce is a PeerAllReduce): the same launches on this rank's heads and channels, but o_proj
         and down_proj write their partial sums into the PeerAllReduce slots, and the two residual-add + RMSNorm kernels of a
         layer become kivi_allreduce_add_rmsnorm_f16 (calls 2i and 2i + 1 of the step), which add up every rank's partials.
@@ -970,13 +936,19 @@ class LlamaForCausalLM_KIVI(nn.Module):
             else:
                 glue.allreduce_add_rmsnorm(f.res, weight, f.h, eps, ar, call=call)
 
+        def linear(x, w, bias, out):
+            if bias is None:
+                torch.mm(x, w, out=out)
+            else:
+                torch.addmm(bias, x, w, out=out)
+
         f.res.copy_(self.model.embed_tokens(self._ids)[:, 0])
         glue.add_rmsnorm(None, f.res, layers[0].input_layernorm.weight, f.h, eps)
         for i, l in enumerate(layers):
-            torch.mm(f.h, f.wqkv[i], out=f.qkv)
+            linear(f.h, f.wqkv[i], f.bqkv[i], f.qkv)
             glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
             cache.decode_attention(i, f.q, f.k, f.v, out=f.attn)
-            torch.mm(f.attn.view(f.B, -1), f.wo[i], out=partial(2 * i))
+            linear(f.attn.view(f.B, -1), f.wo[i], l.self_attn.o_proj.bias, partial(2 * i))
             add_rmsnorm(2 * i, l.post_attention_layernorm.weight)
             torch.mm(f.h, f.wgu[i], out=f.gu)
             glue.silu_mul(f.gu, f.act)
@@ -987,6 +959,23 @@ class LlamaForCausalLM_KIVI(nn.Module):
             ar.epoch.add_(2 * len(layers))                                   # the next step's calls continue the count
         torch.mm(f.h, self.lm_head.weight.t(), out=f.logits16)
         self._logits.copy_(f.logits16)                                       # logits.float() (:881)
+        cache._enqueue_advance()                             # decode_step advances the host mirror after each replay
+        self._pos.add_(1)
+        # greedy sampling inside the step (and inside its CUDA graph): the argmax of a sequence needs only that
+        # sequence's logits, so with data-parallel replicas the exchange is the sampled ids, 8 B per sequence
+        if self._sampling:
+            # in the argmax kernel's place, one kernel as well: a draw per sequence from its own parameters, seed and counter
+            s = self._samp
+            glue.sample(self._logits, s.temperature, s.top_k, s.top_p, s.seed, s.draw, self.next_tokens, self._ids.view(-1))
+        else:
+            if self._exchange is not None:
+                self._exchange.step.add_(1)                  # the step number the peers' arrival counters are compared with
+            # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight
+            # into every peer's buffer over NVLink + arrival counters
+            glue.greedy_sample(self._logits, self.next_tokens, self._ids.view(-1), self._exchange)
+        if self._dist_tokens is not None and self._dist_in_graph:
+            from . import dist as kdist
+            kdist.gather_tokens(self.next_tokens, out=self._dist_tokens)
 
     def first_tokens(self, logits):
         """Greedy ids of prompt logits (prefill / insert) -- under tensor parallelism rank 0's, broadcast, so the ranks can

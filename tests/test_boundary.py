@@ -201,3 +201,16 @@ def test_model_class_contract_on_cpu(tmp_path):
     re_ = LlamaForCausalLM_KIVI._reorder_cache(past, torch.tensor([2, 0, 0]))
     assert len(re_) == 2 and re_[0][8] == 133 and re_[0][1] is None
     assert torch.equal(re_[1][5], past[1][5][[2, 0, 0]])
+
+
+def test_fused_cache_needs_fp16_weights():
+    """The fused cache path runs fp16 weights only: init_cache, and generate() through it, refuse any other dtype with a
+    ValueError that names it, before anything is allocated."""
+    import torch
+    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI, default_config
+    m = LlamaForCausalLM_KIVI(default_config("tiny"))
+    with pytest.raises(ValueError, match="float32"):
+        m.init_cache(2, 16)
+    with pytest.raises(ValueError, match="float32"):
+        m.generate(torch.zeros(2, 3, dtype=torch.long), max_new_tokens=2)
+    assert m.cache is None

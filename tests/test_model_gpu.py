@@ -40,18 +40,57 @@ def test_tuple_hook_matches_oracle(H, Hkv, kb, vb, g, R, n0, steps):
                                       st[i].view(np.uint16) if st[i].dtype == np.float16 else st[i])
 
 
-@pytest.mark.parametrize("name,kw", [("tiny", {}), ("tiny", dict(num_attention_heads=4, num_key_value_heads=1, hidden_size=512,
-                                                                k_bits=4, v_bits=4, group_size=64, residual_length=64))])
+_GQA_K4V4 = dict(num_attention_heads=4, num_key_value_heads=1, hidden_size=512, k_bits=4, v_bits=4, group_size=64,
+                 residual_length=64)
+
+
+@pytest.mark.parametrize("name,kw", [("tiny", {}), ("tiny", _GQA_K4V4), ("tiny", dict(attention_bias=True))])
 def test_fused_model_matches_tuple_model(name, kw):
     """LlamaForCausalLM_KIVI: prefill + greedy decode through the fused cache path (CUDA graph) and through
-    the reference-style forward with per-layer 9-tuples give the same logits (two independent code paths)."""
+    the reference-style forward with per-layer 9-tuples give the same logits (two independent code paths).  With
+    attention biases the tuple path keeps the module linears, the decode step adds the fused biases in its GEMMs."""
     from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI, default_config
     cfg = default_config(name, **kw)
     torch.manual_seed(0)
     model = LlamaForCausalLM_KIVI(cfg).half().cuda().eval()
+    with torch.no_grad():
+        for pname, p in model.named_parameters():
+            if pname.endswith(".bias"):
+                p.uniform_(-1.0, 1.0)                 # as large as the projections' outputs: a dropped bias must show
+    ids = torch.randint(0, cfg.vocab_size, (2, 150), device="cuda")
+    _decode_against_tuple_path(model, ids, steps=40)
+
+
+def test_one_token_prompt_is_prefilled():
+    """A one-token prompt is a prompt like any other: prefill() and forward() write it into the fused cache, the decode
+    steps after it match the 9-tuple path, and a prompt pass on a cache that still holds an earlier sequence reads none
+    of it."""
+    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI, default_config
+    cfg = default_config("tiny", **_GQA_K4V4)
+    torch.manual_seed(0)
+    model = LlamaForCausalLM_KIVI(cfg).half().cuda().eval()
+    B = 2
+    ids = torch.randint(0, cfg.vocab_size, (B, 150), device="cuda")
+    one = ids[:, :1]
+    model.init_cache(B, 8)
+    model.prefill(one)
+    assert model.cache.kv_len == 1
+    assert model(input_ids=one).past_key_values[0][-1] == 1
+    _decode_against_tuple_path(model, one, steps=70)    # crosses a K flush (R = 64) and moves the V window
+    # after a generate() of a longer prompt the same one-token prefill gives the bits it gives on a new cache
+    model.generate(ids, max_new_tokens=8)
+    got = model.prefill(one).clone()
+    assert model.cache.kv_len == 1
+    model.init_cache(B, 8)
+    assert torch.equal(got, model.prefill(one))
+
+
+def _decode_against_tuple_path(model, ids, steps):
+    """Prefill `ids`, then `steps` teacher-forced decode steps on the fused cache (eager, then the CUDA graph) and through
+    forward() on the reference's 9-tuples: logits within the tolerance, argmax equal in all but 3 steps, and the packed
+    cache parts equal bit for bit."""
     model.fused_forward = False                       # forward() = the reference's own 9-tuple path (torch.cat growth, per-op launches)
-    B, n, steps = 2, 150, 40
-    ids = torch.randint(0, cfg.vocab_size, (B, n), device="cuda")
+    B, n = ids.shape
     # tuple path
     logits_t, pasts = model(ids)
     tok_t = logits_t[:, -1].argmax(-1, keepdim=True)
@@ -59,7 +98,6 @@ def test_fused_model_matches_tuple_model(name, kw):
     model.init_cache(B, n + steps + 4)
     logits_f = model.prefill(ids)
     assert torch.allclose(logits_f, logits_t[:, -1], rtol=2e-2, atol=2e-2)
-    tok_f = logits_f.argmax(-1, keepdim=True)
     agree = 0
     for s in range(steps):
         # feed BOTH paths the same token so that the comparison stays aligned
