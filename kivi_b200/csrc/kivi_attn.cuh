@@ -51,9 +51,6 @@ constexpr int kChunkUnroll = KIVI_UNROLL;
 #ifndef KIVI_EVICT_FIRST
 #define KIVI_EVICT_FIRST 1
 #endif
-#ifndef KIVI_SHIFT_IMAD
-#define KIVI_SHIFT_IMAD 0
-#endif
 #ifndef KIVI_PRED_FINALIZE
 #define KIVI_PRED_FINALIZE 1             // 0: the round-1 epilogue (selects); A/B builds
 #endif
@@ -180,26 +177,24 @@ template <int KB>
 __device__ __forceinline__ float2 q_prescale(float mx) {
     constexpr int Q = KB == 4 ? 2 : 0;
     if (!(mx > 0.f) || !(mx < kQPrescaleBelow)) return make_float2(1.f, 1.f);
-    const int k = Q - ((int)((__float_as_uint(mx) >> 23) & 0xff) - 127);   // Q - floor(log2 max|q|) in [Q + 4, Q + 24]
-    return make_float2(__uint_as_float((uint32_t)(127 + k) << 23), __uint_as_float((uint32_t)(127 - k) << 23));
+    const int e = floor_log2f(mx);                                         // Q - e in [Q + 4, Q + 24]
+    return make_float2(pow2f(Q - e), pow2f(e - Q));
 }
 // b of a packed V block whose largest |scale| is m: 0 unless 0 < m < 2^-4 (NaN, inf: 0)
 __device__ __forceinline__ int pv_boost(float m) {
     if (!(m > 0.f) || !(m < 0.0625f)) return 0;
-    return min(-4 - ((int)((__float_as_uint(m) >> 23) & 0xff) - 127), 9);     // >= 1: floor(log2 m) <= -5
+    return min(-4 - floor_log2f(m), 9);                                      // >= 1: floor(log2 m) <= -5
 }
-// floor(log2 |x|) of a normal fp32 x (-127 for 0)
-__device__ __forceinline__ int exp2_floor(float x) { return (int)((__float_as_uint(x) >> 23) & 0xff) - 127; }
 // v of a packed V block whose largest finite |scale| is m: its scales are taken x 2^-v in place, bringing m into [2^8, 2^9)
 // for m >= 2^10 and into [2^-13, 2^-12) (pv_boost 9) for 0 < m < 2^-13; 0 otherwise
 __device__ __forceinline__ int pv_vshift(float m) {
-    const int e = exp2_floor(m);
+    const int e = floor_log2f(m);
     return m >= 1024.f ? e - 8 : (m > 0.f && e < -13) ? e + 13 : 0;
 }
 // exponent of the extra probability scale of a boosted block: e + b, e = floor(log2 S) in [0, 15] (S >= 1: the largest
 // logit contributes exp(0) = 1; NaN -> 15)
 __device__ __forceinline__ int pv_extra_exp(float S, int b) {
-    return min(max((int)((__float_as_uint(S) >> 23) & 0xff) - 127, 0), 15) + b;
+    return min(max(floor_log2f(S), 0), 15) + b;
 }
 __device__ __forceinline__ __half2 pow2_h2(int e) {                           // 2^e as an fp16 pair, 0 <= e <= 15
     const uint32_t h = (uint32_t)(15 + e) << 10, hh = h | (h << 16);
@@ -303,29 +298,10 @@ __device__ __forceinline__ float fast_exp(float x) {
     return y;
 }
 
-__device__ __forceinline__ uint32_t h2_as_u32(const __half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
-__device__ __forceinline__ __half2 u32_as_h2(const uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
 // |h| of both halves, 0 for the non-finite ones (an inf scale must not set the factor of its block's finite groups)
 __device__ __forceinline__ __half2 finite_abs2(uint32_t w) {
     const __half2 a = __habs2(u32_as_h2(w));
     return u32_as_h2(h2_as_u32(a) & __hlt2_mask(a, __float2half2_rn(INFINITY)));
-}
-
-// One B-fragment register: column part 0 -> hi = fp16(x*s); part 1 -> lo = x*s - hi, exact while it is not below fp16's
-// smallest step (the callers prescale x where it would not be: q_prescale, pv_boost).
-#ifndef KIVI_BPREP2
-#define KIVI_BPREP2 1                    // 1: hi, then a PREDICATED fma(x, s, -hi) in the lo lanes (2 instructions); 0: branch-free 3
-#endif
-__device__ __forceinline__ uint32_t b_prep(uint32_t x2, uint32_t s2, __half2 msel) {
-    const __half2 x = u32_as_h2(x2), s = u32_as_h2(s2);
-#if KIVI_BPREP2
-    __half2 b = __hmul2(x, s);
-    if (h2_as_u32(msel) != 0u) b = __hfma2(x, s, __hneg2(b));   // lane-invariant predicate, negation folds into the HFMA2 operand
-    return h2_as_u32(b);
-#else
-    const __half2 nh = __hmul2(__hmul2(x, s), msel);         // nh = hi * (part ? -1 : 0);  b = fma(x, s, nh)
-    return h2_as_u32(__hfma2(x, s, nh));
-#endif
 }
 
 // Multiply the finite scales of the meta units that `keep(idx)` selects by 2^-a in place (idx = lane + 32 i: the (chunk,
@@ -333,7 +309,7 @@ __device__ __forceinline__ uint32_t b_prep(uint32_t x2, uint32_t s2, __half2 mse
 // scale taken down into the fp16 subnormals loses its low bits (those of scales below 2^(a - 14)).  The z rows are untouched.
 template <int NG, class KF>
 __device__ __forceinline__ void rescale_meta(uint4* mt, int a, int lane, KF&& keep) {
-    const float f = __uint_as_float((uint32_t)(127 - a) << 23);
+    const float f = pow2f(-a);
     auto sc = [&](uint32_t w, bool k0, bool k1) {
         const float2 x = __half22float2(u32_as_h2(w));
         return h2_as_u32(__floats2half2_rn(k0 ? x.x * f : 0.f, k1 ? x.y * f : 0.f));
@@ -371,17 +347,11 @@ __device__ __forceinline__ int qk_guard(uint8_t* st, int qexp, int nvalid, int l
     float m = fmaxf(__low2float(m2), __high2float(m2));
     #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    const int fm = exp2_floor(m), e = qexp + fm;
+    const int fm = floor_log2f(m), e = qexp + fm;
     if (!(m > 0.f) || qexp == -127 || (e >= -4 && e <= 14)) return 0;
     const int a = max(e - 13, fm - 14);
     rescale_meta<NG>(mt, a, lane, valid);
     return a;
-}
-
-// exact power of two 2^(24 - P) that undoes the denormal scaling of the fields of MMA mm
-template <int BITS>
-__device__ __forceinline__ float inv_pos_scale(int mm) {
-    return __uint_as_float((uint32_t)(127 + 24 - Lay<BITS>::bitpos(mm % Lay<BITS>::F)) << 23);
 }
 
 // column bookkeeping of the B fragments (G query heads, NG outer groups per block)
@@ -411,9 +381,8 @@ __device__ __forceinline__ void mma_half(const uint8_t* st, int c0, XF&& getx, f
     const int hb = (g8 % (2 * G)) >> 1;                 // head of this lane's B column
     const int gi = g8 / (2 * G);                        // group-in-fragment of this lane's B column
     const int gz = min(g8 >> 1, NG - 1);                // group of this lane's A rows in the zero-term MMA
-    const __half2 msel = (g8 & 1) ? __float2half2_rn(-1.f) : __float2half2_rn(0.f);
+    const __half2 msel = b_mask(g8);
     const uint8_t* meta = st + kHalfChunks * L::kChunkBytes + t * 16;
-    constexpr uint32_t kField = ((1u << BITS) - 1u) * 0x00010001u;
     #pragma unroll (kChunkUnroll)
     for (int cl = 0; cl < kHalfChunks; ++cl) {
         uint32_t xa, xb;
@@ -443,29 +412,9 @@ __device__ __forceinline__ void mma_half(const uint8_t* st, int c0, XF&& getx, f
         for (int sl = 0; sl < L::kSlabs; ++sl) {
             const uint4 w4 = *reinterpret_cast<const uint4*>(st + (cl * L::kSlabs + sl) * 512 + lane * 16);
             const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
-            uint32_t wl4[4], wr4[4], wr6[4], wr8[4];    // the shifted copies a bit width needs (the others fold away)
-            #pragma unroll
-            for (int r = 0; r < 4; ++r) {                 // right shifts as IMAD.HI: the FMA pipe has room, the ALU pipe (LOP3) does not
-#if KIVI_SHIFT_IMAD
-                wl4[r] = w[r] << 4; wr4[r] = __umulhi(w[r], 1u << 28); wr6[r] = __umulhi(w[r], 1u << 26); wr8[r] = __umulhi(w[r], 1u << 24);
-#else
-                wl4[r] = w[r] << 4; wr4[r] = w[r] >> 4; wr6[r] = w[r] >> 6; wr8[r] = w[r] >> 8;
-#endif
-            }
-            #pragma unroll
-            for (int j = 0; j < L::F; ++j) {
-                uint32_t a[4];
-                #pragma unroll
-                for (int r = 0; r < 4; ++r) {
-                    const int sh = L::shr(j);
-                    const uint32_t src = sh == -4 ? wl4[r] : sh == 0 ? w[r] : sh == 4 ? wr4[r] : sh == 6 ? wr6[r] : wr8[r];
-                    a[r] = src & (kField << L::bitpos(j));
-                }
-                const int mm = sl * L::F + j;
-                const int f = ((16 * mm) / GS) / GPF;
-                if (INIT && cl == 0) mma_16816_init(acc[mm], a[0], a[1], a[2], a[3], b0[f], b1[f]);
-                else mma_16816(acc[mm], a[0], a[1], a[2], a[3], b0[f], b1[f]);
-            }
+            auto bpair = [&](int mm) { const int f = ((16 * mm) / GS) / GPF; return make_uint2(b0[f], b1[f]); };
+            if (INIT && cl == 0) slab_mma<BITS, true>(w, sl, acc, bpair);
+            else slab_mma<BITS, false>(w, sl, acc, bpair);
         }
     }
 }
@@ -510,6 +459,7 @@ template <int BITS, int G, int GS, class EF>
 __device__ __forceinline__ void finalize(const float (&acc)[8][4], const float (&zsel)[Cols<G, GS>::NG], int lane,
                                          float post, EF&& emit)
 {
+    using L = Lay<BITS>;
     constexpr int GPF = Cols<G, GS>::GPF;
     const int g8 = lane >> 2, t = lane & 3;
     if (G == 1 && GS == 32) {
@@ -521,7 +471,7 @@ __device__ __forceinline__ void finalize(const float (&acc)[8][4], const float (
         #pragma unroll
         for (int v = 0; v < 4; ++v) {
             if (t == v) {
-                const float sl = inv_pos_scale<BITS>(2 * v) * post, sh = inv_pos_scale<BITS>(2 * v + 1) * post, zt = zsel[v] * post;
+                const float sl = L::field_scale((2 * v) % L::F) * post, sh = L::field_scale((2 * v + 1) % L::F) * post, zt = zsel[v] * post;
                 v0 = fmaf(acc[2 * v][0] + acc[2 * v][1], sl, zt);
                 v1 = fmaf(acc[2 * v][2] + acc[2 * v][3], sl, zt);
                 v2 = fmaf(acc[2 * v + 1][0] + acc[2 * v + 1][1], sh, zt);
@@ -542,8 +492,8 @@ __device__ __forceinline__ void finalize(const float (&acc)[8][4], const float (
             lo[e] = sel4(acc[0][e], acc[2][e], acc[4][e], acc[6][e], t1, t2);
             hi[e] = sel4(acc[1][e], acc[3][e], acc[5][e], acc[7][e], t1, t2);
         }
-        const float sl = sel4(inv_pos_scale<BITS>(0), inv_pos_scale<BITS>(2), inv_pos_scale<BITS>(4), inv_pos_scale<BITS>(6), t1, t2) * post;
-        const float sh = sel4(inv_pos_scale<BITS>(1), inv_pos_scale<BITS>(3), inv_pos_scale<BITS>(5), inv_pos_scale<BITS>(7), t1, t2) * post;
+        const float sl = sel4(L::field_scale(0), L::field_scale(2 % L::F), L::field_scale(4 % L::F), L::field_scale(6 % L::F), t1, t2) * post;
+        const float sh = sel4(L::field_scale(1), L::field_scale(3 % L::F), L::field_scale(5 % L::F), L::field_scale(7 % L::F), t1, t2) * post;
         const float zt = sel4(zsel[0], zsel[1], zsel[2], zsel[3], t1, t2) * post;
         const int o = 32 * t + g8;
         emit(0, o, fmaf(lo[0] + lo[1], sl, zt));
@@ -557,7 +507,7 @@ __device__ __forceinline__ void finalize(const float (&acc)[8][4], const float (
         for (int mm = 0; mm < 8; ++mm) {
             const int grp = (16 * mm) / GS;
             if (grp % GPF == gi_l) {
-                const float sc = inv_pos_scale<BITS>(mm) * post, zt = zsel[grp] * post;
+                const float sc = L::field_scale(mm % L::F) * post, zt = zsel[grp] * post;
                 emit(2 * mm, 16 * mm + g8, fmaf(acc[mm][0] + acc[mm][1], sc, zt));
                 emit(2 * mm + 1, 16 * mm + g8 + 8, fmaf(acc[mm][2] + acc[mm][3], sc, zt));
             }
@@ -1059,7 +1009,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
             if (h == (lane >> 2)) qpost_win = ps.y;
             qmx = fmaxf(qmx, mx * ps.x);
         }
-        const int qexp = exp2_floor(qmx);                                    // floor(log2) of the prescaled max|q| of the unit
+        const int qexp = floor_log2f(qmx);                                   // floor(log2) of the prescaled max|q| of the unit
         __syncwarp();
         if (left > n_here) fetch_q(unit + 1);                                // the range continues into the next unit
 
@@ -1101,10 +1051,10 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 gather_z<G, GS>(zc, lane, zsel);
                 float post = qpost_blk;
                 if (kshift) {                                                // the scales entered x 2^-kshift, the zero term as is
-                    const float dn = __uint_as_float((uint32_t)(127 - kshift) << 23);
+                    const float dn = pow2f(-kshift);
                     #pragma unroll
                     for (int grp = 0; grp < NG; ++grp) zsel[grp] *= dn;
-                    post *= __uint_as_float((uint32_t)(127 + kshift) << 23);
+                    post *= pow2f(kshift);
                 }
                 const int64_t rowi = uq0 + h_l;
                 __half* row = p.w.lg + rowi * p.w.ld + j * kBlockTokens;
@@ -1651,7 +1601,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                         #pragma unroll
                         for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
                         const int vshift = pv_vshift(m);
-                        boost = pv_boost(m * __uint_as_float((uint32_t)(127 - vshift) << 23));
+                        boost = pv_boost(m * pow2f(-vshift));
                         if (vshift)                                          // the end of the store: later slots hold no data
                             rescale_meta<NG>(const_cast<uint4*>(mt), vshift, lane, [&](int idx, int d) {
                                 return nt >= kPartTokens || 16 * ((idx >> 2) / NG) + 2 * (idx & 3) + d < nt; });
@@ -1703,11 +1653,12 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 if (!(boost_b | vshift_b)) {
                     finalize<VB, G, GS>(acc, zsel, lane, 1.f, [&](int slot, int, float v) { run[slot] += v; });
                 } else {                                                     // back to the x 2^6 of the running sums
-                    float post = 0.f;                                        // x 2^(v - e - b); the zero term entered without 2^-v
+                    int pe = 0;                                              // post = 2^(v - e - b); the zero term entered without 2^-v
                     #pragma unroll
                     for (int h = 0; h < G; ++h)
-                        if (h == h_l) post = __uint_as_float((uint32_t)(127 + vshift_b - (boost_b ? pv_extra_exp(S[h], boost_b) : 0)) << 23);
-                    const float zdn = __uint_as_float((uint32_t)(127 - vshift_b) << 23);
+                        if (h == h_l) pe = vshift_b - (boost_b ? pv_extra_exp(S[h], boost_b) : 0);
+                    const float post = pow2f(pe);
+                    const float zdn = pow2f(-vshift_b);
                     #pragma unroll
                     for (int grp = 0; grp < NG; ++grp) zsel[grp] *= zdn;
                     finalize<VB, G, GS>(acc, zsel, lane, post, [&](int slot, int, float v) { run[slot] += v; });

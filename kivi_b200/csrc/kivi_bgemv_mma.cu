@@ -49,22 +49,9 @@ __device__ __forceinline__ void cp_async4(void* dst, const void* src, int src_by
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N_> __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N_) : "memory"); }
 
-__device__ __forceinline__ uint32_t h2u(const __half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
-__device__ __forceinline__ __half2 u2h(const uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
-
-// B-fragment register: hi = fp16(x*s) in the even columns, lo = x*s - hi (exact) in the odd ones
-__device__ __forceinline__ uint32_t b_prep(uint32_t x2, uint32_t s2, bool lo_col) {
-    const __half2 x = u2h(x2), s = u2h(s2);
-    __half2 b = __hmul2(x, s);
-    if (lo_col) b = __hfma2(x, s, __hneg2(b));
-    return h2u(b);
-}
-
 template <int BITS, int G, int GS>
 struct Geo {
-    static constexpr int F = 16 / BITS;              // fields per half word = MMAs per slab
-    static constexpr int kWords = 128 / (2 * F);     // words per 128 outer indices: 8 / 16
-    static constexpr int kSlabs = kWords / 8;        // 1 / 2
+    static constexpr int kWords = 8 * Lay<BITS>::kSlabs;   // words per 128 outer indices: 8 / 16
     static constexpr int NG = 128 / GS;              // outer groups per tile: 4 / 2
     static constexpr int NP = NG * G;                // (group, head) column pairs of the one B fragment
     static_assert(NP <= 4, "one B fragment holds at most 4 (group, head) pairs");
@@ -75,19 +62,12 @@ struct Geo {
     static constexpr int kStage = kCodeBytes + 2 * kMetaBytes;
 };
 
-// exact power of two 2^(24 - P) that undoes the denormal scaling of field j
-template <int BITS>
-__device__ __forceinline__ float inv_pos(int j) {
-    return __uint_as_float((uint32_t)(127 + 24 - Lay<BITS>::bitpos(j)) << 23);
-}
-
 // power of two that brings max|x| into [16, 32): keeps hi = fp16(x*s) clear of overflow and its residual clear of the
 // fp16 denormal range (where the split would stop being exact); the result is rescaled by its exact inverse
 __device__ __forceinline__ float pow2_prescale(float mx) {
     if (!(mx > 0.f) || !(mx < 3.0e38f)) return 1.f;
-    const int e = (int)((__float_as_uint(mx) >> 23) & 0xff) - 127;    // floor(log2 mx) for normal fp32 (every fp16 is one)
-    const int k = max(-14, min(14, 4 - e));
-    return __uint_as_float((uint32_t)(127 + k) << 23);
+    const int k = max(-14, min(14, 4 - floor_log2f(mx)));
+    return pow2f(k);
 }
 
 // Per-tile window of the split.  The row prescale alone does not bound x*s: a large scale overflows hi = fp16(x*s) (a zero
@@ -102,8 +82,6 @@ __device__ __forceinline__ float pow2_prescale(float mx) {
 // non-finite in the reference as well; it does not set the factor of the tile's finite groups.
 constexpr int kSplitMinE = -4, kSplitMaxE = 13;
 
-__device__ __forceinline__ float pow2f(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
-__device__ __forceinline__ int f32_ilogb(float v) { return (int)((__float_as_uint(v) >> 23) & 0xff) - 127; }
 // floor(log2) of a finite non-zero fp16 from its magnitude bits m (0 < m < 0x7c00)
 __device__ __forceinline__ int h_ilogb(uint32_t m) { return m >= 0x400u ? (int)(m >> 10) - 15 : 31 - __clz(m) - 24; }
 // per-half max of fp16 magnitude bits (NaN > inf > every finite value)
@@ -117,40 +95,23 @@ __device__ __forceinline__ uint32_t hfin_max(uint32_t acc, uint32_t w) {
 __device__ __forceinline__ uint32_t warp_hmag_max(uint32_t v) { return __reduce_max_sync(0xffffffffu, max(v & 0xffffu, v >> 16)); }
 // fp16 pair times a power of two, through fp32 (the factor need not be an fp16)
 __device__ __forceinline__ uint32_t h2_scale(uint32_t w, float f) {
-    const float2 v = __half22float2(u2h(w));
-    return h2u(__floats2half2_rn(v.x * f, v.y * f));
+    const float2 v = __half22float2(u32_as_h2(w));
+    return h2_as_u32(__floats2half2_rn(v.x * f, v.y * f));
 }
 
 // One chunk of 16 inner indices on the tensor cores.  W[sl][r]: the lane's raw words of inner rows (t, t+4, t+8, t+12)[r],
 // word column 8 sl + g8.
-template <int BITS, int SLABS, bool INIT>
-__device__ __forceinline__ void chunk_mma(const uint32_t (&W)[SLABS][4], uint32_t b0, uint32_t b1, float (&acc)[8][4])
+template <int BITS, bool INIT>
+__device__ __forceinline__ void chunk_mma(const uint32_t (&W)[Lay<BITS>::kSlabs][4], uint32_t b0, uint32_t b1, float (&acc)[8][4])
 {
-    using L = Lay<BITS>;
-    constexpr int F = L::F;
-    constexpr uint32_t kField = ((1u << BITS) - 1u) * 0x00010001u;
     #pragma unroll
-    for (int sl = 0; sl < SLABS; ++sl) {
+    for (int sl = 0; sl < Lay<BITS>::kSlabs; ++sl) {
         uint32_t m[4];                                   // A registers before field isolation
         m[0] = prmt(W[sl][0], W[sl][1], 0x5410u);        // row g8,     k = 2t, 2t+1   (inner t, t+4):   low halves
         m[1] = prmt(W[sl][0], W[sl][1], 0x7632u);        // row g8 + 8, same k:                          high halves
         m[2] = prmt(W[sl][2], W[sl][3], 0x5410u);        // row g8,     k = 2t+8, 2t+9 (inner t+8, t+12)
         m[3] = prmt(W[sl][2], W[sl][3], 0x7632u);
-        uint32_t ml4[4], mr4[4], mr6[4], mr8[4];
-        #pragma unroll
-        for (int r = 0; r < 4; ++r) { ml4[r] = m[r] << 4; mr4[r] = m[r] >> 4; mr6[r] = m[r] >> 6; mr8[r] = m[r] >> 8; }
-        #pragma unroll
-        for (int j = 0; j < F; ++j) {
-            uint32_t a[4];
-            #pragma unroll
-            for (int r = 0; r < 4; ++r) {
-                const int sh = L::shr(j);
-                const uint32_t src = sh == -4 ? ml4[r] : sh == 0 ? m[r] : sh == 4 ? mr4[r] : sh == 6 ? mr6[r] : mr8[r];
-                a[r] = src & (kField << L::bitpos(j));
-            }
-            if (INIT) mma_16816_init(acc[sl * F + j], a[0], a[1], a[2], a[3], b0, b1);
-            else mma_16816(acc[sl * F + j], a[0], a[1], a[2], a[3], b0, b1);
-        }
+        slab_mma<BITS, INIT>(m, sl, acc, [&](int) { return make_uint2(b0, b1); });
     }
 }
 
@@ -185,7 +146,7 @@ wide_kernel(const Args a)
 {
     using GE = Geo<BITS, G, GS>;
     using WG = WideGeo<BITS, G, GS>;
-    constexpr int F = GE::F, SLABS = GE::kSlabs, NG = GE::NG, NP = GE::NP;
+    constexpr int F = Lay<BITS>::F, SLABS = Lay<BITS>::kSlabs, NG = GE::NG, NP = GE::NP;
     constexpr int TG = WG::kMetaRow / 2;                                     // groups per tile row: 16 / 8
     extern __shared__ __align__(128) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -213,13 +174,13 @@ wide_kernel(const Args a)
         for (int i = 0; i < 4; ++i) qlin[warp * 128 + lane + 32 * i] = xv[i] * ps;
         if (lane == 0) {
             xsc[warp] = 1.f / ps;
-            xex[warp] = !(mx < 3.0e38f) ? kNonFinite : mx == 0.f ? kZeroRow : f32_ilogb(mx * ps);
+            xex[warp] = !(mx < 3.0e38f) ? kNonFinite : mx == 0.f ? kZeroRow : floor_log2f(mx * ps);
         }
     }
     __syncthreads();
     if (warp < G) {                                                         // lane = (chunk c, t): rows 16c + t + {0, 4, 8, 12}
         const float* xl = qlin + warp * 128 + 16 * (lane >> 2) + (lane & 3);
-        q2[warp * 32 + lane] = make_uint2(h2u(__floats2half2_rn(xl[0], xl[4])), h2u(__floats2half2_rn(xl[8], xl[12])));
+        q2[warp * 32 + lane] = make_uint2(h2_as_u32(__floats2half2_rn(xl[0], xl[4])), h2_as_u32(__floats2half2_rn(xl[8], xl[12])));
     }
 
     const int n_tiles = cdiv(a.N, WG::kTileTok);
@@ -269,7 +230,7 @@ wide_kernel(const Args a)
 
     // this lane's B column: pair pi = g8 >> 1 = (group, head), hi | lo by the parity of g8
     const int pi_b = min(g8 >> 1, NP - 1), gam_b = pi_b / G, h_b = pi_b % G;
-    const bool lo_col = g8 & 1;
+    const __half2 msel = b_mask(g8);
     // this lane's accumulator columns 2 t4, 2 t4 + 1 = pair t4
     const int gam_c = t4 / G, h_c = t4 % G;
 
@@ -343,11 +304,11 @@ wide_kernel(const Args a)
                 }
                 const uint2 xq = q2[(h_b * 8 + c) * 4 + t4];
                 const int gcol = warp * NG + gam_b;
-                const uint32_t s01 = h2u(__halves2half2(ss[(r0) * TG + gcol], ss[(r0 + 4) * TG + gcol]));
-                const uint32_t s23 = h2u(__halves2half2(ss[(r0 + 8) * TG + gcol], ss[(r0 + 12) * TG + gcol]));
-                const uint32_t b0 = b_prep(xq.x, s01, lo_col), b1 = b_prep(xq.y, s23, lo_col);
-                if (c == 0) chunk_mma<BITS, SLABS, true>(W, b0, b1, acc);
-                else chunk_mma<BITS, SLABS, false>(W, b0, b1, acc);
+                const uint32_t s01 = h2_as_u32(__halves2half2(ss[(r0) * TG + gcol], ss[(r0 + 4) * TG + gcol]));
+                const uint32_t s23 = h2_as_u32(__halves2half2(ss[(r0 + 8) * TG + gcol], ss[(r0 + 12) * TG + gcol]));
+                const uint32_t b0 = b_prep(xq.x, s01, msel), b1 = b_prep(xq.y, s23, msel);
+                if (c == 0) chunk_mma<BITS, true>(W, b0, b1, acc);
+                else chunk_mma<BITS, false>(W, b0, b1, acc);
             }
             // zero term of this lane's pair: sum_d x_h[d] * z[d][gamma]   (the g8 lanes split the rows, butterfly sum)
             float zt = 0.f;
@@ -375,7 +336,7 @@ wide_kernel(const Args a)
                         __align__(16) __half o[2 * F];
                         #pragma unroll
                         for (int j = 0; j < F; ++j) {
-                            const float sc_j = inv_pos<BITS>(j) * rfac;
+                            const float sc_j = Lay<BITS>::field_scale(j) * rfac;
                             o[j] = __float2half_rn(fmaf(acc[sl * F + j][0] + acc[sl * F + j][1], sc_j, zt) * rs);
                             o[F + j] = __float2half_rn(fmaf(acc[sl * F + j][2] + acc[sl * F + j][3], sc_j, zt) * rs);
                         }
@@ -400,7 +361,7 @@ __global__ void __launch_bounds__(256, 2)
 tall_kernel(const Args a)
 {
     using GE = Geo<BITS, G, GS>;
-    constexpr int F = GE::F, SLABS = GE::kSlabs, NG = GE::NG, NP = GE::NP;
+    constexpr int F = Lay<BITS>::F, SLABS = Lay<BITS>::kSlabs, NG = GE::NG, NP = GE::NP;
     extern __shared__ __align__(128) uint8_t smem[];
     cg::cluster_group cluster = cg::this_cluster();
     const int S = (int)cluster.num_blocks(), crank = (int)cluster.block_rank();
@@ -487,7 +448,7 @@ tall_kernel(const Args a)
     };
 
     const int pi_b = min(g8 >> 1, NP - 1), gam_b = pi_b / G, h_b = pi_b % G;
-    const bool lo_col = g8 & 1;
+    const __half2 msel = b_mask(g8);
     const int gam_c = t4 / G, h_c = t4 % G;
     float run[SLABS][2 * F];                                                // the lane's outputs (useful lanes only), summed over its tiles
     #pragma unroll
@@ -536,7 +497,7 @@ tall_kernel(const Args a)
                 }
                 xq[h] = max(m & 0xffffu, m >> 16);
             }
-            const uint32_t q = h2u(__hmul2(u2h(xq[0] | (xq[G - 1] << 16)), u2h(sm)));
+            const uint32_t q = h2_as_u32(__hmul2(u32_as_h2(xq[0] | (xq[G - 1] << 16)), u32_as_h2(sm)));
             const bool big = __vcmpgeu2(q, 0x7c007c00u) != 0;                // 2^(kSplitMaxE + 2) is past fp16's range
             const uint32_t small = __vcmpltu2(q, 0x2c002c00u);              // per head: below 2^kSplitMinE
             trig = __any_sync(0xffffffffu, big);
@@ -572,7 +533,7 @@ tall_kernel(const Args a)
                     x[i] = __half2float(xh);
                 }
                 m = min(__reduce_max_sync(0xffffffffu, m), 0x7bffu);
-                const int eps = f32_ilogb(xsc[h]);                          // log2 of the row prescale
+                const int eps = floor_log2f(xsc[h]);                        // log2 of the row prescale
                 const int ecx = m != 0 ? 4 - h_ilogb(m) : eps;              // max|x| into [16, 32)
                 const float cx = pow2f(ecx);
                 #pragma unroll
@@ -593,12 +554,12 @@ tall_kernel(const Args a)
                 for (int r = 0; r < 4; ++r)
                     W[sl][r] = *reinterpret_cast<const uint32_t*>(sc + (r0 + 4 * r) * GE::kRowBytes + (sl * 8 + g8) * 4);
             const __half* xh = xb + h_b * 128;
-            const uint32_t x01 = h2u(__halves2half2(xh[r0], xh[r0 + 4])), x23 = h2u(__halves2half2(xh[r0 + 8], xh[r0 + 12]));
-            const uint32_t s01 = h2u(__halves2half2(ss[(r0) * NG + gam_b], ss[(r0 + 4) * NG + gam_b]));
-            const uint32_t s23 = h2u(__halves2half2(ss[(r0 + 8) * NG + gam_b], ss[(r0 + 12) * NG + gam_b]));
-            const uint32_t b0 = b_prep(x01, s01, lo_col), b1 = b_prep(x23, s23, lo_col);
-            if (c == 0) chunk_mma<BITS, SLABS, true>(W, b0, b1, acc);
-            else chunk_mma<BITS, SLABS, false>(W, b0, b1, acc);
+            const uint32_t x01 = h2_as_u32(__halves2half2(xh[r0], xh[r0 + 4])), x23 = h2_as_u32(__halves2half2(xh[r0 + 8], xh[r0 + 12]));
+            const uint32_t s01 = h2_as_u32(__halves2half2(ss[(r0) * NG + gam_b], ss[(r0 + 4) * NG + gam_b]));
+            const uint32_t s23 = h2_as_u32(__halves2half2(ss[(r0 + 8) * NG + gam_b], ss[(r0 + 12) * NG + gam_b]));
+            const uint32_t b0 = b_prep(x01, s01, msel), b1 = b_prep(x23, s23, msel);
+            if (c == 0) chunk_mma<BITS, true>(W, b0, b1, acc);
+            else chunk_mma<BITS, false>(W, b0, b1, acc);
         }
         if (t4 < NP) {
             if (trig) {
@@ -623,7 +584,7 @@ tall_kernel(const Args a)
             for (int sl = 0; sl < SLABS; ++sl)
                 #pragma unroll
                 for (int j = 0; j < F; ++j) {
-                    const float sc_j = inv_pos<BITS>(j) * f;
+                    const float sc_j = Lay<BITS>::field_scale(j) * f;
                     run[sl][j] = fmaf(acc[sl * F + j][0] + acc[sl * F + j][1], sc_j, run[sl][j]);
                     run[sl][F + j] = fmaf(acc[sl * F + j][2] + acc[sl * F + j][3], sc_j, run[sl][F + j]);
                 }

@@ -49,6 +49,14 @@ struct CacheDesc {
 
 enum { ST_TK = 0, ST_R = 1, ST_TV = 2, ST_L = 3, ST_VHEAD = 4, ST_KVLEN = 5 };
 
+// ---- bit helpers of the packed-block contraction (decode attention, reference-layout GEMV) ------
+__device__ __forceinline__ uint32_t h2_as_u32(const __half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
+__device__ __forceinline__ __half2 u32_as_h2(const uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
+// 2^e as an fp32 built from its exponent bits (-126 <= e <= 127)
+__device__ __forceinline__ float pow2f(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
+// floor(log2 |x|) of a normal fp32 x from its exponent bits (-127 for 0); every fp16 is a normal fp32
+__device__ __forceinline__ int floor_log2f(float x) { return (int)((__float_as_uint(x) >> 23) & 0xff) - 127; }
+
 template <int BITS>
 struct Lay {
     static constexpr int F = 16 / BITS;                  // fields per 16-bit half = MMAs per slab
@@ -67,6 +75,8 @@ struct Lay {
         return BITS == 2 ? (j < 2 ? -4 : (j < 5 ? 0 : 6)) : (j == 0 ? -4 : (j == 1 ? 0 : (j == 2 ? 4 : 8)));
     }
     __host__ __device__ static constexpr int bitpos(int j) { return BITS * j - shr(j); }
+    // exact power of two 2^(24 - P) that undoes the denormal scaling of field j
+    __device__ __forceinline__ static float field_scale(int j) { return pow2f(24 - bitpos(j)); }
 };
 
 __host__ __device__ inline int lay_code_bytes(int bits) { return bits == 2 ? 4096 : 8192; }
@@ -196,6 +206,67 @@ __device__ __forceinline__ void mma_16816_init(float (&c)[4], uint32_t a0, uint3
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%10,%10,%10};"
                  : "=f"(c[0]), "=f"(c[1]), "=f"(c[2]), "=f"(c[3])
                  : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "f"(0.f));
+}
+
+// ---- the packed-block contraction shared by the decode attention and the reference-layout GEMV ---
+// Build switches (A/B builds; they apply to both kernels):
+//   KIVI_BPREP2      1: b_prep is hi, then a PREDICATED fma(x, s, -hi) in the lo lanes (2 instructions); 0: branch-free 3
+//   KIVI_SHIFT_IMAD  1: slab_mma's right shifts as IMAD.HI (the FMA pipe has room, the ALU pipe (LOP3) does not); 0: SHF
+#ifndef KIVI_BPREP2
+#define KIVI_BPREP2 1
+#endif
+#ifndef KIVI_SHIFT_IMAD
+#define KIVI_SHIFT_IMAD 0
+#endif
+
+// One B-fragment register: a column with mask 0 gets hi = fp16(x*s), one with mask -1 (b_mask) gets lo = x*s - hi, exact
+// while it is not below fp16's smallest step (the callers prescale x where it would be).
+__device__ __forceinline__ uint32_t b_prep(uint32_t x2, uint32_t s2, __half2 msel) {
+    const __half2 x = u32_as_h2(x2), s = u32_as_h2(s2);
+#if KIVI_BPREP2
+    __half2 b = __hmul2(x, s);
+    if (h2_as_u32(msel) != 0u) b = __hfma2(x, s, __hneg2(b));   // lane-invariant predicate, negation folds into the HFMA2 operand
+    return h2_as_u32(b);
+#else
+    const __half2 nh = __hmul2(__hmul2(x, s), msel);         // nh = hi * (part ? -1 : 0);  b = fma(x, s, nh)
+    return h2_as_u32(__hfma2(x, s, nh));
+#endif
+}
+// the b_prep mask of the lane's B column: hi in the even columns (g8 = lane >> 2), lo in the odd ones.  {-1, -1} / {0, 0}
+// as bit constants, so that b_prep's test folds to g8 & 1.
+__device__ __forceinline__ __half2 b_mask(int g8) { return u32_as_h2((g8 & 1) ? 0xbc00bc00u : 0u); }
+
+// One slab on the tensor cores: w = the lane's four blocked A words of slab sl.  Its F fields are isolated as Lay<BITS>
+// prescribes and MMA j = sl * F + j accumulates into acc[mm] with the B registers bpair(mm) returns (uint2 {b0, b1}).
+// INIT: D = A * B instead of D += A * B.
+template <int BITS, bool INIT, class BF>
+__device__ __forceinline__ void slab_mma(const uint32_t (&w)[4], int sl, float (&acc)[8][4], BF&& bpair)
+{
+    using L = Lay<BITS>;
+    constexpr uint32_t kField = ((1u << BITS) - 1u) * 0x00010001u;
+    uint32_t wl4[4], wr4[4], wr6[4], wr8[4];    // the shifted copies a bit width needs (the others fold away)
+    #pragma unroll
+    for (int r = 0; r < 4; ++r) {
+#if KIVI_SHIFT_IMAD
+        wl4[r] = w[r] << 4; wr4[r] = __umulhi(w[r], 1u << 28); wr6[r] = __umulhi(w[r], 1u << 26); wr8[r] = __umulhi(w[r], 1u << 24);
+#else
+        wl4[r] = w[r] << 4; wr4[r] = w[r] >> 4; wr6[r] = w[r] >> 6; wr8[r] = w[r] >> 8;
+#endif
+    }
+    #pragma unroll
+    for (int j = 0; j < L::F; ++j) {
+        uint32_t a[4];
+        #pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int sh = L::shr(j);
+            const uint32_t src = sh == -4 ? wl4[r] : sh == 0 ? w[r] : sh == 4 ? wr4[r] : sh == 6 ? wr6[r] : wr8[r];
+            a[r] = src & (kField << L::bitpos(j));
+        }
+        const int mm = sl * L::F + j;
+        const uint2 b = bpair(mm);
+        if (INIT) mma_16816_init(acc[mm], a[0], a[1], a[2], a[3], b.x, b.y);
+        else mma_16816(acc[mm], a[0], a[1], a[2], a[3], b.x, b.y);
+    }
 }
 
 // four 8x8 b16 matrices from shared memory, each delivered TRANSPOSED: lane (g8, t) receives, of matrix i, the elements
