@@ -226,6 +226,24 @@ int kivi_decode_attention_ragged_f16(const kivi_cache_t* cache, const void* q, c
                                      int64_t workspace_bytes, void* dbg_logits, void* dbg_probs, int64_t dbg_stride,
                                      int max_kv_len, void* stream);
 
+/* The same step with a SLIDING WINDOW of `window` >= 1 tokens (Mistral's config.sliding_window; transformers keeps
+ * kv_idx > q_idx - window).  With T = kv_len + 1 the shared length including the new token, sequence b sees the positions
+ *   max(clamp(kv_start[b], 0, kv_len), T - window) <= p <= T - 1
+ * (kv_start NULL = no padding) -- the same result as an additive finfo(fp16).min at the other positions of `mask`, which
+ * keeps its meaning and may be combined with the window.  The window start moves every step and is computed on the device
+ * from `state`: the call is CUDA-graph capturable.  The packed blocks before block j0 = min(n_blocks, max(0, T - window)
+ * / 128) of each store lie wholly below the window: they are neither read nor counted in the work split, so the packed
+ * bytes read per unit are (n_kb - j0k) * block_bytes(k_bits, g) + (n_vb - j0v) * block_bytes(v_bits, g), plus the fp16
+ * windows (r + L) * 256 and the logits of the visible V blocks, at most ~ (window + 2 * 128) tokens' worth of each store
+ * instead of kv_len.  A partly visible block and the window items are masked in their epilogues.  dbg_logits is defined
+ * at the visible positions only; dbg_probs is 0 below the window start (entries of the blocks that are not read are
+ * not written: pass a zeroed buffer, as for the ragged entry).  The cache update is that of
+ * kivi_decode_attention_f16.  window < 1: KIVI_ERR_SHAPE. */
+int kivi_decode_attention_window_f16(const kivi_cache_t* cache, const void* q, const void* k_new, const void* v_new,
+                                     const int32_t* kv_start, int window, const void* mask, void* out, void* workspace,
+                                     int64_t workspace_bytes, void* dbg_logits, void* dbg_probs, int64_t dbg_stride,
+                                     int max_kv_len, void* stream);
+
 /* Test hook: the (unit, item) work split of the two decode kernels evaluated on the host (kernel 0 = q.K^T, 1 = p.V cost
  * model); a unit has n_b packed blocks, n_w window items and the new token.  out_lo: 2 * (W + 1) ints, (unit, item) of the first
  * position of every range and of the end; out_owner: NULL or one int per position.  Returns the number of ranges W. */
@@ -236,6 +254,13 @@ int kivi_debug_range_split(int n_units, int n_b, int n_w, int w_cap, int kernel,
  * issued / consumed: cap entries of 4 ints (warp, unit, item, half) each -- the copies the producer issues and the stages
  * the item loop waits on; n_out[0] / n_out[1] receive their counts.  Returns the number of ranges W or a KIVI_ERR_*. */
 int kivi_debug_ragged_items(int n_units, int n_b, int n_w, int w_cap, int kernel, const int* unit_start, int kv_len,
+                            int* issued, int* consumed, int64_t cap, int64_t* n_out);
+
+/* Test hook: the same replay for a call of kivi_decode_attention_window_f16 at shared length T (the new token at T - 1)
+ * with window >= 1.  n_b = the store's packed blocks; the item sequence of a unit starts at block j0 = min(n_b, max(0,
+ * T - window) / 128), and items are reported in the numbering of the whole store (item j0 = packed block j0, item n_b + i =
+ * window item i).  unit_start: NULL (no padding) or the kv_start of every unit's sequence. */
+int kivi_debug_window_items(int n_units, int n_b, int n_w, int w_cap, int kernel, const int* unit_start, int T, int window,
                             int* issued, int* consumed, int64_t cap, int64_t* n_out);
 
 /* Advance `state` by one token (the bookkeeping of :343-356, :386-399); once per step, all layers. */

@@ -8,6 +8,8 @@ A left-padded batch keeps one length for all sequences; `set_kv_start` names eac
 attention then skips the padding on the device (kivi_decode_attention_ragged_f16).  The same offsets let one batch row
 ("slot") take a new sequence while the others decode: `refill` writes a prompt right-aligned to the shared length,
 `release` idles a slot, and `shift` drops timeline positions that no live sequence sees any more.
+A cache built with `sliding_window` = W attends, like transformers' Mistral, to the last W positions only
+(kivi_decode_attention_window_f16): the packed blocks below the window are not read, and `shift` may drop them.
 """
 from __future__ import annotations
 
@@ -58,6 +60,7 @@ def _bind():
     _lib.bind("kivi_decode_workspace_bytes", i64, [P, i32])
     _lib.bind("kivi_decode_attention_f16", i32, [P, vp, vp, vp, vp, vp, vp, i64, vp, vp, i64, i32, vp])
     _lib.bind("kivi_decode_attention_ragged_f16", i32, [P, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, i64, i32, vp])
+    _lib.bind("kivi_decode_attention_window_f16", i32, [P, vp, vp, vp, vp, i32, vp, vp, vp, i64, vp, vp, i64, i32, vp])
     _lib.bind("kivi_cache_advance", i32, [P, vp])
     _lib.bind("kivi_cache_export_f16", i32, [P, i32, i32, i32, i32, i32] + [vp] * 9)
     _lib.bind("kivi_cache_import_f16", i32, [P, i32, i32, i32, i32] + [vp] * 9)
@@ -76,8 +79,11 @@ class KiviCache:
 
     def __init__(self, n_layers: int, batch: int, num_heads: int, num_kv_heads: int, head_dim: int = 128,
                  k_bits: int = 2, v_bits: int = 2, group_size: int = 32, residual_length: int = 128,
-                 max_tokens: int = 4096, device="cuda", overlap_prologue: bool = False, gqa_chunk: int = 0):
-        """overlap_prologue = KIVI_CACHE_OVERLAP_PROLOGUE of include/kivi_b200.h: promise that the kernel enqueued directly
+                 max_tokens: int = 4096, device="cuda", overlap_prologue: bool = False, gqa_chunk: int = 0,
+                 sliding_window: int | None = None):
+        """sliding_window = W: every step attends to the positions max(kv_start, T - W) .. T - 1 only (T = the length
+        including the new token; transformers' kv_idx > q_idx - W); None = the whole cache.
+        overlap_prologue = KIVI_CACHE_OVERLAP_PROLOGUE of include/kivi_b200.h: promise that the kernel enqueued directly
         before every decode_attention() call never writes this cache (true inside a decoder layer, where it produces
         q / k_new / v_new), so the q.K^T launch may overlap its tail.
         gqa_chunk = KIVI_CACHE_GQA_CHUNK: query heads of a KV head that share one work unit (0 = from the geometry)."""
@@ -85,6 +91,9 @@ class KiviCache:
         if head_dim != 128:
             raise NotImplementedError("kivi_b200 fused decode supports head_dim 128 (all models the reference ships)")
         assert residual_length % group_size == 0                     # models/llama_kivi.py:344
+        if sliding_window is not None and int(sliding_window) < 1:
+            raise ValueError(f"sliding_window must be a positive number of tokens or None, got {sliding_window}")
+        self.sliding_window = None if sliding_window is None else int(sliding_window)
         self.device = torch.device(device)
         _lib.require_cuda(torch.empty(0, device=self.device))
         self.n_layers, self.batch, self.num_heads, self.num_kv_heads = n_layers, batch, num_heads, num_kv_heads
@@ -177,8 +186,11 @@ class KiviCache:
         self.set_seq_start(seq, IDLE_START)
 
     def live_starts(self):
-        """{seq: start} of the sequences that see part of the cache (start < kv_len)."""
+        """{seq: start} of the sequences that see part of the cache (start < kv_len).  With a sliding window W the start
+        is the effective one of the next step, max(kv_start, kv_len + 1 - W): positions below it are seen by no one."""
         starts = self.kv_start_host if self.ragged else [0] * self.batch
+        if self.sliding_window is not None:
+            starts = [max(s, self.kv_len + 1 - self.sliding_window) for s in starts]
         return {b: s for b, s in enumerate(starts) if s < self.kv_len}
 
     def refill(self, layer: int, seq: int, k: torch.Tensor, v: torch.Tensor):
@@ -204,7 +216,7 @@ class KiviCache:
     def shift(self, tokens: int):
         """Drop the first `tokens` positions of the shared timeline in every layer (packed blocks move down; windows stay)
         and lower the lengths and every kv_start by as much.  tokens: a positive multiple of max(128, R), at most tk and tv.
-        Raises ValueError if a live sequence would lose a visible position (start < tokens)."""
+        Raises ValueError if a live sequence would lose a visible position (effective start < tokens, live_starts)."""
         q = max(128, self.residual_length)
         if tokens <= 0 or tokens % q != 0:
             raise ValueError(f"shift must be a positive multiple of {q}, got {tokens}")
@@ -269,7 +281,12 @@ class KiviCache:
                 dbg_logits.data_ptr() if dbg_logits is not None else None,
                 dbg_probs.data_ptr() if dbg_probs is not None else None, stride, self.max_tokens, _lib.stream_ptr(self.device))
         with torch.cuda.device(self.device):
-            if self.ragged:                                          # left-padded batch: padded blocks are skipped
+            if self.sliding_window is not None:                      # the blocks below the window are skipped
+                _lib.check(_lib.lib().kivi_decode_attention_window_f16(
+                    ctypes.byref(self._structs[layer]), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
+                    self.kv_start.data_ptr() if self.ragged else None, self.sliding_window, *args),
+                    "kivi_decode_attention_window_f16")
+            elif self.ragged:                                        # left-padded batch: padded blocks are skipped
                 _lib.check(_lib.lib().kivi_decode_attention_ragged_f16(
                     ctypes.byref(self._structs[layer]), q.data_ptr(), k_new.data_ptr(), v_new.data_ptr(),
                     self.kv_start.data_ptr(), *args), "kivi_decode_attention_ragged_f16")

@@ -23,7 +23,9 @@
 //   (fence.proxy.async orders its reads before the async write).
 //   Left-padded batches (RAGGED = true, kivi_decode_attention_ragged_f16): a per-sequence start offset read on the device;
 //   packed blocks wholly in the padding are skipped by producer and consumer alike (ragged_skip), partly padded blocks and
-//   window items are masked in their epilogues.  RAGGED = false is the unpadded kernel, without any of it.
+//   window items are masked in their epilogues.  A sliding window (kivi_decode_attention_window_f16) runs the same RAGGED
+//   kernels with a start that moves every step: the packed blocks wholly below it are not even part of the work split.
+//   RAGGED = false is the unpadded kernel, without any of it.
 //
 // Arithmetic of a packed block (128 inner x 128 outer, kivi_decode.cuh):
 //     sum_i x_i * (s_i,G * c_i,o + z_i,G) = sum_i (x_i * s_i,G) * c_i,o  +  sum_i x_i * z_i,G
@@ -239,16 +241,44 @@ struct AttnParams {
     Workspace w;
     int stage_bytes, spw /*stages per warp*/, hchunks, n_units, nw_eff /*warps that own an sv range*/;
     int max_kv_len;                     // what the workspace rows were sized for
+    int window;                         // sliding window W (RAGGED kernels): positions below T - W are invisible; 0 = none
 };
+
+// ------------------------------------------------------------------------------------------------
+// Sliding window (kivi_decode_attention_window_f16).  With T the shared length including the new token, sequence b sees the
+// positions max(kv_start[b], T - W) <= p <= T - 1.  The packed blocks wholly below T - W are left out of the item sequence of
+// every unit: its packed part starts at block j0 = min(n_blocks, max(0, T - W) / 128), computed per step from `state`, so the
+// work split counts only the blocks a call can see.  Items are numbered from there (item j = block j + j0); the first
+// visible block may still be partly below T - W and takes the masking epilogue of a padded block.
+// ------------------------------------------------------------------------------------------------
+__host__ __device__ __forceinline__ int clamp_start(int start, int kv_len) {
+    return start < 0 ? 0 : (start > kv_len ? kv_len : start);
+}
+// first visible position of a sequence whose kv_start is `start` (T = shared length with the new token; window 0 = none)
+__host__ __device__ __forceinline__ int visible_start(int start, int T, int window) {
+    const int s = clamp_start(start, T - 1);
+    return window > 0 && T - window > s ? T - window : s;
+}
+// first packed block of a unit's item sequence: the blocks before it lie wholly below T - W
+__host__ __device__ __forceinline__ int window_first_block(int T, int window, int n_blocks) {
+    if (window <= 0 || T - window <= 0) return 0;
+    const int j0 = (T - window) / kBlockTokens;
+    return j0 < n_blocks ? j0 : n_blocks;
+}
 
 struct Sched {                          // per-step constants, identical for every unit
     int tk, r, tv, L, vhead, T, seg1;
-    int n_kb, n_kr, n_vb, vr1, n_vr;
+    int n_kb, n_kr, n_vb, vr1, n_vr;    // n_kb / n_vb: the packed blocks in the item sequence (from FirstBlocks on)
     int ipu;                            // qk items per unit: K blocks, K window items, the new token
     int bpu;                            // sv pseudo-blocks per unit: V blocks, V window items, the new token
 };
 
-__device__ __forceinline__ Sched make_sched(const CacheDesc& c) {
+// first packed K / V block of the item sequences (0 without a window).  Kept out of Sched: the p.V kernel hands Sched to its
+// out-of-line cache-update callees by reference, and a larger struct would change the unpadded kernel's stack frame.
+struct FirstBlocks { int k, v; };
+
+// window = 0 (a compile-time 0 in the RAGGED = false kernels) numbers the items from block 0
+__device__ __forceinline__ Sched make_sched(const CacheDesc& c, int window, FirstBlocks& j0) {
     Sched s;
     s.tk = c.state[ST_TK]; s.r = c.state[ST_R]; s.tv = c.state[ST_TV]; s.L = c.state[ST_L]; s.vhead = c.state[ST_VHEAD];
     s.T = s.tk + s.r + 1;
@@ -260,6 +290,10 @@ __device__ __forceinline__ Sched make_sched(const CacheDesc& c) {
     s.n_vr = s.vr1 + cdiv(s.L - s.seg1, kResTile);
     s.ipu = s.n_kb + s.n_kr + 1;
     s.bpu = s.n_vb + s.n_vr + 1;
+    j0.k = window_first_block(s.T, window, s.n_kb);
+    j0.v = window_first_block(s.T, window, s.n_vb);
+    s.n_kb -= j0.k; s.ipu -= j0.k;
+    s.n_vb -= j0.v; s.bpu -= j0.v;
     return s;
 }
 
@@ -803,26 +837,25 @@ __host__ __device__ __forceinline__ void cursor_step(Cursor& cur, int per_unit, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Left-padded batches (kivi_decode_attention_ragged_f16).  Sequence b sees the positions p >= s_b = clamp(kv_start[b], 0,
-// kv_len) and the new token.  A packed block (K or V, 128 tokens) that lies wholly below s_b is neither copied nor contracted;
-// a partly padded block and every window item are masked in their epilogues (q.K^T: no statistics, p.V: probability 0).
-// The skip decision is ONE predicate that the producer (*_issue_next, through ragged_seek) and the consumer (the item loops)
-// both evaluate, so a warp waits on exactly the stages it has issued, in the same order (kivi_debug_ragged_items replays
-// both walks on the host).  The unpadded entry runs the RAGGED = false instantiations: none of this is in them.
+// Left-padded batches (kivi_decode_attention_ragged_f16) and sliding windows (kivi_decode_attention_window_f16).  Sequence b
+// sees the positions p >= s_b = visible_start(kv_start[b], T, W) and the new token.  A packed block (K or V, 128 tokens) that
+// lies wholly below s_b is neither copied nor contracted; a partly hidden block and every window item are masked in their
+// epilogues (q.K^T: no statistics, p.V: probability 0).  The skip decision is ONE predicate that the producer (*_issue_next,
+// through ragged_seek) and the consumer (the item loops) both evaluate, so a warp waits on exactly the stages it has issued,
+// in the same order (kivi_debug_ragged_items / kivi_debug_window_items replay both walks on the host).  Item j of a unit is
+// packed block j + j0 (j0 = window_first_block).  The unpadded entry runs the RAGGED = false instantiations: none of this is
+// in them.
 // ------------------------------------------------------------------------------------------------
-__host__ __device__ __forceinline__ int clamp_start(int start, int kv_len) {
-    return start < 0 ? 0 : (start > kv_len ? kv_len : start);
+__host__ __device__ __forceinline__ bool ragged_skip(int j, int n_b, int j0, int start) {
+    return j < n_b && (j + j0 + 1) * kBlockTokens <= start;
 }
-__host__ __device__ __forceinline__ bool ragged_skip(int j, int n_b, int start) {
-    return j < n_b && (j + 1) * kBlockTokens <= start;
-}
-// producer: move the cursor past the items that need no copy -- the new token and the wholly padded packed blocks.  False
-// when the range is exhausted.  start_of(unit) = the unit's clamped start.
+// producer: move the cursor past the items that need no copy -- the new token and the wholly hidden packed blocks.  False
+// when the range is exhausted.  start_of(unit) = the unit's visible start.
 template <class SF>
-__host__ __device__ __forceinline__ bool ragged_seek(Cursor& cur, int per_unit, int n_b, SF&& start_of) {
+__host__ __device__ __forceinline__ bool ragged_seek(Cursor& cur, int per_unit, int n_b, int j0, SF&& start_of) {
     while (cur.left > 0) {
         if (cur.j == per_unit - 1) { cur.j = 0; ++cur.unit; --cur.left; }
-        else if (cur.half == 0 && ragged_skip(cur.j, n_b, start_of(cur.unit))) { ++cur.j; --cur.left; }
+        else if (cur.half == 0 && ragged_skip(cur.j, n_b, j0, start_of(cur.unit))) { ++cur.j; --cur.left; }
         else return true;
     }
     return false;
@@ -863,10 +896,10 @@ __device__ __forceinline__ void fold_stats(float& m, float& s, const float (&x)[
 // ------------------------------------------------------------------------------------------------
 // q . K^T  (+ scale, mask, per-range softmax statistics)
 // ------------------------------------------------------------------------------------------------
-// the clamped start of work unit `unit` (its sequence's first visible position)
+// the visible start of work unit `unit` (its sequence's first visible position; kv_start NULL: no padding)
 __device__ __forceinline__ int unit_start(const AttnParams& p, const Sched& s, int unit) {
     const int u = p.hchunks == 1 ? unit : unit / p.hchunks;
-    return clamp_start(__ldg(p.kv_start + u / p.c.Hkv), s.T - 1);
+    return visible_start(p.kv_start ? __ldg(p.kv_start + u / p.c.Hkv) : 0, s.T, p.window);
 }
 // the same, held in the cursor: the producer asks once per unit
 __device__ __forceinline__ int cursor_start(Cursor& cur, const AttnParams& p, const Sched& s, int unit) {
@@ -875,12 +908,12 @@ __device__ __forceinline__ int cursor_start(Cursor& cur, const AttnParams& p, co
 }
 
 template <int KB, int GS, bool RAGGED>
-__device__ __forceinline__ void qk_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s,
+__device__ __forceinline__ void qk_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s, int j0,
                                               int lane, uint64_t pol)
 {
     const CacheDesc& c = p.c;
     if constexpr (RAGGED) {
-        if (!ragged_seek(cur, s.ipu, s.n_kb, [&](int un) { return cursor_start(cur, p, s, un); })) return;
+        if (!ragged_seek(cur, s.ipu, s.n_kb, j0, [&](int un) { return cursor_start(cur, p, s, un); })) return;
     } else {
         if (cur.left > 0 && cur.j == s.ipu - 1) {                 // the new token needs no load
             cur.j = 0; ++cur.unit; --cur.left;
@@ -895,7 +928,7 @@ __device__ __forceinline__ void qk_issue_next(Pipe& pp, Cursor& cur, const AttnP
         if (cur.j < s.n_kb) {
             constexpr int cb = kHalfChunks * Lay<KB>::kChunkBytes;    // codes of a stage-item
             const int mb = lay_meta_bytes(GS) / kParts;
-            const uint8_t* blk = c.k_store + ((int64_t)u * c.k_cap_blocks + cur.j) * lay_block_bytes(KB, GS);
+            const uint8_t* blk = c.k_store + ((int64_t)u * c.k_cap_blocks + cur.j + j0) * lay_block_bytes(KB, GS);
             mbar_expect_tx(bar, (uint32_t)(cb + mb));
             if (kParts == 1) {
                 bulk_g2s(dst, blk, (uint32_t)(cb + mb), bar, pol);    // codes and meta are contiguous: one copy
@@ -929,7 +962,8 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     float* qlin = reinterpret_cast<float*>(ptr + kCW * G * 32 * 8) + warp * (G * kD);   // per warp: [G][128] fp32
 
     __shared__ Ranges<CostQK> rg_sh;                                         // items of the whole job over the range owners
-    const Sched s = make_sched(c);
+    FirstBlocks j0;
+    const Sched s = make_sched(c, RAGGED ? p.window : 0, j0);
     if (tid < n_stages) { mbar_init(&full_all[tid], 1); mbar_fence_init(); } // one stage barrier per thread, the work split beside them
     if (tid == kThreads - 1) rg_sh.init(p.n_units, s.n_kb, s.n_kr, p.nw_eff);
     __syncthreads();                                                         // the only CTA barrier: mbarrier init, work split
@@ -953,7 +987,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     // ONE stage goes out before the grid-dependency wait (the packed cache does not depend on the predecessor); the others
     // follow the q fetch below: issued after all of a warp's first stages, the few q words would queue behind the first-stage
     // copies every warp of the grid requests at this moment and arrive last.
-    for (int i = 0; i < (Lat<G>::q_first ? 1 : p.spw); ++i) qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
+    for (int i = 0; i < (Lat<G>::q_first ? 1 : p.spw); ++i) qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, j0.k, lane, pol);
 
     constexpr int NG = Cols<G, GS>::NG;
     const int ratio = c.H / c.Hkv;
@@ -976,7 +1010,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     pdl_wait();                                                              // q / k_new come from the previous kernel of the stream
     fetch_q(unit);
     if (Lat<G>::q_first)
-        for (int i = 1; i < p.spw; ++i) qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
+        for (int i = 1; i < p.spw; ++i) qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, j0.k, lane, pol);
     KIVI_TL(0, gw, 1);
     #pragma unroll 1
     while (left > 0) {
@@ -1020,9 +1054,10 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
         #pragma unroll 1
         for (int k = 0; k < n_here; ++k, ++j) {
             if constexpr (RAGGED) {
-                if (ragged_skip(j, s.n_kb, start)) continue;                 // wholly padded: never copied (qk_issue_next)
+                if (ragged_skip(j, s.n_kb, j0.k, start)) continue;          // wholly hidden: never copied (qk_issue_next)
             }
             if (j < s.n_kb) {                                                // ---- packed K block (tensor cores)
+                const int jb = j + j0.k;                                    // its index in the store
                 float acc[8][4];
                 float zc[4];
                 if (kParts > 1) {                                            // whole-block stages start from D = A * B instead
@@ -1038,14 +1073,14 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 #pragma unroll 1
                 for (int half = 0; half < kParts; ++half) {
                     pp.wait();
-                    kshift = qk_guard<KB, GS>(pp.cons(), qexp, s.tk - j * kBlockTokens, lane);
+                    kshift = qk_guard<KB, GS>(pp.cons(), qexp, s.tk - jb * kBlockTokens, lane);
                     mma_half<KB, G, GS, kParts == 1>(pp.cons(), half * kHalfChunks, [&](int cc, int h, uint32_t& xa, uint32_t& xb) {
                         const uint2 v = q2[(h * 8 + cc) * 4 + t4];
                         xa = v.x; xb = v.y;
                     }, acc, zc, lane);
                     __syncwarp();
                     pp.pop();
-                    qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
+                    qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, j0.k, lane, pol);
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
@@ -1057,9 +1092,9 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     post *= pow2f(kshift);
                 }
                 const int64_t rowi = uq0 + h_l;
-                __half* row = p.w.lg + rowi * p.w.ld + j * kBlockTokens;
-                const int nvalid = s.tk - j * kBlockTokens;                  // < 128 only in the last block when R < 128
-                const bool padded = RAGGED && j * kBlockTokens < start;      // partly padded: the masking epilogue
+                __half* row = p.w.lg + rowi * p.w.ld + jb * kBlockTokens;
+                const int nvalid = s.tk - jb * kBlockTokens;                 // < 128 only in the last block when R < 128
+                const bool padded = RAGGED && jb * kBlockTokens < start;     // partly hidden: the masking epilogue
                 // the lane's logits by compile-time slot; slots of MMAs this lane does not own and tokens past the packed
                 // length stay -inf.  ONE arithmetic for the production and the instrumented / masked / partial-block
                 // epilogues (same fold order, hence bit-identical statistics): they differ only in predicated side work.
@@ -1076,10 +1111,10 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     finalize<KB, G, GS>(acc, zsel, lane, post, [&](int slot, int o, float v) {
                         if (o < nvalid) {
                             __half hv = scale_logit(v);                      // fp16 scaled (+ mask): the softmax input
-                            if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + j * kBlockTokens + o);
+                            if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + jb * kBlockTokens + o);
                             row[o] = hv;
-                            if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + j * kBlockTokens + o] = hv;
-                            if (!padded || j * kBlockTokens + o >= start) x[slot] = __half2float(hv);   // padding: no value
+                            if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + jb * kBlockTokens + o] = hv;
+                            if (!padded || jb * kBlockTokens + o >= start) x[slot] = __half2float(hv);   // hidden: no value
                         }
                     });
                 }
@@ -1104,7 +1139,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 __syncwarp();
                 pp.pop();
-                qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, lane, pol);
+                qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, j0.k, lane, pol);
                 // lane (g8 < G, t): head g8, tokens 2t, 2t+1 (tile 0) and 8+2t, 9+2t (tile 1)
                 if (g8 < G) {
                     const int64_t rowi = uq0 + g8;
@@ -1208,7 +1243,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 if (pj < s.n_vb) {
                     if (lane == 0) {
                         const int u_ = p.hchunks == 1 ? pu : pu / p.hchunks;
-                        bulk_prefetch_l2(c.v_store + ((int64_t)u_ * c.v_cap_blocks + pj) * lay_block_bytes(c.v_bits, GS),
+                        bulk_prefetch_l2(c.v_store + ((int64_t)u_ * c.v_cap_blocks + pj + j0.v) * lay_block_bytes(c.v_bits, GS),
                                          (uint32_t)lay_block_bytes(c.v_bits, GS));
                     }
                     ++pj;
@@ -1241,12 +1276,12 @@ __device__ __forceinline__ void wait_unit_ready(const AttnParams& p, const Sched
 }
 
 template <int VB, int G, int GS, bool RAGGED>
-__device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s,
+__device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s, int j0,
                                               int ratio, int lane, uint64_t pol, const Ranges<CostQK>& rq, int& ready_unit)
 {
     const CacheDesc& c = p.c;
     if constexpr (RAGGED) {
-        if (!ragged_seek(cur, s.bpu, s.n_vb, [&](int un) { return cursor_start(cur, p, s, un); })) return;
+        if (!ragged_seek(cur, s.bpu, s.n_vb, j0, [&](int un) { return cursor_start(cur, p, s, un); })) return;
     } else {
         if (cur.left > 0 && cur.j == s.bpu - 1) {                 // the new token needs no load
             cur.j = 0; ++cur.unit; --cur.left;
@@ -1262,7 +1297,7 @@ __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnP
         if (cur.j < s.n_vb) {
             constexpr int cb = kHalfChunks * Lay<VB>::kChunkBytes;    // codes of a stage-item
             const int mb = lay_meta_bytes(GS) / kParts;
-            const uint8_t* blk = c.v_store + ((int64_t)u * c.v_cap_blocks + cur.j) * lay_block_bytes(VB, GS);
+            const uint8_t* blk = c.v_store + ((int64_t)u * c.v_cap_blocks + cur.j + j0) * lay_block_bytes(VB, GS);
             mbar_expect_tx(bar, (uint32_t)(cb + mb + G * kPartTokens * 2));
             if (kParts == 1) {
                 bulk_g2s(dst, blk, (uint32_t)(cb + mb), bar, pol);    // codes and meta are contiguous: one copy
@@ -1273,7 +1308,7 @@ __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnP
             const int uq0 = u * ratio + hc * G;
             for (int h = 0; h < G; ++h)                               // the logits of the item's tokens (workspace rows)
                 bulk_g2s(dst + cb + mb + h * kPartTokens * 2,
-                         p.w.lg + (int64_t)(uq0 + h) * p.w.ld + cur.j * kBlockTokens + cur.half * kPartTokens,
+                         p.w.lg + (int64_t)(uq0 + h) * p.w.ld + (cur.j + j0) * kBlockTokens + cur.half * kPartTokens,
                          kPartTokens * 2, bar, pol);
         } else {
             const int i = cur.j - s.n_vb;
@@ -1326,7 +1361,8 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
 
     __shared__ Ranges<CostSV> rg_sh;                                         // this kernel's work split
     __shared__ Ranges<CostQK> rq_sh;                                         // the q.K^T kernel's (statistics slots per unit)
-    const Sched s = make_sched(c);
+    FirstBlocks j0;
+    const Sched s = make_sched(c, RAGGED ? p.window : 0, j0);
     if (tid < n_stages) { mbar_init(&full_all[tid], 1); mbar_fence_init(); } // one stage barrier per thread, the work splits beside them
     if (tid == kThreads - 1) rg_sh.init(p.n_units, s.n_vb, s.n_vr, p.nw_eff);
     if (tid == kThreads - 33) rq_sh.init(p.n_units, s.n_kb, s.n_kr, p.nw_eff);
@@ -1422,7 +1458,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         }
         pp.push();
     }
-    for (int i = commit_async ? 1 : 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+    for (int i = commit_async ? 1 : 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
     KIVI_TL(1, gw, 1);
     if (commit_async) {
         pp.wait();
@@ -1434,12 +1470,12 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         if (s.L + 1 > c.R) in.vold = *reinterpret_cast<const uint2*>(st + 512 + 2 * (win_off(s.vhead, lane * 4) - s.vhead * kD));
         __syncwarp();
         pp.pop();
-        sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);     // the freed stage takes the next item at once
+        sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);     // the freed stage takes the next item at once
         commit_unit<KB, VB>(p, s, cu0, lane, scratch, in);
         for (int uu = cu0 + 1; uu < cu1; ++uu) commit_unit<KB, VB>(p, s, uu, lane, scratch, commit_fetch(p, s, uu, lane));
     }
 #else
-    for (int i = 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+    for (int i = 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
     KIVI_TL(1, gw, 1);
 #if KIVI_EARLY_COMMIT && KIVI_COMMIT_LATE && !KIVI_COMMIT_IN_QK
     commit_share();
@@ -1560,7 +1596,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         #pragma unroll 1
         for (int k = 0; k < n_here; ++k, ++j) {
             if constexpr (RAGGED) {
-                if (ragged_skip(j, s.n_vb, start)) continue;                 // wholly padded: never copied (sv_issue_next)
+                if (ragged_skip(j, s.n_vb, j0.v, start)) continue;          // wholly hidden: never copied (sv_issue_next)
             }
             if (j < s.n_vb) {                                                // ---- packed V block (tensor cores)
                 float acc[8][4];
@@ -1577,7 +1613,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 int boost = 0;                                               // pv_boost of the block (warp-uniform)
                 #pragma unroll 1
                 for (int half = 0; half < kParts; ++half) {
-                    const int t0 = j * kBlockTokens + half * kPartTokens, nt = s.tv - t0;   // nt >= kPartTokens except at the end of the store
+                    const int t0 = (j + j0.v) * kBlockTokens + half * kPartTokens, nt = s.tv - t0;   // nt >= kPartTokens except at the end of the store
                     pp.wait();
                     uint8_t* st = pp.cons();
                     __half* prob = reinterpret_cast<__half*>(st + kHalfBytes);   // [G][kPartTokens] logits -> scaled probabilities
@@ -1643,7 +1679,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     }, acc, zc, lane);
                     __syncwarp();
                     pp.pop();
-                    sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+                    sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
@@ -1679,15 +1715,18 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 for (int h = 0; h < G; ++h) {
                     pl[h] = 0.f;
                     if (lane < nt) {
-                        float x;
-                        if (win_bulk) {
+                        // below the start the workspace may hold logits no q.K^T range wrote in this step: never used
+                        const bool hidden = RAGGED && s.tv + l0 + lane < start;
+                        float x = 0.f;
+                        if (hidden) {
+                        } else if (win_bulk) {
                             const int off = (int)(((int64_t)(uq0 + h) * p.w.ld + s.tv + l0) & 7);
                             x = __half2float(reinterpret_cast<const __half*>(st + kResBytes + h * 64)[off + lane]);
                         } else {
                             x = __half2float(__ldcg(p.w.lg + (int64_t)(uq0 + h) * p.w.ld + s.tv + l0 + lane));
                         }
                         __half pr = __float2half_rn(prob_f32(x, M[h], nMl[h], S[h], rS[h]));
-                        if (RAGGED && s.tv + l0 + lane < start) pr = __float2half_rn(0.f);   // padding: probability 0
+                        if (hidden) pr = __float2half_rn(0.f);                   // hidden: probability 0
                         if (p.dbg_probs) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + s.tv + l0 + lane] = pr;
                         pl[h] = __half2float(pr);
                     }
@@ -1721,7 +1760,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 __syncwarp();
                 pp.pop();
-                sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, ratio, lane, pol, rq, ready_unit);
+                sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
                 // lane (g8, t): oacc[mt] = D[16mt + g8 | + 8][heads 2t, 2t+1] -> channel order through shared memory
                 #pragma unroll
                 for (int mt = 0; mt < 8; ++mt)
@@ -1905,11 +1944,11 @@ static int dispatch_attention_g(AttnParams& p, int G, bool overlap_prologue, cud
     return KIVI_ERR_GROUP;
 }
 
-// kv_start == NULL runs the instantiations without any padding logic
+// kv_start == NULL without a window runs the instantiations without any padding logic
 template <int KB, int VB>
 static int dispatch_attention(AttnParams& p, int G, bool overlap_prologue, cudaStream_t st)
 {
-    if (p.kv_start) return dispatch_attention_g<KB, VB, true>(p, G, overlap_prologue, st);
+    if (p.kv_start || p.window > 0) return dispatch_attention_g<KB, VB, true>(p, G, overlap_prologue, st);
     return dispatch_attention_g<KB, VB, false>(p, G, overlap_prologue, st);
 }
 

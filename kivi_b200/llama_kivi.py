@@ -190,6 +190,22 @@ def rope_settings(config):
     return theta, scaling
 
 
+def sliding_window(config):
+    """The sliding window W of a config (config.sliding_window; None or absent = attention over the whole cache).  A
+    config whose `layer_types` mixes attention kinds (per-layer windows) raises NotImplementedError; one whose layers are
+    all full attention has no window."""
+    kinds = set(getattr(config, "layer_types", None) or ())
+    if len(kinds) > 1:
+        raise NotImplementedError(f"layer_types {sorted(kinds)}: per-layer attention kinds (sliding windows on some layers "
+                                  "only) are not supported")
+    w = getattr(config, "sliding_window", None)
+    if w is None or kinds == {"full_attention"}:
+        return None
+    if int(w) != w or int(w) < 1:
+        raise ValueError(f"sliding_window must be a positive number of tokens or None, got {w!r}")
+    return int(w)
+
+
 def _rope_tables(head_dim, max_pos, theta, device, scaling=None):
     """fp16 cos / sin [max_pos, head_dim].  The inverse frequencies follow transformers' RoPE initialisers (default, linear,
     llama3) op for op in fp32, so the tables are the ones its rotary embedding produces."""
@@ -250,7 +266,8 @@ class LlamaFlashAttention_KIVI(nn.Module):
 
     def _prompt_attention(self, q, k, v, attention_mask):
         """Attention over the prompt itself (the reference calls flash-attn here, models/llama_kivi.py:401-423; off the
-        decode hot path): causal, plus the additive mask [B, 1, q_len, q_len] when the batch is padded."""
+        decode hot path): causal, plus the additive mask [B, 1, q_len, q_len] when the batch is padded or a sliding window
+        cuts the prompt (_additive_mask; the mask takes q_len^2 elements per sequence)."""
         kk, vv = repeat_kv(k, self.num_key_value_groups), repeat_kv(v, self.num_key_value_groups)
         if attention_mask is None:
             return F.scaled_dot_product_attention(q, kk, vv, is_causal=True)
@@ -373,19 +390,31 @@ _P2P_SAMPLING = ("sampling with enable_token_allgather(mode='p2p'): the fused ar
                  "use mode='nccl', which gathers the sampled ids")
 
 
-def _additive_mask(attention_mask, q_len: int, total: int, dtype, device):
-    """HF padding mask [B, total] (1 = attend) -> additive [B, 1, q_len, total] with the causal structure, or None
-    when nothing is masked; a 4-D additive mask passes through (what the reference's hook receives, :364-372)."""
-    if attention_mask is None:
-        return None
-    if attention_mask.dim() == 4:
+def _additive_mask(attention_mask, q_len: int, total: int, dtype, device, window: int | None = None, batch: int = 1):
+    """HF padding mask [B, total] (1 = attend; None = no padding) -> additive [B, 1, q_len, total] with the causal
+    structure, or None when nothing is masked; a 4-D additive mask passes through (what the reference's hook receives,
+    :364-372).  window = W (a sliding window): query i, at position total - q_len + i, also drops the keys at or below
+    its position - W (transformers' kv_idx > q_idx - W); `batch` sizes the mask when there is no padding mask."""
+    if attention_mask is not None and attention_mask.dim() == 4:
         return attention_mask
-    keep = attention_mask[:, None, None, :total].to(torch.bool)
-    if q_len == 1 and bool(keep.all()):
+    cut = window is not None and total > window                           # some query loses keys to the window
+    if attention_mask is None:
+        if not cut:
+            return None
+        B = batch
+        keep = torch.ones((1, 1, 1, total), dtype=torch.bool, device=device)
+    else:
+        keep = attention_mask[:, None, None, :total].to(torch.bool)
+        B = keep.shape[0]
+    if q_len == 1 and not cut and bool(keep.all()):
         return None
-    if q_len > 1:
+    if q_len > 1 or cut:
         causal = torch.ones((q_len, total), dtype=torch.bool, device=device).tril(total - q_len)
+        if cut:
+            causal = causal & ~causal.tril(total - q_len - window)
         keep = keep & causal
+        if attention_mask is None:
+            keep = keep.expand(B, 1, q_len, total)
     else:
         keep = keep.expand(-1, 1, 1, total)
     return torch.zeros(keep.shape, dtype=dtype, device=device).masked_fill(~keep, torch.finfo(dtype).min)
@@ -448,6 +477,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             raise NotImplementedError(f"head_dim {head_dim} (hidden_size {config.hidden_size}, {config.num_attention_heads} "
                                       "heads): only head_dim = hidden_size / num_attention_heads = 128 is supported")
         rope_settings(config)                                   # an unsupported RoPE type is refused here, not at the first forward
+        self.sliding_window = sliding_window(config)            # per-layer windows are refused here
         self.config = config
         self.vocab_size = config.vocab_size
         self.tensor_parallel = tensor_parallel
@@ -544,14 +574,17 @@ class LlamaForCausalLM_KIVI(nn.Module):
         return super()._apply(fn, *args, **kwargs)
 
     # ------------------------------------------------------------------ helpers
-    def _tables(self, device):
-        rows = getattr(self.config, "max_position_embeddings", 4096)
+    def _tables(self, device, positions: int = 0):
+        """cos / sin tables with a row for every position the cache can reach, and at least `positions` rows (a rolling
+        generate() reaches positions beyond its cache).  Rebuilding them drops the captured step, which reads them."""
+        rows = max(getattr(self.config, "max_position_embeddings", 4096), positions)
         if self.cache is not None:
             rows = max(rows, self.cache.max_tokens + 1)   # a cache longer than the config's context still has its rows
         if self._rope is None or self._rope[0].device != device or self._rope[0].shape[0] < rows:
             hd = self.config.hidden_size // self.config.num_attention_heads
             theta, scaling = rope_settings(self.config)
             self._rope = _rope_tables(hd, rows, theta, device, scaling)
+            self._graph = None
         return self._rope
 
     def _run_layers(self, input_ids, positions, pasts, attention_mask=None, store_kv=None):
@@ -593,7 +626,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             if start + q_len > rows:            # the slow path's index_select would raise; say why
                 raise ValueError(f"{start + q_len} positions exceed config.max_position_embeddings = {rows}")
             dtype = self.lm_head.weight.dtype
-            mask = _additive_mask(attention_mask, q_len, start + q_len, dtype, input_ids.device)
+            mask = _additive_mask(attention_mask, q_len, start + q_len, dtype, input_ids.device, self.sliding_window, B)
             h, pasts = self._run_layers(input_ids, position_ids, past_key_values, mask)
             logits = self.lm_head(h).float()                                     # logits.float() (:881)
         if return_dict is None:
@@ -686,7 +719,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self.cache = KiviCache(cfg.num_hidden_layers, batch, a.num_heads, a.num_key_value_heads,
                                a.head_dim, cfg.k_bits, cfg.v_bits, cfg.group_size,
                                cfg.residual_length, max_tokens, device=dev,
-                               overlap_prologue=True)       # the attention call follows the layer's RoPE kernel
+                               overlap_prologue=True,       # the attention call follows the layer's RoPE kernel
+                               sliding_window=self.sliding_window)
         if self.tensor_parallel:
             self.cache.tensor_parallel = True
             if self._allreduce is None or self._allreduce.rows_max != batch:
@@ -743,13 +777,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 starts = None
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
-            h, _ = self._run_layers(input_ids, positions, None, store_kv=self.cache.prefill)
+            mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window, B)
+            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=self.cache.prefill)
             self._pos.fill_(n)
         else:
             am = attention_mask.to(input_ids.device)
             positions = am.long().cumsum(-1) - 1                            # prepare_inputs_for_generation (:908-948)
             positions.masked_fill_(am == 0, 1)
-            mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device)
+            mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window)
             h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=self.cache.prefill)
             starts = starts.to(self._pos.device)
             self._pos.copy_((n - starts).to(torch.long).view(B, 1))
@@ -768,7 +803,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if not 1 <= n <= T:
             raise ValueError(f"a prompt of {n} tokens does not fit the shared length {T} (1 <= n <= length)")
         positions = torch.arange(n, device=ids.device).unsqueeze(0)
-        h, _ = self._run_layers(ids, positions, None, store_kv=lambda layer, k, v: self.cache.refill(layer, seq, k, v))
+        mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, ids.device, self.sliding_window)
+        h, _ = self._run_layers(ids, positions, None, mask,
+                                store_kv=lambda layer, k, v: self.cache.refill(layer, seq, k, v))
         self._pos[seq] = n
         self.cache.set_seq_start(seq, T - n)
         return self.lm_head(h[0, -1]).float()
@@ -1039,6 +1076,18 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self.cache._mirror_advance()
         return self._logits
 
+    def _roll(self):
+        """Make room for one more step of a windowed model: drop the largest multiple of max(128, R) positions that no
+        live sequence sees at the next step (KiviCache.live_starts) and that the packed stores hold."""
+        c = self.cache
+        if c.sliding_window is None:
+            raise ValueError("KIVI cache capacity exceeded")
+        q = max(128, c.residual_length)
+        tokens = min([c.tk, c.tv] + list(c.live_starts().values())) // q * q
+        if tokens <= 0:
+            raise ValueError(f"KIVI cache capacity exceeded: no multiple of {q} positions lies below every window")
+        c.shift(tokens)
+
     @torch.no_grad()
     def generate(self, input_ids=None, max_new_tokens: int | None = None, use_graph: bool = True, attention_mask=None,
                  max_length: int | None = None, do_sample: bool = False, temperature=1.0, top_k=50, top_p=1.0, seed=0,
@@ -1049,7 +1098,10 @@ class LlamaForCausalLM_KIVI(nn.Module):
         defaults; scalars or one value per sequence, set_sampling) from the Philox streams of `seed`: the same seed gives
         the same ids, with or without the CUDA graph.  generate() sets the step's mode (set_sampling) to what this call asks
         for and leaves it so: a later decode_step() samples after do_sample=True and takes the argmax after do_sample=False.  attention_mask: an HF padding mask of a LEFT-padded batch
-        (prefill(); the decode steps skip each sequence's padding); right padding raises ValueError."""
+        (prefill(); the decode steps skip each sequence's padding); right padding raises ValueError.
+        A model with a sliding window W rolls its cache: it holds about max(prompt, W) + 2 max(128, R) positions, and
+        before a step that would not fit, the positions that fell out of every window are dropped (KiviCache.shift), so
+        the generated length is bounded by the RoPE tables rather than by cache memory."""
         if do_sample:
             sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
         if attention_mask is not None:
@@ -1059,8 +1111,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
             if max_length is None:
                 raise ValueError("generate() needs max_new_tokens or max_length")
             max_new_tokens = max_length - n
-        if self.cache is None or self.cache.batch != B or self.cache.max_tokens < n + max_new_tokens:
-            self.init_cache(B, n + max_new_tokens)
+        cap = n + max_new_tokens
+        if self.sliding_window is not None:
+            cap = min(cap, max(n, self.sliding_window) + 2 * max(128, self.config.residual_length))
+        if self.cache is None or self.cache.batch != B or self.cache.max_tokens < cap:
+            self.init_cache(B, cap)
+        self._tables(self.cache.device, n + max_new_tokens)                 # positions beyond a rolling cache
         # generate() owns the step's mode; it changes (and the captured step is dropped) only when do_sample does
         if do_sample:
             self.set_sampling(temperature, top_k, top_p, seed)
@@ -1071,6 +1127,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         tok = (self.sample_first(logits) if do_sample else self.first_tokens(logits)).view(B, 1)
         for _ in range(max_new_tokens - 1):
             out.append(tok)
+            if self.cache.kv_len + 1 > self.cache.max_tokens:
+                self._roll()
             self.decode_step(tok, use_graph=use_graph)
             tok = self.next_tokens.view(B, 1).clone()
         out.append(tok)
