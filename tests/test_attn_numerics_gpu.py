@@ -9,7 +9,7 @@ and huge V under flat, spread and peaked softmaxes, a peaked token in each kind 
 fp16 V ring, the new token), query heads of one work unit with different softmaxes, and quantisation groups whose scale is
 inf beside large finite groups.
 
-The bar is the suite's (tests/test_decode_gpu.py, _checked_step): the production and instrumented epilogues give the same
+The bar is the suite's (tests/_attn.py, checked_step): the production and instrumented epilogues give the same
 bits, every stage is checked against the oracle applied to the kernel's own previous stage, the output end to end, and the
 exported cache against the oracle's 9-tuple bit for bit.  Every regime asserts its precondition: where the oracle output is
 meant to be finite it is, and in ragged batches the oracle's masked probabilities are exactly 0.  The sequences that carry
@@ -22,7 +22,6 @@ Case matrix:
   * every regime on the kernels of the shipped configurations (and K4V4 g64 G1) at about 600 tokens;
   * the precision regimes at 4096 and 32768 tokens on those kernels, and ragged at 4096;
   * one profiler trace in which exactly the 72 expected (qk_kernel, sv_kernel) pairs run."""
-import itertools
 import json
 import re
 
@@ -30,11 +29,9 @@ import numpy as np
 import pytest
 import torch
 
-from tests._util import to_np
-from tests.test_decode_gpu import (BITS, E2E_ATOL_FRAC, E2E_RTOL, GQA_CHUNKS, GROUPS, NEG16, RAGGED_STARTS, RESIDUALS,
-                                   _checked_step, _mirror_lengths, _oracle_prefill, _oracle_step, _stage_checks,
-                                   _start_mask, _tuple_equal)
-from tests.test_decode_numerics_gpu import OUTLIER_CHANNELS, _put_k_edges, _put_v_edges
+from oracle import ref
+from tests._attn import (NEG16, OUTLIER_CHANNELS, RAGGED_STARTS, _put_k_edges, _put_v_edges, checked_step, hidden_mask,
+                         instantiation_cases, make_cache, mirror_lengths)
 
 pytestmark = pytest.mark.gpu
 
@@ -100,7 +97,7 @@ def _bad_seqs(rname, ragged):
 
 
 def _put_edges(x, pos0, bits, put, bad):
-    """The edge rows of test_decode_numerics_gpu (put: _put_k_edges / _put_v_edges), the overflowing ones in `bad` only."""
+    """The edge rows of tests/_attn.py (put: _put_k_edges / _put_v_edges), the overflowing ones in `bad` only."""
     for b in range(x.shape[0]):
         pair = np.repeat(x[b:b + 1], 2, axis=0)
         put(pair, pos0, bits)
@@ -143,7 +140,7 @@ def _make_case(rname, B, H, Hkv, n0, steps, g, kb, vb, R, G, bad):
                 first = (grp == 1) & (pos % g == 0)
                 k[b, :, first, KINF_C] = -60000.0
                 k[b, :, np.roll(first, 1), KINF_C] = 60000.0
-    tk, _, tv, _ = _mirror_lengths(n0, R)
+    tk, _, tv, _ = mirror_lengths(n0, R)
     j_fixed = _peak_token(spec.get("peak", "blk"), tk, tv, n0 + 1, 0)
     if spec.get("vinf"):                          # token groups: channels [0, g) inf scale (bad sequences), [c, c + g) large;
         c = g if 2 * g <= D else 0                # g = 128: one group per token, the inf one on the next token of the block
@@ -189,66 +186,37 @@ def _make_case(rname, B, H, Hkv, n0, steps, g, kb, vb, R, G, bad):
     return k[:, :, :n0], v[:, :, :n0], steps_out
 
 
-def _check_step(cache, st, q, kn, vn, g, kb, vb, R, starts, bad):
-    """One decode step with the regime's preconditions, then the suite's checks.  `bad`: sequences whose oracle output may
-    be non-finite.  Returns the oracle's 9-tuple after the step."""
-    B, H = q.shape[:2]
-    T = st[8] + 1
-    mask = None if starts is None else _start_mask(starts, B, T)
-    exp_out, exp_p, st_next = _oracle_step(st, q, kn, vn, g, kb, vb, R, mask)
-    good = [b for b in range(B) if b not in bad]
+def _check_step(cache, st, q, kn, vn, cfg, starts, bad):
+    """One decode step with the regime's preconditions, then the suite's checks (checked_step).  `bad`: sequences whose
+    oracle output may be non-finite; they are held to the oracle's non-finite positions.  Returns the oracle's 9-tuple
+    after the step."""
+    mask = hidden_mask(q.shape[0], st[8] + 1, starts)
+    exp_out, exp_p, _ = ref.decode_step(st, q, kn, vn, *cfg, mask)
+    good = [b for b in range(q.shape[0]) if b not in bad]
     assert np.isfinite(exp_out[good]).all(), "precondition: the oracle output of the regime is finite"
     if bad:
         assert not np.isfinite(exp_out[sorted(bad)]).all(), "precondition: the inf-scale groups reach the oracle output"
     if mask is not None:
         pm = np.broadcast_to(mask == NEG16, exp_p.shape)[good]
         assert (exp_p[good][pm] == 0).all(), "precondition: the oracle's masked probabilities are exactly 0"
-    if not bad:
-        return _checked_step(cache, st, q, kn, vn, g, kb, vb, R, starts)
-    # sequences with inf-scale groups (test_edge_values_through_cache_quantisers): the finite ones get every check, the
-    # kernel is non-finite exactly where the oracle is, and within the end-to-end bar where it is finite
-    qd, kd, vd = (torch.from_numpy(np.ascontiguousarray(a[:, :, 0])).cuda() for a in (q, kn, vn))
-    dbg_s = torch.zeros((B, H, T + 8), dtype=torch.float16, device="cuda")
-    dbg_p = torch.zeros_like(dbg_s)
-    out_fast = cache.decode_attention(0, qd, kd, vd).clone()
-    out = cache.decode_attention(0, qd, kd, vd, dbg_logits=dbg_s, dbg_probs=dbg_p)
-    cache.advance()
-    torch.cuda.synchronize()
-    assert torch.equal(out_fast.view(torch.int16), out.view(torch.int16)), "production and instrumented epilogues disagree"
-    got = to_np(out)[:, :, None, :]
-    got_s, got_p = to_np(dbg_s)[:, :, None, :T].copy(), to_np(dbg_p)[:, :, None, :T]
-    mfull = None
-    if mask is not None:
-        mfull = np.broadcast_to(mask, (B, H, 1, T))
-        got_s[mfull == NEG16] = NEG16
-    stg = tuple(None if t is None else t[good] for t in st[:8]) + (st[8],)
-    _stage_checks(stg, q[good], kn[good], vn[good], g, kb, vb, R, got[good], got_s[good], got_p[good],
-                  mask=None if mfull is None else mfull[good])
-    fin = np.isfinite(exp_out)
-    np.testing.assert_array_equal(np.isfinite(got), fin, err_msg="non-finite positions differ from the oracle's")
-    x, e = exp_out.astype(np.float64)[fin], got.astype(np.float64)[fin]
-    tol = E2E_RTOL * np.abs(x) + E2E_ATOL_FRAC * np.abs(x).max()
-    assert (np.abs(e - x) <= tol).all(), f"end-to-end: worst err / bar {(np.abs(e - x) / np.maximum(tol, 1e-30)).max():.2f}"
-    _tuple_equal(cache.export(0), st_next)
-    return st_next
+    return checked_step(cache, st, q, kn, vn, cfg, starts=starts, bad=bad)
 
 
 def _run_case(rname, kb, vb, g, G, R, Hkv, ratio, n0, starts, steps=2):
     """Prefill n0 tokens of the regime (r = R - 2: the second step completes the K window and flushes it), then `steps`
     fully checked decode steps."""
-    from kivi_b200.cache import KiviCache
     bad = _bad_seqs(rname, starts is not None)
     B = len(starts) if starts is not None else 2 if bad else 1      # unpadded: sequence 0 finite, sequence 1 with inf scales
     H = ratio * Hkv
     k, v, stepdata = _make_case(rname, B, H, Hkv, n0, steps, g, kb, vb, R, G, bad)
-    cache = KiviCache(1, B, H, Hkv, D, kb, vb, g, R, n0 + steps + 16, gqa_chunk=G)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + steps + 16, gqa_chunk=G)
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda(),
                   kv_start=None if starts is None else torch.tensor(starts))
     assert cache.ragged == (starts is not None)
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
     tk0 = cache.tk
     for q, kn, vn in stepdata:
-        st = _check_step(cache, st, q, kn, vn, g, kb, vb, R, starts, bad)
+        st = _check_step(cache, st, q, kn, vn, (g, kb, vb, R), starts, bad)
     assert cache.tk == tk0 + R, "the steps crossed a K flush"
     assert cache.read_state()[:6] == [cache.tk, cache.r, cache.tv, cache.L, cache.vhead, cache.kv_len]
 
@@ -260,7 +228,7 @@ def _prompt_len(T, R):
 
 def _ragged_starts(n0, R):
     """test_every_instantiation_matches_oracle's starts: whole blocks skipped, partly padded blocks, inside the windows."""
-    tk, r, tv, L = _mirror_lengths(n0, R)
+    tk, r, tv, L = mirror_lengths(n0, R)
     return RAGGED_STARTS + [tk + r // 2, tv + L // 2]
 
 
@@ -271,43 +239,27 @@ SHORT = ["q-2^-20", "k-wide", "k-wide-live", "k-1e-4", "v-1e-4-peak", "v-2000-pe
 SHORT_MIXED = ["mixed-v-2000"]                    # G > 1
 
 
-def _instantiations():
-    """(kb, vb, g, G, ragged, R, ratio) of the 72 kernel pairs, R and ratio varied as in test_every_instantiation."""
-    out = []
-    for (ik, kb), (iv, vb), g, (iG, G), ragged in itertools.product(enumerate(BITS), enumerate(BITS), GROUPS,
-                                                                      enumerate(GQA_CHUNKS), (False, True)):
-        Rs = [R for R in RESIDUALS if R % g == 0]
-        R = Rs[(2 * ik + iv + iG + ragged) % len(Rs)]
-        ratio = 2 * G if (2 * ik + iv + iG + GROUPS.index(g)) % 5 == 0 else G
-        out.append((kb, vb, g, G, ragged, R, ratio))
-    return out
-
-
-def _inst_id(kb, vb, g, G, ragged, R, ratio):
-    return f"k{kb}v{vb}-g{g}-G{G}-R{R}-ratio{ratio}-{'ragged' if ragged else 'unpadded'}"
-
-
 def _matrix_a():
     cases = []
-    for inst in _instantiations():
-        G = inst[3]
+    for inst in instantiation_cases("ragged"):
+        kb, vb, g, G, R, ratio, ragged = inst.values
         for rname in SHORT + (SHORT_MIXED if G > 1 else []):
-            cases.append(pytest.param(*inst, rname, id=f"{_inst_id(*inst)}-{rname}"))
+            cases.append(pytest.param(kb, vb, g, G, ragged, R, ratio, rname, id=f"{inst.id}-{rname}"))
     return cases
 
 
 # Open: in these two cases the p.V stage of one step is off the oracle by 2 fp16 steps in 1-3 outputs (1.02x and 1.33x
 # the stage bar); the outputs are finite and every other check holds.  The test pins exactly that, so that any other
 # failure, or a larger excess, still fails.
-STAGE3_OPEN = {("k2v2-g32-G2-R64-ratio2-unpadded", "mixed-v-2000"), ("k2v2-g64-G4-R256-ratio4-unpadded", "v-3500-peak")}
+STAGE3_OPEN = {"k2v2-g32-G2-R64-ratio2-unpadded-mixed-v-2000", "k2v2-g64-G4-R256-ratio4-unpadded-v-3500-peak"}
 
 
 @pytest.mark.parametrize("kb,vb,g,G,ragged,R,ratio,rname", _matrix_a())
-def test_every_instantiation_across_magnitudes(kb, vb, g, G, ragged, R, ratio, rname):
+def test_every_instantiation_across_magnitudes(kb, vb, g, G, ragged, R, ratio, rname, request):
     Hkv = 2 if ratio == G else 1
     n0 = _prompt_len(600, R)
     run = lambda: _run_case(rname, kb, vb, g, G, R, Hkv, ratio, n0, _ragged_starts(n0, R) if ragged else None)  # noqa: E731
-    if (_inst_id(kb, vb, g, G, ragged, R, ratio), rname) not in STAGE3_OPEN:
+    if request.node.callspec.id not in STAGE3_OPEN:
         run()
         return
     with pytest.raises(AssertionError, match=r"attention output \(own probs\): [1-3] / \d+ elements .* max err [0-9.e+-]+, "
@@ -359,7 +311,7 @@ def test_long_context_precision(kname, rname, T, ragged):
     n0 = _prompt_len(T, R)
     starts = None
     if ragged:                                    # unpadded, whole blocks skipped + a partly padded block, inside the V ring
-        tk, r, tv, L = _mirror_lengths(n0, R)
+        tk, r, tv, L = mirror_lengths(n0, R)
         starts = [0, 1000, tv + L // 2]
     _run_case(rname, kb, vb, g, G, R, Hkv, G, n0, starts)
 
@@ -375,9 +327,9 @@ def test_instantiations_reach_every_kernel_pair(tmp_path):
     """One profiler trace around one decode step of every instantiation: the (qk_kernel, sv_kernel) pairs that ran, in
     order, are exactly the 72 expected ones."""
     from torch.profiler import ProfilerActivity, profile
-    from kivi_b200.cache import KiviCache
     prepared, expected = [], []
-    for kb, vb, g, G, ragged, R, ratio in _instantiations():
+    for inst in instantiation_cases("ragged"):
+        kb, vb, g, G, R, ratio, ragged = inst.values
         Hkv = 2 if ratio == G else 1
         H = ratio * Hkv
         n0 = _prompt_len(300, R)
@@ -386,7 +338,7 @@ def test_instantiations_reach_every_kernel_pair(tmp_path):
         rng = np.random.default_rng(kb + 3 * vb + g + G + R)
         k = torch.from_numpy(rng.standard_normal((B, Hkv, n0, D)).astype(np.float16)).cuda()
         v = torch.from_numpy(rng.standard_normal((B, Hkv, n0, D)).astype(np.float16)).cuda()
-        cache = KiviCache(1, B, H, Hkv, D, kb, vb, g, R, n0 + 8, gqa_chunk=G)
+        cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, gqa_chunk=G)
         cache.prefill(0, k, v, kv_start=None if starts is None else torch.tensor(starts))
         q = torch.from_numpy((rng.standard_normal((B, H, D)) * 0.7).astype(np.float16)).cuda()
         prepared.append((cache, q, k[:, :, -1].contiguous(), v[:, :, -1].contiguous()))

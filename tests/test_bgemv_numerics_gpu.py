@@ -26,8 +26,8 @@ import pytest
 import torch
 
 from oracle import ref
+from tests._attn import OUTLIER_CHANNELS, _edge_rows
 from tests._util import FLOOR_COEF, l1_mass_ref_layout, to_np
-from tests.test_decode_numerics_gpu import _edge_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -269,7 +269,6 @@ QK_KERNELS = {   # name: B, H, Hkv, Tk, g, bits
     "wide-4-2-64": (1, 4, 1, 2048, 64, 4),
     "simt-wide-G1": (1, 2, 2, 2048, 32, 2),
 }
-OUTLIER_CHANNELS = [5, 37, 77, 120]
 QK_REGIMES = {   # name: seed, q std, K std, extras
     "unit": (1, 1.0, 1.0, {}),
     "q-2^-6": (2, 2.0 ** -6, 1.0, {}),

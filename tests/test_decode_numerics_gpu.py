@@ -12,9 +12,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests._util import to_np
-from tests.test_decode_gpu import (E2E_ATOL_FRAC, E2E_RTOL, _checked_step, _oracle_prefill, _oracle_step,
-                                   _stage_checks, _tuple_equal)
+from oracle import ref
+from tests._attn import OUTLIER_CHANNELS, _put_k_edges, _put_v_edges, checked_step, make_cache, rand16, tuple_equal
 
 pytestmark = pytest.mark.gpu
 
@@ -25,7 +24,6 @@ KERNELS = {   # name: k_bits, v_bits, g, R, G, Hkv  (B = 1, H = G * Hkv: the ora
     "k4v2-g128-G2": (4, 2, 128, 128, 2, 2),
 }
 
-OUTLIER_CHANNELS = [5, 37, 77, 120]
 REGIMES = {   # name: seed, q std, K std, V std, extras
     "unit": (1, 1.0, 1.0, 1.0, {}),
     "q-2^-6": (2, 2.0 ** -6, 1.0, 1.0, {}),
@@ -56,9 +54,8 @@ def _sweep_cases():
 
 @pytest.mark.parametrize("kname,rname,T", _sweep_cases())
 def test_magnitude_sweep_matches_oracle(kname, rname, T):
-    """Prefill T - 1 tokens of the regime, then two decode steps, each fully checked (_checked_step: fast == instrumented,
+    """Prefill T - 1 tokens of the regime, then two decode steps, each fully checked (checked_step: fast == instrumented,
     every stage against the oracle at the suite's bars, end to end, the exported cache bit for bit)."""
-    from kivi_b200.cache import KiviCache
     kb, vb, g, R, G, Hkv = KERNELS[kname]
     seed, qs, ks, vs, extra = REGIMES[rname]
     B, H, n0 = 1, G * Hkv, T - 1
@@ -71,9 +68,9 @@ def test_magnitude_sweep_matches_oracle(kname, rname, T):
         return k.astype(np.float16), (rng.standard_normal((B, Hkv, n, 128)) * vs).astype(np.float16)
 
     k, v = kv(n0)
-    cache = KiviCache(1, B, H, Hkv, 128, kb, vb, g, R, T + 16, gqa_chunk=G)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, T + 16, gqa_chunk=G)
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda())
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
     for step in range(2):
         if "peaked" in extra:                        # aligned with a token of the packed K store
             j = (n0 // 3) + step
@@ -81,51 +78,12 @@ def test_magnitude_sweep_matches_oracle(kname, rname, T):
         else:
             q = (rng.standard_normal((B, H, 1, 128)) * qs).astype(np.float16)
         k_new, v_new = kv(1)
-        st = _checked_step(cache, st, q, k_new, v_new, g, kb, vb, R)
+        st = checked_step(cache, st, q, k_new, v_new, (g, kb, vb, R))
 
 
 # ---------------------------------------------------------------------------------------------------
 # edge values through the cache's own quantisers
 # ---------------------------------------------------------------------------------------------------
-def _edge_rows(bits, finite):
-    """The rows of test_pack_edge_values (64 values each: two groups of 32).  finite=False adds the rows whose group range
-    overflows fp16 (large magnitudes, +-60000: the scale becomes inf)."""
-    rng = np.random.default_rng(5)
-    rows = [np.full(64, 1.25),                                                        # constant -> degenerate group
-            np.zeros(64),
-            np.concatenate([np.linspace(0, 3, 32), np.linspace(-7, 8, 32)]),         # ties / grid points
-            rng.standard_normal(64) * 6e-6,                                           # fp16 subnormals
-            np.arange(64) % (2 ** bits) * 0.5]                                        # exact levels
-    if not finite:
-        rows += [rng.standard_normal(64) * 2e4,
-                 np.concatenate([[-60000.0, 60000.0], rng.standard_normal(62)])]
-    return [r.astype(np.float16) for r in rows]
-
-
-def _edge_channels(n_rows):
-    return [3 + 17 * e for e in range(n_rows)]
-
-
-def _put_k_edges(k, pos0, kb):
-    """K channel c_e of token t (absolute position pos0 + t) = row e at t mod 64: whole quantisation groups along tokens.
-    Sequence 0 gets the finite rows, sequence 1 all of them."""
-    for b in range(k.shape[0]):
-        rows = _edge_rows(kb, finite=(b == 0))
-        for c, row in zip(_edge_channels(len(rows)), rows):
-            k[b, :, :, c] = row[(pos0 + np.arange(k.shape[2])) % 64]
-
-
-def _put_v_edges(v, pos0, vb):
-    """Token t with (pos0 + t) % 5 == 2 of every sequence is an edge row over its 128 channels (two rows of 64)."""
-    for b in range(v.shape[0]):
-        rows = _edge_rows(vb, finite=(b == 0))
-        for t in range(v.shape[2]):
-            p = pos0 + t
-            if p % 5 == 2:
-                e = (p // 5) % len(rows)
-                v[b, :, t, :] = np.concatenate([rows[e], rows[(e + 1) % len(rows)]])
-
-
 @pytest.mark.parametrize("kb,vb,g,R,n0", [(2, 2, 32, 32, 3 * 128 + 5), (4, 4, 64, 64, 4 * 64 + 5),
                                           (2, 4, 32, 64, 2 * 128 + 5), (4, 2, 128, 128, 3 * 128 + 5)])
 def test_edge_values_through_cache_quantisers(kb, vb, g, R, n0):
@@ -134,51 +92,28 @@ def test_edge_values_through_cache_quantisers(kb, vb, g, R, n0):
     after every step.  A sequence whose oracle output is finite (finite edge rows only) gets every check of the suite; where
     the oracle's output is not finite (the rows whose scale overflows), the kernel's must be non-finite at exactly the same
     positions, and equal within the end-to-end bar where it is finite."""
-    from kivi_b200.cache import KiviCache
     B, H, Hkv = 2, 4, 2
+    cfg = (g, kb, vb, R)
     rng = np.random.default_rng(kb * 31 + vb * 7 + g + R)
-    k = rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)
-    v = rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)
+    k, v = rand16(rng, (B, Hkv, n0, 128)), rand16(rng, (B, Hkv, n0, 128))
     _put_k_edges(k, 0, kb)
     _put_v_edges(v, 0, vb)
     steps = 2 * R - 4 if R <= 64 else R - 4                          # r = 5 -> flushes at r = R - 1
-    cache = KiviCache(1, B, H, Hkv, 128, kb, vb, g, R, n0 + steps + 8)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + steps + 8)
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda())
-    st = _oracle_prefill(k, v, g, kb, vb, R)
-    _tuple_equal(cache.export(0), st)
+    st = ref.prefill_cache(k, v, *cfg)
+    tuple_equal(cache.export(0), st, "prefill")
     flushes = 0
     for step in range(steps):
         pos = cache.kv_len
-        q = (rng.standard_normal((B, H, 1, 128)) * 0.7).astype(np.float16)
-        k_new = rng.standard_normal((B, Hkv, 1, 128)).astype(np.float16)
-        v_new = rng.standard_normal((B, Hkv, 1, 128)).astype(np.float16)
+        q, k_new, v_new = rand16(rng, (B, H, 1, 128), 0.7), rand16(rng, (B, Hkv, 1, 128)), rand16(rng, (B, Hkv, 1, 128))
         _put_k_edges(k_new, pos, kb)
         _put_v_edges(v_new, pos, vb)
         tk0 = cache.tk
-        # sequence 0 (finite) through every check of the suite, on its own slice of the oracle state
-        T = pos + 1
-        qd, kd, vd = (torch.from_numpy(np.ascontiguousarray(a[:, :, 0])).cuda() for a in (q, k_new, v_new))
-        dbg_s = torch.zeros((B, H, T + 8), dtype=torch.float16, device="cuda")
-        dbg_p = torch.zeros_like(dbg_s)
-        out_fast = cache.decode_attention(0, qd, kd, vd).clone()
-        out = cache.decode_attention(0, qd, kd, vd, dbg_logits=dbg_s, dbg_probs=dbg_p)
-        cache.advance()
-        torch.cuda.synchronize()
-        assert torch.equal(out_fast.view(torch.int16), out.view(torch.int16)), f"step {step}: fast / instrumented"
-        got = to_np(out)[:, :, None, :]
-        exp_out, _, st_next = _oracle_step(st, q, k_new, v_new, g, kb, vb, R)
-        fin = np.isfinite(exp_out)
+        fin = np.isfinite(ref.decode_step(st, q, k_new, v_new, *cfg)[0])
         assert fin[0].all(), "the finite edge rows must give a finite oracle output"
         assert (~fin[1]).any(), "the overflowing edge rows must reach the output"
-        np.testing.assert_array_equal(np.isfinite(got), fin, err_msg=f"step {step}: non-finite positions differ")
-        sl = slice(0, 1)
-        st0 = tuple(None if t is None else t[sl] for t in st[:8]) + (st[8],)
-        _stage_checks(st0, q[sl], k_new[sl], v_new[sl], g, kb, vb, R, got[sl], to_np(dbg_s)[sl, :, None, :T],
-                      to_np(dbg_p)[sl, :, None, :T])
-        x, e = exp_out.astype(np.float64), got.astype(np.float64)
-        tol = E2E_RTOL * np.abs(x[fin]) + E2E_ATOL_FRAC * np.abs(x[fin]).max()
-        assert (np.abs(e[fin] - x[fin]) <= tol).all(), f"step {step}: end-to-end"
-        st = st_next
-        _tuple_equal(cache.export(0), st)
+        # sequence 0 (finite) through every check of the suite; sequence 1 held to the oracle's non-finite positions
+        st = checked_step(cache, st, q, k_new, v_new, cfg, bad=(1,))
         flushes += cache.tk != tk0
     assert flushes == (2 if R <= 64 else 1)

@@ -4,33 +4,9 @@ import numpy as np
 import pytest
 import torch
 
+from tests._attn import hidden_mask, left_padded, make_cache, tiny_model, tuple_equal
+
 pytestmark = pytest.mark.gpu
-
-NEG = float(torch.finfo(torch.float16).min)
-
-
-def _mk_cache(B, H, Hkv, kb, vb, g, R, max_tokens):
-    from kivi_b200.cache import KiviCache
-    return KiviCache(1, B, H, Hkv, 128, kb, vb, g, R, max_tokens)
-
-
-def _tuple_bits_equal(a, b, what):
-    assert a[8] == b[8], what
-    for i in range(8):
-        if a[i] is None or b[i] is None:
-            assert a[i] is None and b[i] is None, (what, i)
-            continue
-        x, y = a[i], b[i]
-        if x.dtype == torch.float16:
-            x, y = x.view(torch.int16), y.view(torch.int16)
-        assert torch.equal(x, y), f"{what}: tuple[{i}]"
-
-
-def _mask_of(starts, B, T, dev):
-    m = torch.zeros((B, T), dtype=torch.float16, device=dev)
-    for b, s in enumerate(starts):
-        m[b, :min(max(s, 0), T - 1)] = NEG
-    return m
 
 
 RAGGED_CASES = [  # kb, vb, g, R, H, Hkv  (G = 4 / 2 / 1 from H / Hkv)
@@ -56,7 +32,7 @@ def test_ragged_matches_mask_path(kb, vb, g, R, H, Hkv):
     n0 = max(3, -(-400 // R)) * R + R - 3                            # r = R - 3: the K window flushes at step 3
     steps = 6
     B = 10
-    ragged, masked = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 64), _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 64)
+    ragged, masked = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 64), make_cache(B, H, Hkv, kb, vb, g, R, n0 + 64)
     k = torch.from_numpy(rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)).to(dev)
     v = torch.from_numpy(rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)).to(dev)
     ragged.prefill(0, k, v)
@@ -77,7 +53,8 @@ def test_ragged_matches_mask_path(kb, vb, g, R, H, Hkv):
         # production epilogues first (no debug pointers: unpadded blocks take the fast epilogue), then instrumented
         out_fast = ragged.decode_attention(0, q, kn, vn).clone()
         out_r = ragged.decode_attention(0, q, kn, vn, dbg_logits=dl_r, dbg_probs=dp_r)
-        out_m = masked.decode_attention(0, q, kn, vn, mask=_mask_of(starts, B, T, dev), dbg_logits=dl_m, dbg_probs=dp_m)
+        mask = torch.from_numpy(hidden_mask(B, T, starts)).to(dev)
+        out_m = masked.decode_attention(0, q, kn, vn, mask=mask, dbg_logits=dl_m, dbg_probs=dp_m)
         torch.cuda.synchronize()
         assert torch.equal(out_fast.view(torch.int16), out_r.view(torch.int16)), f"step {step}: fast / instrumented"
         assert torch.equal(out_r.view(torch.int16), out_m.view(torch.int16)), f"step {step}: out"
@@ -87,7 +64,7 @@ def test_ragged_matches_mask_path(kb, vb, g, R, H, Hkv):
             assert torch.equal(dl_r[b, :, s:T].view(torch.int16), dl_m[b, :, s:T].view(torch.int16)), f"step {step}: logits {b}"
         ragged.advance()
         masked.advance()
-        _tuple_bits_equal(ragged.export(0), masked.export(0), f"step {step}")
+        tuple_equal(ragged.export(0), masked.export(0), f"step {step}")
     assert ragged.read_state() == masked.read_state()
 
 
@@ -98,7 +75,7 @@ def test_padded_blocks_are_not_read():
     rng = np.random.default_rng(7)
     B, H, Hkv, kb, vb, g, R, n0 = 4, 4, 2, 2, 2, 32, 128, 700
     starts = [0, 300, 129, 512]
-    clean = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
+    clean = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
     k = torch.from_numpy(rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)).to(dev)
     v = torch.from_numpy(rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)).to(dev)
     clean.prefill(0, k, v, kv_start=torch.tensor(starts))
@@ -110,7 +87,7 @@ def test_padded_blocks_are_not_read():
         tup[2][b, :, :, :nb * 128 // g] = float("nan")               # K scales [B, Hkv, 128, tk / g]
         tup[6][b, :, :nb * 128, :] = float("nan")                    # V scales [B, Hkv, tv, 128 / g]
     assert poisoned_blocks > 0
-    bad = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
+    bad = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
     bad.import_tuple(0, tuple(tup), kv_start=torch.tensor(starts))
     q = torch.from_numpy((rng.standard_normal((B, H, 128)) * 0.7).astype(np.float16)).to(dev)
     kn = torch.from_numpy(rng.standard_normal((B, Hkv, 128)).astype(np.float16)).to(dev)
@@ -121,7 +98,7 @@ def test_padded_blocks_are_not_read():
     assert not torch.isnan(out_clean).any()
     assert torch.equal(out_clean.view(torch.int16), out_bad.view(torch.int16))
     bad.set_kv_start(None)                                           # the same cache through the additive-mask path
-    out_mask = bad.decode_attention(0, q, kn, vn, mask=_mask_of(starts, B, bad.kv_len + 1, dev))
+    out_mask = bad.decode_attention(0, q, kn, vn, mask=torch.from_numpy(hidden_mask(B, bad.kv_len + 1, starts)).to(dev))
     torch.cuda.synchronize()
     for b in range(1, B):                                            # every sequence with a wholly padded block
         assert torch.isnan(out_mask[b]).any(), f"poison did not reach the mask path (sequence {b})"
@@ -132,7 +109,7 @@ def test_start_at_or_beyond_kv_len_sees_only_the_new_token(kb, vb, g, R, H, Hkv)
     dev = torch.device("cuda")
     rng = np.random.default_rng(11)
     B, n0 = 3, 333
-    cache = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
     k = torch.from_numpy(rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)).to(dev)
     v = torch.from_numpy(rng.standard_normal((B, Hkv, n0, 128)).astype(np.float16)).to(dev)
     cache.prefill(0, k, v, kv_start=torch.tensor([n0, n0 + 1, 1 << 30]))
@@ -148,29 +125,12 @@ def test_start_at_or_beyond_kv_len_sees_only_the_new_token(kb, vb, g, R, H, Hkv)
         cache.set_kv_start(torch.full((B,), cache.kv_len, dtype=torch.int32))
 
 
-def _tiny(seed=0, **kw):
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI, default_config
-    cfg = default_config("tiny", **kw)
-    torch.manual_seed(seed)
-    return LlamaForCausalLM_KIVI(cfg).half().cuda().eval(), cfg
-
-
-def _left_padded(cfg, lengths, n, seed=0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    ids = torch.randint(0, cfg.vocab_size, (len(lengths), n), device="cuda", generator=g)
-    mask = torch.zeros((len(lengths), n), dtype=torch.long, device="cuda")
-    for b, ln in enumerate(lengths):
-        mask[b, n - ln:] = 1
-        ids[b, :n - ln] = 0                                          # pad token
-    return ids, mask
-
-
 def test_padded_decode_step_graph_matches_eager():
-    model, cfg = _tiny(5, num_attention_heads=4, num_key_value_heads=2, hidden_size=512)
-    twin, _ = _tiny(5, num_attention_heads=4, num_key_value_heads=2, hidden_size=512)
+    model, cfg = tiny_model(5, num_attention_heads=4, num_key_value_heads=2, hidden_size=512)
+    twin, _ = tiny_model(5, num_attention_heads=4, num_key_value_heads=2, hidden_size=512)
     twin.load_state_dict(model.state_dict())
     n = 200
-    ids, mask = _left_padded(cfg, [200, 130, 40], n, seed=1)
+    ids, mask = left_padded(cfg, [200, 130, 40], n, seed=1, low=0)
     for m in (model, twin):
         m.init_cache(3, n + 16)
     lg = model.prefill(ids, attention_mask=mask)
@@ -189,12 +149,12 @@ def test_padded_decode_step_graph_matches_eager():
 def test_padded_model_matches_tuple_model(name, kw):
     """B = 3 left-padded prompts (one shorter than R: its padding reaches the fp16 windows), 40 steps across a K flush:
     the fused padded decode against the tuple path with the 2-D padding mask, both fed the same tokens."""
-    model, cfg = _tiny(0, **kw)
+    model, cfg = tiny_model(0, **kw)
     model.fused_forward = False                       # forward() = the reference's own 9-tuple path
     R = cfg.residual_length
     n, steps = 2 * R + R - 28 if R < 128 else R + 100, 40
     lengths = [n, n - 60, R // 2 - 5]
-    ids, mask = _left_padded(cfg, lengths, n, seed=3)
+    ids, mask = left_padded(cfg, lengths, n, seed=3, low=0)
     B = len(lengths)
     pos = mask.long().cumsum(-1) - 1
     pos.masked_fill_(mask == 0, 1)
@@ -228,13 +188,13 @@ def test_padded_model_matches_tuple_model(name, kw):
 
 
 def test_generate_with_masks():
-    model, cfg = _tiny(1)
+    model, cfg = tiny_model(1)
     ids = torch.randint(0, cfg.vocab_size, (3, 140), device="cuda")
     plain = model.generate(ids, max_new_tokens=12)
     ones = model.generate(ids, max_new_tokens=12, attention_mask=torch.ones_like(ids))
     assert torch.equal(plain, ones)
     assert not model.cache.ragged
-    pids, mask = _left_padded(cfg, [140, 90, 20], 140, seed=2)
+    pids, mask = left_padded(cfg, [140, 90, 20], 140, seed=2, low=0)
     out = model.generate(pids, max_new_tokens=12, attention_mask=mask)
     assert out.shape == (3, 152) and torch.equal(out[:, :140], pids) and model.cache.ragged
     again = model.generate(ids, max_new_tokens=12)                  # the unpadded step graph again

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests._attn import tiny_model
 from tests.test_sample_cpu import greedy_id, reference_pick, reference_row, uniform24
 
 pytestmark = pytest.mark.gpu
@@ -267,13 +268,6 @@ def test_argument_errors_launch_nothing():
 
 
 # ------------------------------------------------------------------------------------------------------------ model level
-def _tiny(seed=0, **kw):
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI, default_config
-    cfg = default_config("tiny", **kw)
-    torch.manual_seed(seed)
-    return LlamaForCausalLM_KIVI(cfg).half().cuda().eval(), cfg
-
-
 def _prompt(cfg, B, n, seed=0):
     g = torch.Generator(device="cuda").manual_seed(seed)
     return torch.randint(1, cfg.vocab_size, (B, n), device="cuda", generator=g)
@@ -283,7 +277,7 @@ SAMPLED = dict(do_sample=True, temperature=1.3, top_k=40, top_p=0.95)
 
 
 def test_generate_samples_reproducibly():
-    model, cfg = _tiny(1)
+    model, cfg = tiny_model(1)
     ids = _prompt(cfg, 4, 37)
     a = model.generate(ids, max_new_tokens=24, seed=7, **SAMPLED)
     b = model.generate(ids, max_new_tokens=24, seed=7, **SAMPLED)
@@ -307,8 +301,8 @@ def test_in_graph_sampler_is_the_stand_alone_call():
     on the logits decode_step returned, with the same seeds and draw numbers."""
     from kivi_b200 import glue
     from kivi_b200.llama_kivi import sampling_rows
-    model, cfg = _tiny(2)
-    twin, _ = _tiny(2)
+    model, cfg = tiny_model(2)
+    twin, _ = tiny_model(2)
     B, n, new = 3, 29, 20
     ids = _prompt(cfg, B, n, seed=3)
     got = model.generate(ids, max_new_tokens=new, seed=11, **SAMPLED)
@@ -340,8 +334,8 @@ def test_mode_flip_keeps_launch_count_and_greedy_bits(monkeypatch):
     launch count is the same in both modes, and greedy decoding after sampling is bit for bit a fresh model's."""
     monkeypatch.setattr(_CountingGraph, "made", 0)
     monkeypatch.setattr(torch.cuda, "CUDAGraph", _CountingGraph)
-    model, cfg = _tiny(3)
-    fresh, _ = _tiny(3)
+    model, cfg = tiny_model(3)
+    fresh, _ = tiny_model(3)
     ids = _prompt(cfg, 2, 33, seed=5)
     g0 = model.generate(ids, max_new_tokens=12)
     greedy_launches = model.launches_per_step
@@ -374,7 +368,7 @@ def test_mode_flip_keeps_launch_count_and_greedy_bits(monkeypatch):
 
 
 def test_p2p_exchange_with_sampling_is_rejected():
-    model, cfg = _tiny(3)
+    model, cfg = tiny_model(3)
     model.init_cache(2, 64)
     model._exchange = object()                                            # what enable_token_allgather(2, mode="p2p") sets
     with pytest.raises(NotImplementedError, match="greedy only"):
@@ -399,7 +393,7 @@ def _requests(cfg, params):
 
 def test_serve_mixes_greedy_and_sampled_requests():
     from kivi_b200.serve import serve
-    model, cfg = _tiny(2)
+    model, cfg = tiny_model(2)
     par = lambda s: dict(temperature=1.2, top_k=30, top_p=0.9, seed=s)     # noqa: E731
     mixed = [None, par(1), None, par(2), par(3), None, par(4), None]
     all_greedy = dict(serve(model, _requests(cfg, [None] * 8), 3, 260))

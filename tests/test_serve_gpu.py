@@ -6,12 +6,12 @@ import pytest
 import torch
 
 from oracle import ref
+from tests._attn import assert_e2e, hidden_mask, left_padded, make_cache, rand16, tiny_model, tuple_equal
+from tests._util import to_np
 
 pytestmark = pytest.mark.gpu
 
 IDLE = 1 << 30
-NEG16 = np.finfo(np.float16).min
-E2E_RTOL, E2E_ATOL_FRAC = 2e-2, 5e-3       # the end-to-end bars of the decode suite
 
 CASES = [  # kb, vb, g, R, H, Hkv  (G = 4 / 2 / 1 from H / Hkv): the geometries of the left-padded decode tests
     (2, 2, 32, 32, 4, 1),
@@ -26,38 +26,13 @@ CASES = [  # kb, vb, g, R, H, Hkv  (G = 4 / 2 / 1 from H / Hkv): the geometries 
 ]
 
 
-def _cache(B, H, Hkv, kb, vb, g, R, max_tokens):
-    from kivi_b200.cache import KiviCache
-    return KiviCache(1, B, H, Hkv, 128, kb, vb, g, R, max_tokens)
-
-
 def _h(rng, *shape, scale=1.0):
-    return torch.from_numpy((rng.standard_normal(shape) * scale).astype(np.float16)).cuda()
-
-
-def _np(t):
-    return None if t is None else t.detach().cpu().numpy()
+    return torch.from_numpy(rand16(rng, shape, scale)).cuda()
 
 
 def _row(tup, b):
     """Sequence b's part of an exported 9-tuple (batch dim kept)."""
     return tuple(t[b:b + 1] if torch.is_tensor(t) else t for t in tup)
-
-
-def _bits_equal(got, exp, what):
-    """got: a torch 9-tuple; exp: a torch or numpy 9-tuple; bit for bit."""
-    assert got[8] == exp[8], what
-    for i in range(8):
-        a, b = got[i], exp[i]
-        b = _np(b) if torch.is_tensor(b) else b
-        if b is None or b.size == 0:
-            assert a is None or a.numel() == 0, f"{what}: tuple[{i}] should be empty"
-            continue
-        a = _np(a)
-        assert a.shape == b.shape, (what, i, a.shape, b.shape)
-        if a.dtype == np.float16:
-            a, b = a.view(np.uint16), b.view(np.uint16)
-        np.testing.assert_array_equal(a, b, err_msg=f"{what}: tuple[{i}]")
 
 
 def _live(kb, vb, g, R, H, Hkv, seed, B=4, steps=None):
@@ -66,7 +41,7 @@ def _live(kb, vb, g, R, H, Hkv, seed, B=4, steps=None):
     rng = np.random.default_rng(seed)
     n0 = max(3, -(-400 // R)) * R + R - 3
     cap = n0 + R + 64
-    cache = _cache(B, H, Hkv, kb, vb, g, R, cap)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, cap)
     k, v = _h(rng, B, Hkv, n0, 128), _h(rng, B, Hkv, n0, 128)
     cache.prefill(0, k, v)
     steps = R + 2 if steps is None else steps
@@ -84,10 +59,6 @@ def _padded(src, s):
     return src[:, idx]
 
 
-def _oracle_prefill(x_k, x_v, g, kb, vb, R):
-    return ref.prefill_cache(x_k[None], x_v[None], g, kb, vb, R)
-
-
 @pytest.mark.parametrize("kb,vb,g,R,H,Hkv", CASES)
 def test_refill_is_exact(kb, vb, g, R, H, Hkv):
     """Slot 2 of a live cache refilled with n tokens exports exactly what a B = 1 prefill of the pad-filled T-token
@@ -100,13 +71,13 @@ def test_refill_is_exact(kb, vb, g, R, H, Hkv):
         k, v = _h(rng, Hkv, n, 128), _h(rng, Hkv, n, 128)
         cache.refill(0, 2, k, v)
         got = cache.export(0)
-        x_k, x_v = _padded(_np(k), T - n), _padded(_np(v), T - n)
-        one = _cache(1, H, Hkv, kb, vb, g, R, T + 8)
-        one.prefill(0, torch.from_numpy(x_k[None]).cuda(), torch.from_numpy(x_v[None]).cuda())
-        _bits_equal(_row(got, 2), one.export(0), f"n {n}: slot 2 vs a B = 1 prefill")
-        _bits_equal(_row(got, 2), _oracle_prefill(x_k, x_v, g, kb, vb, R), f"n {n}: slot 2 vs the oracle")
+        x_k, x_v = _padded(to_np(k), T - n)[None], _padded(to_np(v), T - n)[None]
+        one = make_cache(1, H, Hkv, kb, vb, g, R, T + 8)
+        one.prefill(0, torch.from_numpy(x_k).cuda(), torch.from_numpy(x_v).cuda())
+        tuple_equal(_row(got, 2), one.export(0), f"n {n}: slot 2 vs a B = 1 prefill")
+        tuple_equal(_row(got, 2), ref.prefill_cache(x_k, x_v, g, kb, vb, R), f"n {n}: slot 2 vs the oracle")
         for b in (0, 1, 3):
-            _bits_equal(_row(got, b), _row(before, b), f"n {n}: slot {b}")
+            tuple_equal(_row(got, b), _row(before, b), f"n {n}: slot {b}")
         assert cache.read_state() == state
 
 
@@ -126,7 +97,7 @@ def test_decode_after_refill(kb, vb, g, R, H, Hkv):
     for c in (cache, twin):
         c.set_kv_start(torch.tensor([0, 0, s, 0]))
         c.release(1)
-    st = _oracle_prefill(_padded(_np(k), s), _padded(_np(v), s), g, kb, vb, R)
+    st = ref.prefill_cache(_padded(to_np(k), s)[None], _padded(to_np(v), s)[None], g, kb, vb, R)
     for step in range(6):
         q = _h(rng, 4, H, 128, scale=0.7)
         kn, vn = _h(rng, 4, Hkv, 128), _h(rng, 4, Hkv, 128)
@@ -138,15 +109,11 @@ def test_decode_after_refill(kb, vb, g, R, H, Hkv):
             assert torch.equal(out[b].view(torch.int16), out_t[b].view(torch.int16)), f"step {step}: slot {b}"
         idle = vn[1].repeat_interleave(H // Hkv, dim=0)
         assert torch.equal(out[1].view(torch.int16), idle.view(torch.int16)), f"step {step}: released slot"
-        mask = np.zeros((1, 1, 1, st[8] + 1), np.float16)
-        mask[..., :s] = NEG16
-        exp, _, st = ref.decode_step(st, _np(q[2:3])[:, :, None], _np(kn[2:3])[:, :, None], _np(vn[2:3])[:, :, None],
-                                     g, kb, vb, R, mask)
-        e, x = _np(out[2:3]).astype(np.float64)[:, :, None], exp.astype(np.float64)
-        tol = E2E_RTOL * np.abs(x) + E2E_ATOL_FRAC * np.abs(x).max()
-        assert (np.abs(e - x) <= tol).all(), f"step {step}: worst err / bar {(np.abs(e - x) / tol).max():.2f}"
+        exp, _, st = ref.decode_step(st, to_np(q[2:3])[:, :, None], to_np(kn[2:3])[:, :, None], to_np(vn[2:3])[:, :, None],
+                                     g, kb, vb, R, hidden_mask(1, st[8] + 1, [s]))
+        assert_e2e(to_np(out[2:3])[:, :, None], exp, f"step {step}")
     assert cache.tk > T - T % R, "the steps crossed a K flush"
-    _bits_equal(_row(cache.export(0), 2), st, "slot 2 after the steps")
+    tuple_equal(_row(cache.export(0), 2), st, "slot 2 after the steps")
     assert cache.read_state() == twin.read_state()
 
 
@@ -174,11 +141,11 @@ def test_shift(kb, vb, g, R, H, Hkv, blocks):
     kf, vf = 32 // kb, 32 // vb
     exp = (before[0][..., shift // kf:], before[1], before[2][..., shift // g:], before[3][..., shift // g:],
            before[4][:, :, shift:], before[5], before[6][:, :, shift:], before[7][:, :, shift:], before[8] - shift)
-    _bits_equal(after, exp, "shifted export")
+    tuple_equal(after, exp, "shifted export")
     assert cache.read_state()[:6] == [st0[0] - shift, st0[1], st0[2] - shift, st0[3], st0[4], st0[5] - shift]
     new_starts = [s - shift for s in starts]
     assert cache.kv_start.tolist() == new_starts and cache.kv_start_host == new_starts
-    fresh = _cache(4, H, Hkv, kb, vb, g, R, cache.max_tokens)
+    fresh = make_cache(4, H, Hkv, kb, vb, g, R, cache.max_tokens)
     fresh.import_tuple(0, after, kv_start=torch.tensor(new_starts))
     for step in range(6):
         q = _h(rng, 4, H, 128, scale=0.7)
@@ -188,28 +155,11 @@ def test_shift(kb, vb, g, R, H, Hkv, blocks):
         cache.advance()
         fresh.advance()
         assert torch.equal(a.view(torch.int16), b.view(torch.int16)), f"step {step}"
-    _bits_equal(cache.export(0), fresh.export(0), "after the steps")
+    tuple_equal(cache.export(0), fresh.export(0), "after the steps")
 
 
 # ------------------------------------------------------------------------------------------------------------ model level
-def _tiny(seed=0, **kw):
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI, default_config
-    cfg = default_config("tiny", **kw)
-    torch.manual_seed(seed)
-    return LlamaForCausalLM_KIVI(cfg).half().cuda().eval(), cfg
-
-
 GQA = dict(num_attention_heads=4, num_key_value_heads=1, hidden_size=512)
-
-
-def _left_padded(cfg, lengths, n, seed=0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    ids = torch.randint(1, cfg.vocab_size, (len(lengths), n), device="cuda", generator=g)
-    mask = torch.zeros((len(lengths), n), dtype=torch.long, device="cuda")
-    for b, ln in enumerate(lengths):
-        mask[b, n - ln:] = 1
-        ids[b, :n - ln] = 0
-    return ids, mask
 
 
 class _CountingGraph(torch.cuda.CUDAGraph):
@@ -225,11 +175,11 @@ def test_graph_replays_after_refill_and_shift(monkeypatch):
     to the same model decoding without a graph."""
     monkeypatch.setattr(_CountingGraph, "made", 0)
     monkeypatch.setattr(torch.cuda, "CUDAGraph", _CountingGraph)
-    model, cfg = _tiny(5, **GQA)
-    twin, _ = _tiny(5, **GQA)
+    model, cfg = tiny_model(5, **GQA)
+    twin, _ = tiny_model(5, **GQA)
     twin.load_state_dict(model.state_dict())
     n = 300
-    ids, mask = _left_padded(cfg, [300, 170, 150], n, seed=1)
+    ids, mask = left_padded(cfg, [300, 170, 150], n, seed=1)
     for m in (model, twin):
         m.init_cache(3, 600)
         m.prefill(ids, attention_mask=mask)
@@ -269,7 +219,7 @@ def test_serve(kw, monkeypatch):
     from kivi_b200.serve import serve
     monkeypatch.setattr(_CountingGraph, "made", 0)
     monkeypatch.setattr(torch.cuda, "CUDAGraph", _CountingGraph)
-    model, cfg = _tiny(2, **kw)
+    model, cfg = tiny_model(2, **kw)
     reqs = _requests(cfg)
     stats = {}
     got = dict(serve(model, reqs, 3, 360, stats=stats))
@@ -294,10 +244,10 @@ def test_serve(kw, monkeypatch):
 def test_inserted_request_matches_tuple_path():
     """An inserted sequence continued two ways from the same cache contents: the fused batch (its slot) and the
     reference's tuple path on that slot's exported 9-tuples with its padding mask, fed the same tokens."""
-    model, cfg = _tiny(3, **GQA)
+    model, cfg = tiny_model(3, **GQA)
     R = cfg.residual_length
     n = 2 * R + 100                                     # r = 105 after the prompt and 5 steps: the 40 steps flush K
-    ids, mask = _left_padded(cfg, [n, n - 50, 90], n, seed=4)
+    ids, mask = left_padded(cfg, [n, n - 50, 90], n, seed=4)
     model.init_cache(3, n + 80)
     model.prefill(ids, attention_mask=mask)
     for _ in range(5):
@@ -332,7 +282,7 @@ def test_inserted_request_matches_tuple_path():
 def test_inserted_prompt_does_not_reach_other_requests():
     """Replacing an inserted request's prompt (same length and budget) changes no token of any other request."""
     from kivi_b200.serve import serve
-    model, cfg = _tiny(4)
+    model, cfg = tiny_model(4)
     reqs = _requests(cfg, seed=1)
     a = dict(serve(model, reqs, 3, 360))
     g = torch.Generator().manual_seed(99)

@@ -6,11 +6,9 @@ import pytest
 import torch
 
 from oracle import ref
+from tests._attn import NEG16, assert_e2e, checked_call, hidden_mask, make_cache, rand16, tuple_equal
 
 pytestmark = pytest.mark.gpu
-
-NEG16 = np.finfo(np.float16).min
-E2E_RTOL, E2E_ATOL_FRAC = 2e-2, 5e-3       # the end-to-end bar of the decode-attention oracle suite
 
 CASES = [  # kb, vb, g, R, H, Hkv  (G = 4 / 2 / 1 from H / Hkv; the 4-bit K G = 4 kernels run 12 warps per CTA)
     (2, 2, 32, 128, 4, 1),
@@ -24,64 +22,22 @@ CASES = [  # kb, vb, g, R, H, Hkv  (G = 4 / 2 / 1 from H / Hkv; the 4-bit K G = 
 ]
 
 
-def _mk_cache(B, H, Hkv, kb, vb, g, R, max_tokens, window=None):
-    from kivi_b200.cache import KiviCache
-    return KiviCache(1, B, H, Hkv, 128, kb, vb, g, R, max_tokens, sliding_window=window)
-
-
-def _visible(starts, B, T, W):
-    return [max(min(max(int(starts[b]) if starts is not None else 0, 0), T - 1), T - W) for b in range(B)]
-
-
-def _mask(first, B, T):
-    m = np.zeros((B, 1, 1, T), np.float16)
-    for b, s in enumerate(first):
-        m[b, ..., :s] = NEG16
-    return m
-
-
-def _bits_equal(a, b, what):
-    assert torch.equal(a.view(torch.int16), b.view(torch.int16)), what
-
-
-def _exports_equal(x, y, what):
-    a, b = x.export(0), y.export(0)
-    assert a[8] == b[8], what
-    for i in range(8):
-        if a[i] is None or b[i] is None:
-            assert a[i] is None and b[i] is None, (what, i)
-            continue
-        u, v = a[i], b[i]
-        if u.dtype == torch.float16:
-            u, v = u.view(torch.int16), v.view(torch.int16)
-        assert torch.equal(u, v), f"{what}: tuple[{i}]"
-
-
-def _e2e(got, exp, what):
-    e, x = got.astype(np.float64), exp.astype(np.float64)
-    err = np.abs(e - x)
-    tol = E2E_RTOL * np.abs(x) + E2E_ATOL_FRAC * np.abs(x).max()
-    assert (err <= tol).all(), f"{what}: worst err / bar {(err / np.maximum(tol, 1e-30)).max():.2f}"
-
-
-def _rand(rng, shape, scale=1.0):
-    return (rng.standard_normal(shape) * scale).astype(np.float16)
-
-
 @pytest.mark.parametrize("padded", [False, True])
 @pytest.mark.parametrize("kb,vb,g,R,H,Hkv", CASES)
 def test_window_matches_oracle(kb, vb, g, R, H, Hkv, padded):
     """Several windows per step (1, below R, inside a packed block, on a block edge, two blocks, beyond T), with and without
-    kv_start, over steps that cross a K flush and a V-ring wrap: the output against the oracle with the equivalent mask,
-    dbg_probs 0 below the window (the partly visible block writes zeros there, blocks that are not read leave the zeroed
-    buffer as it is), and the cache after every step bit-identical to a twin driven by the unpadded entry."""
+    kv_start, over steps that cross a K flush and a V-ring wrap: every window by the suite's check against the oracle with
+    the equivalent mask (dbg_probs 0 below the window: the partly visible block writes zeros there, blocks that are not
+    read leave the zeroed buffer as it is), and the cache after every step bit-identical to a twin driven by the unpadded
+    entry."""
     dev = torch.device("cuda")
     rng = np.random.default_rng(kb * 1000 + vb * 100 + g + R + H + int(padded))
     B = 4
     n0 = max(3, -(-600 // R)) * R + R - 3                            # r = R - 3: the K window flushes at step 3
     steps = 6
-    cache, twin = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 16, window=1), _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 16)
-    k, v = _rand(rng, (B, Hkv, n0, 128)), _rand(rng, (B, Hkv, n0, 128))
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 16, sliding_window=1)
+    twin = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 16)
+    k, v = rand16(rng, (B, Hkv, n0, 128)), rand16(rng, (B, Hkv, n0, 128))
     starts = [0, 130, 257, n0 - 50] if padded else None
     cache.prefill(0, torch.from_numpy(k).to(dev), torch.from_numpy(v).to(dev),
                   kv_start=None if starts is None else torch.tensor(starts))
@@ -89,26 +45,18 @@ def test_window_matches_oracle(kb, vb, g, R, H, Hkv, padded):
     st = ref.prefill_cache(k, v, g, kb, vb, R)
     for step in range(steps):
         T = cache.kv_len + 1
-        q, kn, vn = _rand(rng, (B, H, 1, 128), 0.7), _rand(rng, (B, Hkv, 1, 128)), _rand(rng, (B, Hkv, 1, 128))
+        q, kn, vn = rand16(rng, (B, H, 1, 128), 0.7), rand16(rng, (B, Hkv, 1, 128)), rand16(rng, (B, Hkv, 1, 128))
         qd, kd, vd = (torch.from_numpy(np.ascontiguousarray(a[:, :, 0])).to(dev) for a in (q, kn, vn))
         for W in (1, R // 2, 200, 256, 384, T + 5):
-            cache.sliding_window = W
-            dbg_p = torch.zeros((B, H, T + 8), dtype=torch.float16, device=dev)
-            dbg_s = torch.zeros_like(dbg_p)
-            out_fast = cache.decode_attention(0, qd, kd, vd).clone()
-            out = cache.decode_attention(0, qd, kd, vd, dbg_logits=dbg_s, dbg_probs=dbg_p)
-            torch.cuda.synchronize()
-            _bits_equal(out_fast, out, f"step {step} W {W}: production and instrumented epilogues")
-            first = _visible(starts, B, T, W)
-            exp_out, _, _ = ref.decode_step(st, q, kn, vn, g, kb, vb, R, _mask(first, B, T))
-            _e2e(out.cpu().numpy()[:, :, None, :], exp_out, f"step {step} W {W}")
-            for b, s in enumerate(first):
-                assert not bool(dbg_p[b, :, :s].any()), f"step {step} W {W}: probabilities below the window"
+            try:
+                _, _, nxt, _ = checked_call(cache, st, q, kn, vn, (g, kb, vb, R), starts=starts, window=W)
+            except AssertionError as e:
+                raise AssertionError(f"step {step} W {W}: {e}") from None
         twin.decode_attention(0, qd, kd, vd)
-        _, _, st = ref.decode_step(st, q, kn, vn, g, kb, vb, R)
+        st = nxt
         cache.advance()
         twin.advance()
-        _exports_equal(cache, twin, f"step {step}")
+        tuple_equal(cache.export(0), twin.export(0), f"step {step}")
     assert cache.read_state() == twin.read_state()
 
 
@@ -118,13 +66,14 @@ def test_window_covering_everything_is_the_unpadded_call(kb, vb, g, R, H, Hkv):
     dev = torch.device("cuda")
     rng = np.random.default_rng(5 + kb + g)
     B, n0 = 3, 5 * R + 17
-    a, b = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, window=n0 + 1), _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
-    k, v = (torch.from_numpy(_rand(rng, (B, Hkv, n0, 128))).to(dev) for _ in range(2))
+    a, b = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, sliding_window=n0 + 1), make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8)
+    k, v = (torch.from_numpy(rand16(rng, (B, Hkv, n0, 128))).to(dev) for _ in range(2))
     a.prefill(0, k, v)
     b.prefill(0, k, v)
     for step in range(4):
-        q, kn, vn = (torch.from_numpy(_rand(rng, s)).to(dev) for s in ((B, H, 128), (B, Hkv, 128), (B, Hkv, 128)))
-        _bits_equal(a.decode_attention(0, q, kn, vn), b.decode_attention(0, q, kn, vn), f"step {step}")
+        q, kn, vn = (torch.from_numpy(rand16(rng, s)).to(dev) for s in ((B, H, 128), (B, Hkv, 128), (B, Hkv, 128)))
+        oa, ob = a.decode_attention(0, q, kn, vn), b.decode_attention(0, q, kn, vn)
+        assert torch.equal(oa.view(torch.int16), ob.view(torch.int16)), f"step {step}"
         a.sliding_window += 1
         a.advance()
         b.advance()
@@ -136,8 +85,8 @@ def test_blocks_below_the_window_are_not_read():
     dev = torch.device("cuda")
     rng = np.random.default_rng(9)
     B, H, Hkv, kb, vb, g, R, n0, W = 3, 4, 2, 2, 4, 32, 128, 1000, 300
-    clean = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, window=W)
-    k, v = (torch.from_numpy(_rand(rng, (B, Hkv, n0, 128))).to(dev) for _ in range(2))
+    clean = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, sliding_window=W)
+    k, v = (torch.from_numpy(rand16(rng, (B, Hkv, n0, 128))).to(dev) for _ in range(2))
     clean.prefill(0, k, v)
     T = clean.kv_len + 1
     nb = (T - W) // 128                                              # blocks wholly below T - W
@@ -150,14 +99,14 @@ def test_blocks_below_the_window_are_not_read():
     tup[4][:, :, :nb * 128] = nan_word                               # V codes [B, Hkv, tv, 128 * vb / 32]
     tup[6][:, :, :nb * 128] = float("nan")                           # V scales / zeros [B, Hkv, tv, 128 / g]
     tup[7][:, :, :nb * 128] = float("nan")
-    bad = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, window=W)
+    bad = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 8, sliding_window=W)
     bad.import_tuple(0, tuple(tup))
-    q, kn, vn = (torch.from_numpy(_rand(rng, s)).to(dev) for s in ((B, H, 128), (B, Hkv, 128), (B, Hkv, 128)))
+    q, kn, vn = (torch.from_numpy(rand16(rng, s)).to(dev) for s in ((B, H, 128), (B, Hkv, 128), (B, Hkv, 128)))
     out_clean = clean.decode_attention(0, q, kn, vn).clone()
     out_bad = bad.decode_attention(0, q, kn, vn).clone()
     torch.cuda.synchronize()
     assert not torch.isnan(out_clean).any()
-    _bits_equal(out_clean, out_bad, "poisoned blocks below the window")
+    assert torch.equal(out_clean.view(torch.int16), out_bad.view(torch.int16)), "poisoned blocks below the window"
     bad.sliding_window = None                                        # the same cache through the additive-mask path
     m = torch.zeros((B, T), dtype=torch.float16, device=dev)
     m[:, :T - W] = float(NEG16)
@@ -174,8 +123,8 @@ def test_window_in_captured_step(kb, vb, g, R, H, Hkv, padded):
     dev = torch.device("cuda")
     rng = np.random.default_rng(21 + kb + int(padded))
     B, n0, W, steps = 3, 4 * R + R - 3, 160, 40
-    cache = _mk_cache(B, H, Hkv, kb, vb, g, R, n0 + steps + 4, window=W)
-    k, v = _rand(rng, (B, Hkv, n0, 128)), _rand(rng, (B, Hkv, n0, 128))
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + steps + 4, sliding_window=W)
+    k, v = rand16(rng, (B, Hkv, n0, 128)), rand16(rng, (B, Hkv, n0, 128))
     starts = [0, 70, n0 - 30] if padded else None
     cache.prefill(0, torch.from_numpy(k).to(dev), torch.from_numpy(v).to(dev),
                   kv_start=None if starts is None else torch.tensor(starts))
@@ -196,12 +145,12 @@ def test_window_in_captured_step(kb, vb, g, R, H, Hkv, padded):
     cache.state.copy_(state0)                                        # capture does not execute; the warm-up did not advance
     for step in range(steps):
         T = cache.kv_len + 1
-        q, kn, vn = _rand(rng, (B, H, 1, 128), 0.7), _rand(rng, (B, Hkv, 1, 128)), _rand(rng, (B, Hkv, 1, 128))
+        q, kn, vn = rand16(rng, (B, H, 1, 128), 0.7), rand16(rng, (B, Hkv, 1, 128)), rand16(rng, (B, Hkv, 1, 128))
         for dst, src in ((qb, q), (kb_, kn), (vb_, vn)):
             dst.copy_(torch.from_numpy(np.ascontiguousarray(src[:, :, 0])))
         graph.replay()
         cache._mirror_advance()
         torch.cuda.synchronize()
-        exp_out, _, st = ref.decode_step(st, q, kn, vn, g, kb, vb, R, _mask(_visible(starts, B, T, W), B, T))
-        _e2e(out.cpu().numpy()[:, :, None, :], exp_out, f"replay {step}")
+        exp_out, _, st = ref.decode_step(st, q, kn, vn, g, kb, vb, R, hidden_mask(B, T, starts, W))
+        assert_e2e(out.cpu().numpy()[:, :, None, :], exp_out, f"replay {step}")
     assert cache.read_state()[:6] == [cache.tk, cache.r, cache.tv, cache.L, cache.vhead, cache.kv_len]

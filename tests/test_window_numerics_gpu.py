@@ -3,8 +3,8 @@ unpadded entries are: every instantiation at every window-edge position, value m
 windows cut into many warp ranges per unit, the benchmarked Mistral-7B layer, the window combined with an additive mask,
 and a captured step replayed over a long walk.
 
-Each window is checked as _checked_step checks a step (tests/test_decode_gpu.py), except that the cache is advanced only
-after the step's last window: the production and instrumented epilogues give the same bits, every stage matches the oracle
+Each window is checked as checked_step checks a step (tests/_attn.py), except that the cache is advanced only after the
+step's last window: the production and instrumented epilogues give the same bits, every stage matches the oracle
 applied to the kernel's previous stage with the equivalent finfo(fp16).min mask below the per-sequence visible start
 max(clamp(kv_start), T - W), the output matches end to end at the suite's bar, and the kernel's probabilities are exactly 0
 wherever the mask hides a position.  After the step the exported cache equals the oracle's 9-tuple bit for bit.
@@ -12,15 +12,14 @@ wherever the mask hides a position.  After the step the exported cache equals th
 The window's start s = T - W is placed on purpose, from the host mirror of the lengths (tk, r, tv, L, vhead): on the
 edges where the kernels switch between a wholly hidden, a partly visible and a wholly visible item, in every kind of item
 (packed K / V block, fp16 K window row, V ring row of either ring segment)."""
-import itertools
-
 import numpy as np
 import pytest
 import torch
 
+from oracle import ref
+from tests._attn import (E2E_ATOL_FRAC, E2E_RTOL, NEG16, _slab, assert_e2e, check_stages, checked_call, hidden_mask,
+                         instantiation_cases, make_cache, mirror_lengths, rand16, tuple_equal)
 from tests._util import to_np
-from tests.test_decode_gpu import (BITS, E2E_ATOL_FRAC, E2E_RTOL, GQA_CHUNKS, GROUPS, NEG16, RESIDUALS, _mirror_lengths,
-                                   _oracle_prefill, _oracle_step, _slab, _stage_checks, _start_mask, _tuple_equal)
 
 pytestmark = pytest.mark.gpu
 
@@ -28,63 +27,8 @@ D = 128
 SQRT_D = 11.313708
 
 
-def _cache(B, H, Hkv, kb, vb, g, R, max_tokens, G, W=1):
-    from kivi_b200.cache import KiviCache
-    return KiviCache(1, B, H, Hkv, D, kb, vb, g, R, max_tokens, gqa_chunk=G, sliding_window=W)
-
-
-def _visible(starts, B, T, W):
-    """visible_start() of kivi_attn.cuh per sequence: max(clamp(kv_start, 0, T - 1), T - W)."""
-    return [max(min(max(0 if starts is None else int(starts[b]), 0), T - 1), T - W) for b in range(B)]
-
-
-def _e2e(got, exp, what):
-    e, x = got.astype(np.float64), exp.astype(np.float64)
-    err = np.abs(e - x)
-    tol = E2E_RTOL * np.abs(x) + E2E_ATOL_FRAC * np.abs(x).max()
-    assert (err <= tol).all(), f"{what}: end-to-end worst err / bar {(err / np.maximum(tol, 1e-30)).max():.2f}"
-
-
-def _window_step(cache, st, q, kn, vn, g, kb, vb, R, starts, W, user=None):
-    """One call of the window entry with window W on the cache's current state (oracle 9-tuple `st`), every check of
-    _checked_step but the cache update.  user: an additive fp16 mask [B, T] (0 or finfo.min) passed with the window; the
-    oracle then hides a position wherever either one hides it.  Returns (oracle output, oracle probabilities, the
-    kernel's scaled logits with the hidden positions set to finfo.min)."""
-    B, H = q.shape[:2]
-    T = st[8] + 1
-    what = f"T {T} W {W}"
-    cache.sliding_window = W
-    qd, kd, vd = (torch.from_numpy(np.ascontiguousarray(a[:, :, 0])).cuda() for a in (q, kn, vn))
-    md = None if user is None else torch.from_numpy(user).cuda()
-    dbg_s = torch.zeros((B, H, T + 8), dtype=torch.float16, device="cuda")
-    dbg_p = torch.zeros_like(dbg_s)
-    out_fast = cache.decode_attention(0, qd, kd, vd, mask=md).clone()
-    out = cache.decode_attention(0, qd, kd, vd, mask=md, dbg_logits=dbg_s, dbg_probs=dbg_p)
-    torch.cuda.synchronize()
-    assert torch.equal(out_fast.view(torch.int16), out.view(torch.int16)), f"{what}: production and instrumented epilogues"
-    mask = _start_mask(_visible(starts, B, T, W), B, T)
-    if user is not None:
-        mask[user.reshape(B, 1, 1, T) == NEG16] = NEG16
-    got_out = to_np(out)[:, :, None, :]
-    got_s, got_p = to_np(dbg_s)[:, :, None, :T].copy(), to_np(dbg_p)[:, :, None, :T]
-    hidden = np.broadcast_to(mask == NEG16, got_s.shape)
-    assert not got_p[hidden].any(), f"{what}: probabilities at hidden positions"
-    got_s[hidden] = NEG16                                            # not part of the kernel's result
-    try:
-        _stage_checks(st, q, kn, vn, g, kb, vb, R, got_out, got_s, got_p, mask=np.broadcast_to(mask, (B, H, 1, T)))
-    except AssertionError as e:
-        raise AssertionError(f"{what}: {e}") from None
-    exp_out, exp_p, _ = _oracle_step(st, q, kn, vn, g, kb, vb, R, mask)
-    _e2e(got_out, exp_out, what)
-    return exp_out, exp_p, got_s
-
-
-def _rand(rng, shape, scale=1.0):
-    return (rng.standard_normal(shape) * scale).astype(np.float16)
-
-
 def _step_inputs(rng, B, H, Hkv):
-    return _rand(rng, (B, H, 1, D), 0.7), _rand(rng, (B, Hkv, 1, D)), _rand(rng, (B, Hkv, 1, D))
+    return rand16(rng, (B, H, 1, D), 0.7), rand16(rng, (B, Hkv, 1, D)), rand16(rng, (B, Hkv, 1, D))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -114,20 +58,7 @@ def _edge_windows(cache):
     return out
 
 
-def _edge_cases():
-    """The 36 (k_bits, v_bits, g, G) kernels, unpadded and left-padded; R and ratio chosen as _instantiation_cases does."""
-    cases = []
-    for (ik, kb), (iv, vb), g, (iG, G), padded in itertools.product(enumerate(BITS), enumerate(BITS), GROUPS,
-                                                                      enumerate(GQA_CHUNKS), (False, True)):
-        Rs = [R for R in RESIDUALS if R % g == 0]
-        R = Rs[(2 * ik + iv + iG + padded) % len(Rs)]
-        ratio = 2 * G if (2 * ik + iv + iG + GROUPS.index(g)) % 5 == 0 else G
-        cases.append(pytest.param(kb, vb, g, G, R, ratio, padded,
-                                  id=f"k{kb}v{vb}-g{g}-G{G}-R{R}-ratio{ratio}-{'padded' if padded else 'unpadded'}"))
-    return cases
-
-
-@pytest.mark.parametrize("kb,vb,g,G,R,ratio,padded", _edge_cases())
+@pytest.mark.parametrize("kb,vb,g,G,R,ratio,padded", instantiation_cases("padded"))
 def test_every_instantiation_at_every_window_edge(kb, vb, g, G, R, ratio, padded):
     """Prefill to r = R - 3 at 600-1000 tokens, then six steps that cross a K flush and wrap the V ring; at every step a
     window per edge class (_edge_windows).  Padded: one unpadded sequence, one start in a partly padded block, one in
@@ -137,13 +68,13 @@ def test_every_instantiation_at_every_window_edge(kb, vb, g, G, R, ratio, padded
     n0 = max(3, -(-600 // R)) * R + R - 3
     rng = np.random.default_rng(1000 * kb + 100 * vb + g + 7 * G + R + ratio + 3 * padded)
     B = 4 if padded else 2
-    tk0, r0, tv0, _ = _mirror_lengths(n0, R)
+    tk0, r0, tv0, _ = mirror_lengths(n0, R)
     starts = [0, 130, tv0 + 1, tk0 + r0 // 2] if padded else None
-    cache = _cache(B, H, Hkv, kb, vb, g, R, n0 + 16, G)
-    k, v = _rand(rng, (B, Hkv, n0, D)), _rand(rng, (B, Hkv, n0, D))
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 16, gqa_chunk=G)
+    k, v = rand16(rng, (B, Hkv, n0, D)), rand16(rng, (B, Hkv, n0, D))
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda(),
                   kv_start=None if starts is None else torch.tensor(starts))
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
     reached, arms = set(), set()
     for step in range(6):
         T = cache.kv_len + 1
@@ -153,7 +84,7 @@ def test_every_instantiation_at_every_window_edge(kb, vb, g, G, R, ratio, padded
             by_w.setdefault(W, []).append(cls)
         for W, classes in sorted(by_w.items()):
             try:
-                _window_step(cache, st, q, kn, vn, g, kb, vb, R, starts, W)
+                _, _, nxt, _ = checked_call(cache, st, q, kn, vn, (g, kb, vb, R), starts=starts, window=W)
             except AssertionError as e:
                 raise AssertionError(f"step {step}, s = T - W = {T - W} {classes}: {e}") from None
             reached.update(classes)
@@ -161,8 +92,8 @@ def test_every_instantiation_at_every_window_edge(kb, vb, g, G, R, ratio, padded
                 if 0 < x < T - 1 and T - W > 0:
                     arms.add("window" if T - W > x else "kv_start" if x > T - W else "equal")
         cache.advance()
-        _, _, st = _oracle_step(st, q, kn, vn, g, kb, vb, R)
-        _tuple_equal(cache.export(0), st)
+        st = nxt
+        tuple_equal(cache.export(0), st, f"step {step}")
     assert reached == set(EDGE_CLASSES), f"edge classes never reached: {sorted(set(EDGE_CLASSES) - reached)}"
     assert r0 == R - 3 and cache.r == 3 and cache.vhead >= 2, "the steps crossed a K flush and wrapped the V ring"
     if padded:
@@ -206,7 +137,7 @@ def test_magnitudes_at_the_window_edge(kname, place):
     B, Hkv = 1, 2
     H = G * Hkv
     n0 = max(3, -(-900 // R)) * R + R - 3
-    tk, r, tv, L = _mirror_lengths(n0, R)
+    tk, r, tv, L = mirror_lengths(n0, R)
     p = _peak_position(place, tk, tv, g)
     rng = np.random.default_rng(PLACES.index(place) * 31 + kb * 7 + vb + g + G)
     k = rng.standard_normal((B, Hkv, n0, D))
@@ -218,9 +149,10 @@ def test_magnitudes_at_the_window_edge(kname, place):
         v[0, hk, p - 3:p, 0], v[0, hk, p - 3:p, 1] = -VBIG, VBIG
     k, v = k.astype(np.float16), v.astype(np.float16)
     assert np.isfinite(k).all() and np.isfinite(v).all()
-    cache = _cache(B, H, Hkv, kb, vb, g, R, n0 + 16, G)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 16, gqa_chunk=G)
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda())
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
+    cfg = (g, kb, vb, R)
     ratio = H // Hkv
     for step in range(2):
         T = cache.kv_len + 1
@@ -230,21 +162,21 @@ def test_magnitudes_at_the_window_edge(kname, place):
         assert p // 128 == (p + 1) // 128 or kind_k == "window", "s = p + 1 lies in the peak's block: partly visible"
         q = np.repeat(qbase[:, :, None, :], ratio, axis=1) + rng.standard_normal((B, H, 1, D)) * 0.01
         q = q.astype(np.float16)
-        kn, vn = _rand(rng, (B, Hkv, 1, D)), _rand(rng, (B, Hkv, 1, D))
+        kn, vn = rand16(rng, (B, Hkv, 1, D)), rand16(rng, (B, Hkv, 1, D))
         # just inside: the peak carries almost all of the mass, and its logit leads every other visible one by PEAK_GAP
-        exp_out, exp_p, got_s = _window_step(cache, st, q, kn, vn, g, kb, vb, R, None, T - p)
+        exp_out, exp_p, _, got_s = checked_call(cache, st, q, kn, vn, cfg, window=T - p)
         assert np.isfinite(exp_out).all(), "precondition: the oracle output is finite"
         assert (exp_p[..., p] > 0.99).all(), "precondition: the visible peak carries the mass"
         rest = np.delete(got_s.astype(np.float64), p, axis=-1).max(-1)
         assert (got_s[..., p].astype(np.float64) - rest > PEAK_GAP).all(), "precondition: the peak's logit advantage"
         # just outside: the peak and the VBIG rows hidden
-        exp_out, exp_p, _ = _window_step(cache, st, q, kn, vn, g, kb, vb, R, None, T - p - 1)
+        exp_out, exp_p, nxt, _ = checked_call(cache, st, q, kn, vn, cfg, window=T - p - 1)
         assert np.isfinite(exp_out).all(), "precondition: the oracle output is finite"
         assert (exp_p[..., p - 3:p + 1] == 0).all() and (exp_p.max(-1) < 0.5).all(), "precondition: a spread softmax"
         assert np.abs(exp_out).max() < 10.0, "precondition: the VBIG rows do not reach the oracle output"
         cache.advance()
-        _, _, st = _oracle_step(st, q, kn, vn, g, kb, vb, R)
-        _tuple_equal(cache.export(0), st)
+        st = nxt
+        tuple_equal(cache.export(0), st, f"step {step}")
         if st[6] is not None:
             assert np.isfinite(st[6]).all(), "precondition: finite V scales"
 
@@ -270,18 +202,17 @@ def test_long_windows_many_ranges_per_unit(name):
     B, H, Hkv, kb, vb, g, R, G, T, starts = LONG[name]
     n0 = T - 1
     rng = np.random.default_rng(T + H + Hkv + kb)
-    k, v = _rand(rng, (B, Hkv, n0, D)), _rand(rng, (B, Hkv, n0, D))
-    cache = _cache(B, H, Hkv, kb, vb, g, R, T + 16, G)
+    k, v = rand16(rng, (B, Hkv, n0, D)), rand16(rng, (B, Hkv, n0, D))
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, T + 16, gqa_chunk=G)
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda(),
                   kv_start=None if starts is None else torch.tensor(starts))
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
     del k, v
-    q, kn, vn = _rand(rng, (B, H, 1, D), 0.5), _rand(rng, (B, Hkv, 1, D)), _rand(rng, (B, Hkv, 1, D))
+    q, kn, vn = rand16(rng, (B, H, 1, D), 0.5), rand16(rng, (B, Hkv, 1, D)), rand16(rng, (B, Hkv, 1, D))
     for W in (T - 1, 16384, 4097, 129):
-        _window_step(cache, st, q, kn, vn, g, kb, vb, R, starts, W)
+        _, _, nxt, _ = checked_call(cache, st, q, kn, vn, (g, kb, vb, R), starts=starts, window=W)
     cache.advance()
-    _, _, st = _oracle_step(st, q, kn, vn, g, kb, vb, R)
-    _tuple_equal(cache.export(0), st)
+    tuple_equal(cache.export(0), nxt, "after the step")
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -304,7 +235,7 @@ def test_mistral_layer_window_4096_at_32k():
     B, H, Hkv, kb, vb, g, R, T, W = 16, 32, 8, 4, 4, 64, 64, 32768, 4096
     n0, ratio = T - 1, H // Hkv
     gen = torch.Generator(device="cuda").manual_seed(4096)
-    cache = _cache(B, H, Hkv, kb, vb, g, R, T + 64, 0, W)
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, T + 64, sliding_window=W)
     k = torch.randn((B, Hkv, n0, D), generator=gen, device="cuda", dtype=torch.float16)
     v = torch.randn((B, Hkv, n0, D), generator=gen, device="cuda", dtype=torch.float16)
     cache.prefill(0, k, v)
@@ -344,20 +275,15 @@ def test_mistral_layer_window_4096_at_32k():
     tol = E2E_RTOL * exp.abs() + E2E_ATOL_FRAC * exp.abs().amax(-1, keepdim=True)
     assert bool((err <= tol).all()), f"float64 reference: worst err / bar {float((err / tol.clamp_min(1e-30)).max()):.2f}"
     # a slab of units stage by stage against the oracle, then its cache update
-    mask = _start_mask([s0], 1, T)
+    after = {}
     for b, hk in [(0, 0), (9, 3), (15, 7)]:
         st4, q4, kn4, vn4, out4, s4, p4 = _slab(tup, q, kn, vn, out, dbg_s, dbg_p, b, hk, ratio)
-        s4 = s4[..., :T].copy()
-        s4[np.broadcast_to(mask == NEG16, s4.shape)] = NEG16
-        _stage_checks(st4, q4, kn4, vn4, g, kb, vb, R, out4, s4, p4[..., :T], mask=np.broadcast_to(mask, (1, ratio, 1, T)))
-        exp4, _, _ = _oracle_step(st4, q4, kn4, vn4, g, kb, vb, R, mask)
-        _e2e(out4, exp4, f"slab ({b}, {hk})")
+        _, _, after[b, hk], _ = check_stages(st4, q4, kn4, vn4, (g, kb, vb, R), out4, s4, p4, hidden_mask(1, T, window=W))
     cache.advance()
     tup2 = cache.export(0)
     for b, hk in [(0, 0), (15, 7)]:
-        st4, q4, kn4, vn4, *_ = _slab(tup, q, kn, vn, out, dbg_s, dbg_p, b, hk, ratio)
-        _, _, exp_st = _oracle_step(st4, q4, kn4, vn4, g, kb, vb, R)
-        _tuple_equal(tuple(None if t is None else t[b:b + 1, hk:hk + 1] for t in tup2[:8]) + (tup2[8],), exp_st)
+        got = tuple(None if t is None else t[b:b + 1, hk:hk + 1] for t in tup2[:8]) + (tup2[8],)
+        tuple_equal(got, after[b, hk], f"slab ({b}, {hk})")
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -371,13 +297,13 @@ def test_window_with_mask(kb, vb, g, R, G, H, Hkv, padded):
     B = 4
     n0 = max(3, -(-600 // R)) * R + R - 3
     rng = np.random.default_rng(kb + 10 * vb + g + R + padded)
-    tk0, r0, tv0, _ = _mirror_lengths(n0, R)
+    tk0, r0, tv0, _ = mirror_lengths(n0, R)
     starts = [0, 200, tv0 + 1, 50] if padded else None
-    cache = _cache(B, H, Hkv, kb, vb, g, R, n0 + 16, G)
-    k, v = _rand(rng, (B, Hkv, n0, D)), _rand(rng, (B, Hkv, n0, D))
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + 16, gqa_chunk=G)
+    k, v = rand16(rng, (B, Hkv, n0, D)), rand16(rng, (B, Hkv, n0, D))
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda(),
                   kv_start=None if starts is None else torch.tensor(starts))
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
     for step in range(4):                                            # the third step flushes the K window
         T = cache.kv_len + 1
         q, kn, vn = _step_inputs(rng, B, H, Hkv)
@@ -386,13 +312,13 @@ def test_window_with_mask(kb, vb, g, R, G, H, Hkv, padded):
             user = np.where(rng.random((B, T)) < 0.15, NEG16, 0).astype(np.float16)
             user[:, max(s - 6, 0):s + 6] = NEG16                    # a run across the window's start
             user[:, T - 1] = 0                                       # the new token stays visible
-            vis = _visible(starts, B, T, W)
+            vis = (hidden_mask(B, T, starts, W)[:, 0, 0] == NEG16).sum(-1)      # the first visible position
             assert all((user[b, x:T - 1] == NEG16).any() for b, x in enumerate(vis)), "the mask hides visible positions"
             assert all((user[b, :x] == NEG16).any() for b, x in enumerate(vis) if x > 0), "the mask hides hidden ones"
-            _window_step(cache, st, q, kn, vn, g, kb, vb, R, starts, W, user=user)
+            _, _, nxt, _ = checked_call(cache, st, q, kn, vn, (g, kb, vb, R), starts=starts, window=W, user=user)
         cache.advance()
-        _, _, st = _oracle_step(st, q, kn, vn, g, kb, vb, R)
-        _tuple_equal(cache.export(0), st)
+        st = nxt
+        tuple_equal(cache.export(0), st, f"step {step}")
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -407,10 +333,10 @@ def test_captured_window_step_over_a_long_walk():
     n0, steps = 1100 + R - 3, 300
     rng = np.random.default_rng(300)
     starts = [0, 300, n0 - 200]                                      # below T - W, crossed by it mid-walk, above it
-    cache = _cache(B, H, Hkv, kb, vb, g, R, n0 + steps + 8, G, W)
-    k, v = _rand(rng, (B, Hkv, n0, D)), _rand(rng, (B, Hkv, n0, D))
+    cache = make_cache(B, H, Hkv, kb, vb, g, R, n0 + steps + 8, gqa_chunk=G, sliding_window=W)
+    k, v = rand16(rng, (B, Hkv, n0, D)), rand16(rng, (B, Hkv, n0, D))
     cache.prefill(0, torch.from_numpy(k).cuda(), torch.from_numpy(v).cuda(), kv_start=torch.tensor(starts))
-    st = _oracle_prefill(k, v, g, kb, vb, R)
+    st = ref.prefill_cache(k, v, g, kb, vb, R)
     qb, kb_, vb_ = (torch.zeros(s, dtype=torch.float16, device="cuda") for s in ((B, H, D), (B, Hkv, D), (B, Hkv, D)))
     out = torch.zeros_like(qb)
     state0 = cache.state.clone()
@@ -435,10 +361,10 @@ def test_captured_window_step_over_a_long_walk():
         graph.replay()
         cache._mirror_advance()
         torch.cuda.synchronize()
-        exp_out, _, st = _oracle_step(st, q, kn, vn, g, kb, vb, R, _start_mask(_visible(starts, B, T, W), B, T))
-        _e2e(to_np(out)[:, :, None, :], exp_out, f"replay {step}")
+        exp_out, _, st = ref.decode_step(st, q, kn, vn, g, kb, vb, R, hidden_mask(B, T, starts, W))
+        assert_e2e(to_np(out)[:, :, None, :], exp_out, f"replay {step}")
         j0s.add((T - W) // 128)
         flushes += cache.tk != tk0
     assert len(j0s) >= 3 and flushes >= 4, (j0s, flushes)
     assert cache.read_state()[:6] == [cache.tk, cache.r, cache.tv, cache.L, cache.vhead, cache.kv_len]
-    _tuple_equal(cache.export(0), st)
+    tuple_equal(cache.export(0), st, "after the walk")
