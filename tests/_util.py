@@ -1,4 +1,6 @@
 """Shared helpers for the parity tests."""
+import hashlib
+
 import numpy as np
 import torch
 
@@ -40,3 +42,24 @@ def rand_quantised(rng, shape_rows_T, g, bits):
     from oracle import ref
     x = rng.standard_normal(shape_rows_T).astype(np.float16)
     return (x,) + ref.pack_lastdim(x, g, bits)
+
+
+EXT_CASES = [(2, 8, 8, 739, 128, 32), (2, 8, 2, 128, 1024, 32), (1, 4, 1, 333, 128, 64)]   # (B, nh, nh_kv, IC, OC, GS)
+
+
+def reference_extension_inputs(BIT):
+    """The seeded inputs of test_against_reference_cuda_extension, case by case: the packed weights in the reference
+    layout (code, scale, mn [nkv, IC, *]) and in the kernel layout (qw_t, sc_t, mn_t [nkv, *, IC])."""
+    from oracle import ref
+    rng = np.random.default_rng(1)
+    for (B, nh, nh_kv, IC, OC, GS) in EXT_CASES:
+        nkv = B * nh_kv
+        inp = rng.standard_normal((B * nh, 1, IC)).astype(np.float16)
+        w = rng.standard_normal((nkv, IC, OC)).astype(np.float16)
+        code, scale, mn = ref.pack_lastdim(w, GS, BIT)
+        kernel_layout = [np.ascontiguousarray(a.transpose(0, 2, 1)) for a in (code, scale, mn)]
+        yield (B, nh, nh_kv, IC, OC, GS), inp, (code, scale, mn), kernel_layout
+
+
+def input_digest(*arrays):
+    return hashlib.sha256(b"".join(np.ascontiguousarray(a).tobytes() for a in arrays)).digest()

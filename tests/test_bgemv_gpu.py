@@ -1,7 +1,6 @@
 """Parity of the CUDA dequant-GEMVs (kivi_bgemv.cu through the C ABI / Python surface) with the oracle
 (reference summation order, oracle/kivi_oracle.c) and with the stored outputs of the UNMODIFIED reference CUDA
 extension on the same inputs.  Tolerance: tests/_util.py."""
-import hashlib
 import os
 
 import numpy as np
@@ -9,7 +8,7 @@ import pytest
 import torch
 
 from oracle import ref
-from tests._util import assert_gemv_close, l1_mass_ref_layout, to_np
+from tests._util import assert_gemv_close, input_digest, l1_mass_ref_layout, reference_extension_inputs, to_np
 
 pytestmark = pytest.mark.gpu
 
@@ -137,26 +136,6 @@ def test_kernel_layout_reference_test_case(BIT, mqa):
     l1 = (x * np.repeat(wmax, (B * nh) // wmax.shape[0], 0)).sum(-1)[:, None, None]
     mean_rel = assert_gemv_close(to_np(out), exp, l1, f"kernel layout bit {BIT} mqa {mqa}")
     assert mean_rel < 1e-4
-
-
-EXT_CASES = [(2, 8, 8, 739, 128, 32), (2, 8, 2, 128, 1024, 32), (1, 4, 1, 333, 128, 64)]   # (B, nh, nh_kv, IC, OC, GS)
-
-
-def reference_extension_inputs(BIT):
-    """The seeded inputs of test_against_reference_cuda_extension, case by case: the packed weights in the reference
-    layout (code, scale, mn [nkv, IC, *]) and in the kernel layout (qw_t, sc_t, mn_t [nkv, *, IC])."""
-    rng = np.random.default_rng(1)
-    for (B, nh, nh_kv, IC, OC, GS) in EXT_CASES:
-        nkv = B * nh_kv
-        inp = rng.standard_normal((B * nh, 1, IC)).astype(np.float16)
-        w = rng.standard_normal((nkv, IC, OC)).astype(np.float16)
-        code, scale, mn = ref.pack_lastdim(w, GS, BIT)
-        kernel_layout = [np.ascontiguousarray(a.transpose(0, 2, 1)) for a in (code, scale, mn)]
-        yield (B, nh, nh_kv, IC, OC, GS), inp, (code, scale, mn), kernel_layout
-
-
-def input_digest(*arrays):
-    return hashlib.sha256(b"".join(np.ascontiguousarray(a).tobytes() for a in arrays)).digest()
 
 
 @pytest.mark.parametrize("BIT", [2, 4])

@@ -31,107 +31,34 @@ checkpoints.
 
 Transformers' eager attention turns a fully masked query row into NaN, and a left-padded prompt has such rows at its pad
 positions; the NaN then reaches real rows through 0 * NaN.  The prompt pass therefore gives transformers the 4-D mask
-that lets each pad query see itself (_hf_mask); what real rows see is unchanged.
+that lets each pad query see itself (tests/_hf.py: hf_prompt_mask); what real rows see is unchanged.
 """
 import pytest
 import torch
 
-from tests._hf import CASES, write_checkpoint
+from tests._hf import Bar, Decoder, checkpoints, hf_kw, hf_positions, load_kivi, pad_mask, reference_models  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-ALPHA, BETA = 4.0, 1e-3
-
-WORST = {}              # check -> worst err / max|hf16 - ref64| seen (printed at the end of the module)
-DECIDED = [0, 0]        # rows where the argmax check applied, rows compared
+bar = Bar()
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    print("\n[hf parity] worst max|ours - ref64| / max|hf16 - ref64| per check:")
-    for k, v in sorted(WORST.items()):
-        print(f"  {k:28s} {v[0]:.3f}   (err / max|ref64| {v[1]:.2e})")
-    print(f"  argmax checked on {DECIDED[0]} of {DECIDED[1]} rows")
-
-
-@pytest.fixture(scope="module")
-def checkpoints(tmp_path_factory):
-    made = {}
-
-    def get(name):
-        if name not in made:
-            path = tmp_path_factory.mktemp(name.replace(".", "_"))
-            write_checkpoint(name, path)
-            made[name] = path
-        return made[name]
-    return get
-
-
-def _reference_models(name, path):
-    import transformers
-    cls = getattr(transformers, CASES[name][0].replace("Config", "ForCausalLM"))
-    ref64 = cls.from_pretrained(str(path), dtype=torch.float64, attn_implementation="eager").cuda().eval()
-    hf16 = cls.from_pretrained(str(path), dtype=torch.float16, attn_implementation="eager").cuda().eval()
-    return ref64, hf16
-
-
-def check(what, ours, ref, hf):
-    """The bar on one logits tensor [..., vocab] (see the module docstring)."""
-    ours, ref, hf = (t.reshape(-1, t.shape[-1]).double() for t in (ours, ref, hf))
-    assert torch.isfinite(ours).all(), what
-    err = (ours - ref).abs().max().item()
-    hf_err = (hf - ref).abs().max().item()
-    scale = ref.abs().max().item()
-    bar = ALPHA * hf_err + BETA * scale
-    w = WORST.setdefault(what.split(" step")[0], [0.0, 0.0])
-    w[0], w[1] = max(w[0], err / hf_err), max(w[1], err / scale)
-    assert err <= bar, f"{what}: max|ours - ref64| = {err:.4g} > {bar:.4g} (hf16 {hf_err:.4g}, max|ref64| {scale:.4g})"
-    top2 = ref.topk(2, dim=-1).values
-    decided = (top2[:, 0] - top2[:, 1]) > 2 * bar
-    DECIDED[0] += int(decided.sum())
-    DECIDED[1] += decided.numel()
-    same = ours.argmax(-1) == ref.argmax(-1)
-    assert same[decided].all(), f"{what}: argmax differs on rows {torch.nonzero(decided & ~same).flatten().tolist()}"
-
-
-def _assert_decided(before, share=0.05):
-    """The precondition of the argmax check: the logits spread enough that it applies to a fair share of the rows."""
-    decided, rows = DECIDED[0] - before[0], DECIDED[1] - before[1]
-    assert decided >= share * rows, f"the argmax check applied to only {decided} of {rows} rows"
-
-
-def _positions(mask):
-    """What transformers' generate passes with a left-padded batch: cumsum - 1, pad positions 1."""
-    pos = mask.long().cumsum(-1) - 1
-    return pos.masked_fill(mask == 0, 1)
-
-
-def _hf_mask(kw, dtype):
-    """The left-padding mask as transformers' eager attention must be given it: 4-D additive, causal, pad keys hidden, and
-    each pad query seeing itself.  With the 2-D mask a pad query row is fully masked, transformers' eager softmax makes it
-    NaN, and the NaN reaches the real rows of the next layer through 0 * NaN.  Real rows see exactly what the 2-D mask
-    gives them."""
-    if "attention_mask" not in kw:
-        return kw
-    mask = kw["attention_mask"].bool()
-    n = mask.shape[1]
-    keep = mask[:, None, None, :] & torch.ones(n, n, dtype=torch.bool, device=mask.device).tril()
-    keep |= torch.eye(n, dtype=torch.bool, device=mask.device)
-    add = torch.zeros(keep.shape, dtype=dtype, device=mask.device).masked_fill(~keep, torch.finfo(dtype).min)
-    return dict(kw, attention_mask=add)
+    bar.report("hf parity")
 
 
 def _prompt(name, model, ref64, hf16, ids, pads, forward=True, tag=""):
     """model(ids) (the 9-tuple forward, every real position) and prefill(ids) (the last position) against the reference
     on a left-padded batch (pads[b] pad tokens in front of row b; all 0 = no mask).  Returns prefill's logits."""
     B, n = ids.shape
-    mask = (torch.arange(n, device="cuda")[None, :] >= torch.tensor(pads, device="cuda")[:, None]).long()
+    mask = pad_mask(pads, n)
     padded = any(pads)
-    kw = dict(attention_mask=mask, position_ids=_positions(mask)) if padded else {}
-    out = ref64(input_ids=ids, output_attentions=not padded, **_hf_mask(kw, torch.float64))
+    kw = dict(attention_mask=mask, position_ids=hf_positions(mask)) if padded else {}
+    out = ref64(input_ids=ids, output_attentions=not padded, **hf_kw(kw, torch.float64))
     ref = out.logits
-    hf = hf16(input_ids=ids, **_hf_mask(kw, torch.float16)).logits
+    hf = hf16(input_ids=ids, **hf_kw(kw, torch.float16)).logits
     if not padded:      # the precondition: attention is peaked, so a position or mask error changes the logits
         for layer, att in enumerate(out.attentions):
             peak = att[:, :, -1].max(-1).values.mean().item()
@@ -141,94 +68,10 @@ def _prompt(name, model, ref64, hf16, ids, pads, forward=True, tag=""):
         model.fused_forward = False                           # forward() on the reference's own 9-tuples
         ours = model(input_ids=ids, **kw).logits
         model.fused_forward = True
-        check(f"{name} forward{tag}", ours[real], ref[real], hf[real])
+        bar.check(f"{name} forward{tag}", ours[real], ref[real], hf[real])
     last = model.prefill(ids, attention_mask=mask if padded else None)
-    check(f"{name} prefill{tag}", last, ref[:, -1], hf[:, -1])
+    bar.check(f"{name} prefill{tag}", last, ref[:, -1], hf[:, -1])
     return last
-
-
-def _kv(model, layer):
-    """Post-RoPE K, V [B, Hkv, T, 128] in fp64 from the cache's export(): codes dequantised exactly, then the windows."""
-    from oracle import ref
-    c, cache = model.config, model.cache
-    g = c.group_size
-    sharded = cache.tensor_parallel
-    cache.tensor_parallel = sharded and model.tp_world > 1          # at world 1 the one rank holds every head
-    try:
-        kc, kfull, ks, km, vc, vfull, vs, vm, _ = cache.export(layer)
-    finally:
-        cache.tensor_parallel = sharded
-    ks_, vs_ = [], []
-    if kc is not None:
-        codes = torch.from_numpy(ref.unpack_codes_lastdim(kc.cpu().numpy(), c.k_bits)).cuda().double()
-        k = codes * ks.double().repeat_interleave(g, -1) + km.double().repeat_interleave(g, -1)
-        ks_.append(k.transpose(2, 3))
-    if kfull is not None:
-        ks_.append(kfull.double())
-    if vc is not None:
-        codes = torch.from_numpy(ref.unpack_codes_lastdim(vc.cpu().numpy(), c.v_bits)).cuda().double()
-        vs_.append(codes * vs.double().repeat_interleave(g, -1) + vm.double().repeat_interleave(g, -1))
-    vs_.append(vfull.double())
-    return torch.cat(ks_, 2), torch.cat(vs_, 2)
-
-
-class Decoder:
-    """Teacher-forced decode steps on the model, each checked step against ref64 / hf16 seeded with the model's cache.
-    The test keeps its own books: T (the shared length), pos[b] (row b's next position) and start[b] (row b's first
-    visible timeline position; None = a released slot, which sees its own token only)."""
-
-    def __init__(self, name, model, ref64, hf16, T, pos, start, seed=0):
-        self.name, self.model, self.ref64, self.hf16 = name, model, ref64, hf16
-        self.T, self.pos, self.start = T, list(pos), list(start)
-        self.gen = torch.Generator(device="cuda").manual_seed(seed)
-        self.step_no, self.flushes, self.vpacks, self.flushed = 0, 0, 0, False
-
-    def _reference(self, tok):
-        from transformers import DynamicCache
-        B, T = len(self.pos), self.T
-        kv = [_kv(self.model, layer) for layer in range(len(self.model.model.layers))]
-        assert kv[0][0].shape[2] == T
-        mask = torch.zeros(B, T + 1, dtype=torch.long, device="cuda")
-        for b, s in enumerate(self.start):
-            mask[b, T if s is None else s:] = 1
-        pos = torch.tensor(self.pos, device="cuda").view(B, 1)
-        logits = []
-        for m, dt in ((self.ref64, torch.float64), (self.hf16, torch.float16)):
-            cache = DynamicCache()
-            for layer, (k, v) in enumerate(kv):
-                cache.update(k.to(dt), v.to(dt), layer)
-            logits.append(m(input_ids=tok.view(B, 1), past_key_values=cache, attention_mask=mask,
-                            position_ids=pos).logits[:, -1])
-        return logits
-
-    def run(self, steps, tag=""):
-        model, cache = self.model, self.model.cache
-        B = len(self.pos)
-        for s in range(steps):
-            checked = s < 3 or s >= steps - 3 or self.step_no % 7 == 0 or self.flushed
-            tok = torch.randint(0, model.config.vocab_size, (B,), device="cuda", generator=self.gen)
-            if checked:
-                ref, hf = self._reference(tok)
-            tk, tv = cache.tk, cache.tv
-            ours = model.decode_step(tok.view(B, 1), use_graph=self.step_no >= 2).clone()
-            if checked:
-                check(f"{self.name} decode{tag} step {self.step_no}", ours, ref, hf)
-            self.flushed = cache.tk > tk
-            self.flushes += int(self.flushed)
-            self.vpacks += cache.tv - tv
-            self.T += 1
-            self.pos = [p + 1 for p in self.pos]
-            self.step_no += 1
-        assert cache.kv_len == self.T
-
-
-def _load(name, path, **kw):
-    """The reference's documented usage: the transformers config of the checkpoint, KIVI attributes set on it."""
-    import transformers
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI
-    config = getattr(transformers, CASES[name][0]).from_pretrained(str(path))
-    config.k_bits, config.v_bits, config.group_size, config.residual_length = CASES[name][2]
-    return LlamaForCausalLM_KIVI.from_pretrained(str(path), config=config, device_map="cuda", **kw)
 
 
 @pytest.mark.parametrize("name,tp", [("llama2", False), ("llama3", False), ("llama3.1", False), ("mistral", False),
@@ -237,10 +80,10 @@ def test_prompt_and_decode_match_transformers(checkpoints, name, tp):
     """Prompt pass unpadded and left-padded (0, 17, n - 5 pads) at B = 3, then 2R + 3 or more decode steps after each
     prefill, crossing K flushes and wrapping the V ring.  tp: the tensor-parallel loader at world 1 (safetensors read slice
     by slice), which has no 9-tuple forward."""
-    decided0 = list(DECIDED)
+    decided0 = list(bar.decided)
     path = checkpoints(name)
-    ref64, hf16 = _reference_models(name, path)
-    model = _load(name, path, tensor_parallel=tp)
+    ref64, hf16 = reference_models(name, path)
+    model = load_kivi(name, path, tensor_parallel=tp)
     if tp:
         name += " tp"
     R = model.config.residual_length
@@ -255,14 +98,16 @@ def test_prompt_and_decode_match_transformers(checkpoints, name, tp):
         _prompt(name, plain, ref64, hf16, ids, [0] * B, forward=False, tag=" config.json")
         del plain
     for pads in ([0] * B, [0, 17, n - 5]):
+        tag = " padded" if any(pads) else ""
         model.init_cache(B, n + steps + 8)
-        _prompt(name, model, ref64, hf16, ids, pads, forward=not tp, tag=" padded" if any(pads) else "")
-        dec = Decoder(name, model, ref64, hf16, T=n, pos=[n - p for p in pads], start=list(pads), seed=sum(pads))
+        _prompt(name, model, ref64, hf16, ids, pads, forward=not tp, tag=tag)
+        dec = Decoder(bar, model, ref64, hf16, T=n, pos=[n - p for p in pads], start=pads,
+                      gen=torch.Generator(device="cuda").manual_seed(sum(pads)))
         tk0 = model.cache.tk
-        dec.run(steps, tag=" padded" if any(pads) else "")
+        dec.run(steps, f"{name} decode{tag}")
         assert model.cache.tk > tk0 and dec.flushes >= 2, "the steps must cross K flushes"
         assert model.cache.vhead != 0 and dec.vpacks > model.cache.v_res_cap, "the steps must wrap the V ring"
-    _assert_decided(decided0)
+    bar.assert_decided(decided0)
 
 
 def test_continuous_batching_matches_transformers(checkpoints):
@@ -270,10 +115,10 @@ def test_continuous_batching_matches_transformers(checkpoints):
     at B = 1, then positions n, n + 1, ... over the last n timeline positions), releases slot 1 (its own token only, from
     position 0), shifts the timeline by 128 and keeps decoding across K flushes and the V ring."""
     name = "llama3.1"
-    decided0 = list(DECIDED)
+    decided0 = list(bar.decided)
     path = checkpoints(name)
-    ref64, hf16 = _reference_models(name, path)
-    model = _load(name, path)
+    ref64, hf16 = reference_models(name, path)
+    model = load_kivi(name, path)
     R = model.config.residual_length
     B, n = 4, 200
     pads = [128, 5, 0, 136]             # the live rows start at 128 or later, so a shift of 128 keeps them whole
@@ -281,24 +126,25 @@ def test_continuous_batching_matches_transformers(checkpoints):
     ids = torch.randint(0, model.config.vocab_size, (B, n), device="cuda", generator=gen)
     model.init_cache(B, n + 3 * R + 64)
     _prompt(name, model, ref64, hf16, ids, pads, forward=False, tag=" batch")
-    dec = Decoder(name, model, ref64, hf16, T=n, pos=[n - p for p in pads], start=list(pads), seed=3)
-    dec.run(10, tag=" batch")
+    dec = Decoder(bar, model, ref64, hf16, T=n, pos=[n - p for p in pads], start=pads,
+                  gen=torch.Generator(device="cuda").manual_seed(3))
+    dec.run(10, f"{name} decode batch")
     # a new request in slot 2
     n_new = 40
     prompt = torch.randint(0, model.config.vocab_size, (1, n_new), device="cuda", generator=gen)
     got = model.insert(2, prompt)
-    check(f"{name} insert", got[None], ref64(input_ids=prompt).logits[:, -1], hf16(input_ids=prompt).logits[:, -1])
+    bar.check(f"{name} insert", got[None], ref64(input_ids=prompt).logits[:, -1], hf16(input_ids=prompt).logits[:, -1])
     dec.pos[2], dec.start[2] = n_new, dec.T - n_new
-    dec.run(R // 2, tag=" inserted")
+    dec.run(R // 2, f"{name} decode inserted")
     # slot 1 idles: it sees its own token only, from position 0
     model.release(1)
     dec.pos[1], dec.start[1] = 0, None
-    dec.run(10, tag=" released")
+    dec.run(10, f"{name} decode released")
     # drop the first 128 timeline positions
     tk0 = model.cache.tk
     model.cache.shift(128)
     dec.T -= 128
     dec.start = [None if s is None else s - 128 for s in dec.start]
-    dec.run(2 * R + 3, tag=" shifted")
+    dec.run(2 * R + 3, f"{name} decode shifted")
     assert model.cache.tk > tk0 - 128 and model.cache.vhead != 0 and dec.flushes >= 2    # flushes after the shift
-    _assert_decided(decided0)
+    bar.assert_decided(decided0)

@@ -1,5 +1,5 @@
 """Sampling on the GPU.  Kernel level (kivi_sample_f32 through glue.sample) against the numpy reference of
-tests/test_sample_cpu.py: the uniform number bit for bit, greedy rows, the kept set, the chosen id, the distribution,
+tests/_sample.py: the uniform number bit for bit, greedy rows, the kept set, the chosen id, the distribution,
 determinism across placements, argument errors.  Model level: generate(do_sample=True), serve() with per-request
 parameters, tensor parallelism."""
 import os
@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from tests._attn import tiny_model
-from tests.test_sample_cpu import greedy_id, reference_pick, reference_row, uniform24
+from tests._sample import greedy_id, reference_pick, reference_row, uniform24
 
 pytestmark = pytest.mark.gpu
 
