@@ -16,7 +16,8 @@ import pytest
 import torch
 
 from oracle import ref
-from tests._util import assert_gemv_close, l1_mass_ref_layout, to_np
+from tests._gemv import OUTLIER_CHANNELS, edge_rows, rtol_bar  # noqa: F401  (the tests use OUTLIER_CHANNELS)
+from tests._util import to_np
 
 E2E_RTOL, E2E_ATOL_FRAC = 2e-2, 5e-3       # end-to-end |err| <= 2e-2*|ref| + 5e-3*max|ref|
 NEG16 = np.finfo(np.float16).min
@@ -98,31 +99,13 @@ def _slab(tup, q, kn, vn, out, dbg_s, dbg_p, b, hk, ratio):
 
 
 # ---------------------------------------------------------------------------------------------------
-# edge values (the rows of test_pack_edge_values) and outlier channels
+# edge values (the rows of test_pack_edge_values, tests/_gemv.py) as K and V
 # ---------------------------------------------------------------------------------------------------
-OUTLIER_CHANNELS = [5, 37, 77, 120]
-
-
-def _edge_rows(bits, finite):
-    """The rows of test_pack_edge_values (64 values each: two groups of 32).  finite=False adds the rows whose group range
-    overflows fp16 (large magnitudes, +-60000: the scale becomes inf)."""
-    rng = np.random.default_rng(5)
-    rows = [np.full(64, 1.25),                                                        # constant -> degenerate group
-            np.zeros(64),
-            np.concatenate([np.linspace(0, 3, 32), np.linspace(-7, 8, 32)]),         # ties / grid points
-            rng.standard_normal(64) * 6e-6,                                           # fp16 subnormals
-            np.arange(64) % (2 ** bits) * 0.5]                                        # exact levels
-    if not finite:
-        rows += [rng.standard_normal(64) * 2e4,
-                 np.concatenate([[-60000.0, 60000.0], rng.standard_normal(62)])]
-    return [r.astype(np.float16) for r in rows]
-
-
 def _put_k_edges(k, pos0, kb):
     """K channel 3 + 17e of token t (absolute position pos0 + t) = row e at t mod 64: whole quantisation groups along
     tokens.  Sequence 0 gets the finite rows, sequence 1 all of them."""
     for b in range(k.shape[0]):
-        rows = _edge_rows(kb, finite=(b == 0))
+        rows = edge_rows(kb, finite=(b == 0))
         for e, row in enumerate(rows):
             k[b, :, :, 3 + 17 * e] = row[(pos0 + np.arange(k.shape[2])) % 64]
 
@@ -130,7 +113,7 @@ def _put_k_edges(k, pos0, kb):
 def _put_v_edges(v, pos0, vb):
     """Token t with (pos0 + t) % 5 == 2 of every sequence is an edge row over its 128 channels (two rows of 64)."""
     for b in range(v.shape[0]):
-        rows = _edge_rows(vb, finite=(b == 0))
+        rows = edge_rows(vb, finite=(b == 0))
         for t in range(v.shape[2]):
             p = pos0 + t
             if p % 5 == 2:
@@ -179,6 +162,15 @@ def assert_e2e(got, exp, what):
     err = np.abs(e - x)
     tol = E2E_RTOL * np.abs(x) + E2E_ATOL_FRAC * np.abs(x).max(initial=0.0)
     assert (err <= tol).all(), f"{what}: end-to-end worst err / bar {(err / np.maximum(tol, 1e-30)).max():.2f}"
+
+
+def l1_mass_ref_layout(fA, scales, zeros, maxq):
+    """Upper bound of sum_k |x_k| * max_n |s*c+z| per (b, head): fA [B,H,1,K], scales/zeros [B,Hkv,K,G]."""
+    x = np.abs(np.asarray(fA, np.float64))[:, :, 0, :]                                  # [B,H,K]
+    w = (np.abs(np.asarray(scales, np.float64)) * maxq + np.abs(np.asarray(zeros, np.float64))).max(-1)  # [B,Hkv,K]
+    rep = x.shape[1] // w.shape[1]
+    w = np.repeat(w, rep, axis=1)
+    return (x * w).sum(-1)[:, :, None, None]                                            # [B,H,1,1]
 
 
 def _step16(x):
@@ -248,7 +240,7 @@ def _stage_checks(st, q, k_new, v_new, cfg, got_out, got_s, got_p, mask=None):
         exp_out = out_r
     # rtol covers one rounding step of a normal fp16 output (2^-10 relative at most); a subnormal output's step is 2^-24
     l1o = l1o + np.where(np.abs(exp_out.astype(np.float64)) < 2.0 ** -14, 2.0 ** -24 / 1e-6, 0.0)
-    assert_gemv_close(got_out, exp_out, l1o, "attention output (own probs)")
+    rtol_bar(got_out, exp_out, l1o, "attention output (own probs)")
 
 
 def check_stages(st, q, kn, vn, cfg, got_out, got_s, got_p, mask, bad=()):

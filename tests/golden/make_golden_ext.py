@@ -17,7 +17,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 
 from oracle import build_ref  # noqa: E402
-from tests._util import input_digest, reference_extension_inputs  # noqa: E402
+from tests._gemv import reference_extension_inputs  # noqa: E402
+from tests._util import input_digest  # noqa: E402
 
 
 def main(out_dir):

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from oracle import ref, torch_ref
+from tests._gemv import check_gemv
 from tests._util import to_np
 
 pytestmark = pytest.mark.gpu
@@ -82,8 +83,8 @@ def test_4d_qmatmul_reference_case(bits):
     """quant/test.py:173-202 `test_4d_qmatmul`: seed 0, integer-valued k = randint(10) [16, 32, 1024, 128] and
     q = randint(5), g 64; quant_and_pack_kcache -> transpose to the "trans" layout (:190-193) -> q.K^T through
     triton_bmm_fA_qB_outer, against torch.matmul on the unquantised k.  Asserted: no NaN (:197-198); the kernel equals
-    the fp32 evaluation of sum q*(s*c+z) on its own packed operands (1e-3 rtol + floor) on ALL units, the C oracle of
-    the reference kernel on a slab; and the distance to the unquantised matmul stays within the quantisation step."""
+    the fp32 evaluation of sum q*(s*c+z) on its own packed operands (1e-3 rtol + floor) on ALL units, the exact bar of
+    tests/_gemv.py on a slab; and the distance to the unquantised matmul stays within the quantisation step."""
     from quant.matmul import triton_bmm_fA_qB_outer
     from quant.new_pack import quant_and_pack_kcache, unpack_and_dequant_kcache
     torch.manual_seed(0)
@@ -99,7 +100,7 @@ def test_4d_qmatmul_reference_case(bits):
     our_out = triton_bmm_fA_qB_outer(group_size, query_state, code_t, scale_t, mn_t, bits)
     ref_out = torch.matmul(query_state, k.transpose(2, 3))
     assert not bool(our_out.isnan().any()) and not bool(ref_out.isnan().any())       # :197-198
-    # fp32 evaluation on the packed operands
+    # fp32 evaluation on the packed operands, on the device: the only check of all 16 x 32 units (too many for the C oracle)
     fpi = 32 // bits
     shifts = torch.arange(fpi, device="cuda", dtype=torch.int32) * bits
     c = ((code.unsqueeze(3) >> shifts.view(1, 1, 1, fpi, 1)) & (2 ** bits - 1)).reshape(BS, nh, T, D).float()
@@ -110,13 +111,10 @@ def test_4d_qmatmul_reference_case(bits):
     l1 = torch.einsum("bhd,bhtd->bht", query_state[:, :, 0].double().abs(), w.double().abs())
     err = (our_out[:, :, 0].double() - exact).abs()
     assert bool((err <= 1e-3 * exact.abs() + 1e-6 * l1 + 2 ** -11 * exact.abs()).all()), float(err.max())
-    # C oracle of the reference CUDA kernel on a slab (the Triton kernel computes the same sum, fp32 accumulate)
-    sb = slice(4, 5)
-    exp = ref.bmm_fA_qB_outer(group_size, to_np(query_state[sb, :2]), to_np(code_t[sb, :2].contiguous()),
-                              to_np(scale_t[sb, :2].contiguous()), to_np(mn_t[sb, :2].contiguous()), bits) if bits != 8 else None
-    if exp is not None:
-        d = np.abs(to_np(our_out[sb, :2]).astype(np.float64) - exp.astype(np.float64))
-        assert (d <= 1e-3 * np.abs(exp.astype(np.float64)) + 1e-6 * to_np(l1[sb, :2])[:, :, None, :]).all(), d.max()
+    if bits != 8:                    # the C oracle of the reference kernel (the same sum, fp32 accumulate) on a slab
+        sb = slice(4, 5)
+        slab = (to_np(t[sb, :2].contiguous()) for t in (our_out, query_state, code_t, scale_t, mn_t))
+        check_gemv("bmm", *slab, group_size, bits, "4d qmatmul slab")
     # the printed metric (:199-202): relative gap to the unquantised product, bounded by the step size
     gap = torch.nan_to_num((our_out - ref_out) / ref_out)
     assert float(gap.float().abs().mean()) < {8: 0.01, 4: 0.05, 2: 0.3}[bits]
@@ -154,12 +152,8 @@ def test_streaming_kvcache_reference_case():
         v_code, v_scale, v_mn = torch.cat([v_code, c], 2), torch.cat([v_scale, s], 2), torch.cat([v_mn, m], 2)
         out = triton_bmm_fA_qB_outer(group_size, w, v_code, v_scale, v_mn, bits)
         # (a) oracle on the same operands
-        exp_q = ref.bmm_fA_qB_outer(group_size, to_np(q), to_np(k_code), to_np(k_scale), to_np(k_mn), bits)
-        d = np.abs(to_np(att_q).astype(np.float64) - exp_q.astype(np.float64))
-        assert (d <= 1e-3 * np.abs(exp_q.astype(np.float64)) + 2e-3).all(), (i, d.max())
-        exp_o = ref.bmm_fA_qB_outer(group_size, to_np(w), to_np(v_code), to_np(v_scale), to_np(v_mn), bits)
-        d = np.abs(to_np(out).astype(np.float64) - exp_o.astype(np.float64))
-        assert (d <= 1e-3 * np.abs(exp_o.astype(np.float64)) + 2e-4).all(), (i, d.max())
+        check_gemv("bmm", to_np(att_q), *map(to_np, (q, k_code, k_scale, k_mn)), group_size, bits, f"step {i} q.K^T")
+        check_gemv("bmm", to_np(out), *map(to_np, (w, v_code, v_scale, v_mn)), group_size, bits, f"step {i} p.V")
         ec, es, em = ref.pack_lastdim(to_np(v_new), group_size, bits)
         np.testing.assert_array_equal(to_np(c), ec)
         # (b) against fp16 attention on the unquantised tensors
