@@ -1,24 +1,14 @@
 """N > 1 host logic on CPU: world_size-2 gloo run of the batch sharding + logits all-gather + identical
 greedy sampling (the only collective of the design, SURVEY 8e)."""
 import os
-import socket
 
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
+
+from tests._model import spawn_ranks
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, ws, port, gb, out_dir):
-    os.environ.update(RANK=str(rank), WORLD_SIZE=str(ws), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1",
-                      MASTER_PORT=str(port))
+def _worker(rank, ws, out_dir, gb):
     from kivi_b200 import dist as kdist
     r, w, _ = kdist.init(backend="gloo")
     assert (r, w) == (rank, ws)
@@ -40,12 +30,13 @@ def _worker(rank, ws, port, gb, out_dir):
     kdist.barrier()
     torch.save(toks, os.path.join(out_dir, f"toks{rank}.pt"))
     dist.destroy_process_group()
+    with open(os.path.join(out_dir, f"ok{rank}"), "w") as f:
+        f.write("ok")
 
 
 def test_dp_sharding_and_logits_allgather_gloo(tmp_path):
     for gb in (8, 7):                                            # even and ragged global batch
-        port = _free_port()
-        mp.spawn(_worker, args=(2, port, gb, str(tmp_path)), nprocs=2, join=True)
+        spawn_ranks(_worker, 2, tmp_path, gb)
         a, b = torch.load(tmp_path / "toks0.pt"), torch.load(tmp_path / "toks1.pt")
         assert torch.equal(a, b) and a.numel() == gb
 

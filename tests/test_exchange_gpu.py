@@ -2,10 +2,11 @@
 fused argmax + peer-store exchange against an NCCL all-gather of the same ids (one process per GPU, NCCL rendezvous on
 127.0.0.1)."""
 import os
-import socket
 
 import pytest
 import torch
+
+from tests._model import spawn_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -27,16 +28,7 @@ def test_greedy_sample_matches_torch_argmax():
         assert torch.equal(nxt, first)
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, ws, port, out_dir):
-    os.environ.update(RANK=str(rank), WORLD_SIZE=str(ws), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+def _worker(rank, ws, out_dir):
     import torch.distributed as dist
     from kivi_b200 import dist as kdist, glue
     kdist.init()
@@ -74,7 +66,4 @@ def _worker(rank, ws, port, out_dir):
 
 @pytest.mark.skipif(torch.cuda.is_available() and torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_peer_token_exchange_two_gpus(tmp_path):
-    import torch.multiprocessing as mp
-    ws = 2
-    mp.spawn(_worker, args=(ws, _free_port(), str(tmp_path)), nprocs=ws, join=True)
-    assert all((tmp_path / f"ok{r}").exists() for r in range(ws))
+    spawn_ranks(_worker, 2, tmp_path)

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from oracle import ref
+from tests._model import TupleBar, packed_parts_equal, tuple_prompt, tuple_steps
 from tests._util import to_np
 
 pytestmark = pytest.mark.gpu
@@ -45,7 +46,7 @@ _GQA_K4V4 = dict(num_attention_heads=4, num_key_value_heads=1, hidden_size=512, 
 
 
 @pytest.mark.parametrize("name,kw", [("tiny", {}), ("tiny", _GQA_K4V4), ("tiny", dict(attention_bias=True))])
-def test_fused_model_matches_tuple_model(name, kw):
+def test_fused_model_matches_tuple_model(name, kw, request):
     """LlamaForCausalLM_KIVI: prefill + greedy decode through the fused cache path (CUDA graph) and through
     the reference-style forward with per-layer 9-tuples give the same logits (two independent code paths).  With
     attention biases the tuple path keeps the module linears, the decode step adds the fused biases in its GEMMs."""
@@ -58,7 +59,7 @@ def test_fused_model_matches_tuple_model(name, kw):
             if pname.endswith(".bias"):
                 p.uniform_(-1.0, 1.0)                 # as large as the projections' outputs: a dropped bias must show
     ids = torch.randint(0, cfg.vocab_size, (2, 150), device="cuda")
-    _decode_against_tuple_path(model, ids, steps=40)
+    _decode_against_tuple_path(model, ids, 40, request.node.name)
 
 
 def test_one_token_prompt_is_prefilled():
@@ -76,7 +77,8 @@ def test_one_token_prompt_is_prefilled():
     model.prefill(one)
     assert model.cache.kv_len == 1
     assert model(input_ids=one).past_key_values[0][-1] == 1
-    _decode_against_tuple_path(model, one, steps=70)    # crosses a K flush (R = 64) and moves the V window
+    # 70 steps cross a K flush (R = 64) and move the V window
+    _decode_against_tuple_path(model, one, 70, "test_one_token_prompt_is_prefilled")
     # after a generate() of a longer prompt the same one-token prefill gives the bits it gives on a new cache
     model.generate(ids, max_new_tokens=8)
     got = model.prefill(one).clone()
@@ -85,40 +87,14 @@ def test_one_token_prompt_is_prefilled():
     assert torch.equal(got, model.prefill(one))
 
 
-def _decode_against_tuple_path(model, ids, steps):
-    """Prefill `ids`, then `steps` teacher-forced decode steps on the fused cache (eager, then the CUDA graph) and through
-    forward() on the reference's 9-tuples: logits within the tolerance, argmax equal in all but 3 steps, and the packed
-    cache parts equal bit for bit."""
-    model.fused_forward = False                       # forward() = the reference's own 9-tuple path (torch.cat growth, per-op launches)
-    B, n = ids.shape
-    # tuple path
-    logits_t, pasts = model(ids)
-    tok_t = logits_t[:, -1].argmax(-1, keepdim=True)
-    # fused path
-    model.init_cache(B, n + steps + 4)
-    logits_f = model.prefill(ids)
-    assert torch.allclose(logits_f, logits_t[:, -1], rtol=2e-2, atol=2e-2)
-    agree = 0
-    for s in range(steps):
-        # feed BOTH paths the same token so that the comparison stays aligned
-        tok = tok_t
-        lt, pasts = model(tok, pasts)
-        lf = model.decode_step(tok, use_graph=(s >= 2))
-        d = (lf - lt[:, -1]).abs().max().item()
-        scale = lt[:, -1].abs().max().item()
-        assert d <= 3e-2 * scale + 3e-2, f"step {s}: logits differ by {d} (scale {scale})"
-        agree += int((lf.argmax(-1) == lt[:, -1].argmax(-1)).all())
-        tok_t = lt[:, -1].argmax(-1, keepdim=True)
-    assert agree >= steps - 3
-    # cache contents of the two paths agree bit for bit in the packed parts
-    tup = model.cache.export(0)
-    ref_t = pasts[0]
-    for i in (0, 2, 3, 4, 6, 7):
-        if ref_t[i] is None:
-            assert tup[i] is None
-        else:
-            assert torch.equal(tup[i], ref_t[i].view_as(tup[i])), f"tuple[{i}]"
-    assert tup[8] == ref_t[8]
+def _decode_against_tuple_path(model, ids, steps, site):
+    """Prefill `ids`, then `steps` teacher-forced decode steps on the fused cache and through forward() on the reference's
+    9-tuples (tests/_model.py: TupleBar), and the packed cache parts equal."""
+    bar = TupleBar(site)
+    model.init_cache(ids.shape[0], ids.shape[1] + steps + 4)
+    pasts = tuple_steps(model, *tuple_prompt(model, ids, bar), steps, bar)
+    bar.done(steps)
+    packed_parts_equal(model.cache.export(0), pasts[0], "layer 0")
 
 
 def test_forward_loop_runs_on_the_fused_cache():
@@ -171,11 +147,10 @@ def test_forward_loop_runs_on_the_fused_cache():
     model.fused_forward = False
     lt2, tp2 = model(input_ids=tok_t, past_key_values=tp)
     assert isinstance(fp_[0], KiviPast) and fp_[0][-1] == tp2[0][-1] == n + 2
-    d = (lf - lt2).abs().max().item()
-    assert d <= 3e-2 * lt2.abs().max().item() + 3e-2, d
-    for i in (0, 2, 3, 4, 6, 7):
-        a, b = fp_[0][i], tp2[0][i]
-        assert (a is None and b is None) or torch.equal(a, b.view_as(a)), i
+    bar = TupleBar("test_forward_loop_runs_on_the_fused_cache")
+    bar.step(lf, lt2, "the step after the import")
+    bar.report()
+    packed_parts_equal(fp_[0], tp2[0], "layer 0")
     # a padding mask is outside the fused path: real 9-tuples come back
     model.fused_forward = True
     mask = torch.ones(B, n, dtype=torch.long, device="cuda")

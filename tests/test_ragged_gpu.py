@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from tests._attn import hidden_mask, left_padded, make_cache, tiny_model, tuple_equal
+from tests._model import TupleBar, packed_parts_equal, same_logits, tuple_prompt, tuple_steps
 
 pytestmark = pytest.mark.gpu
 
@@ -136,55 +137,25 @@ def test_padded_decode_step_graph_matches_eager():
     lg = model.prefill(ids, attention_mask=mask)
     lt = twin.prefill(ids, attention_mask=mask)
     assert torch.equal(lg, lt) and model.cache.ragged
-    tok = lg.argmax(-1, keepdim=True)
-    for step in range(10):
-        a = model.decode_step(tok).clone()
-        b = twin.decode_step(tok, use_graph=False).clone()
-        assert torch.equal(a, b), step
-        tok = a.argmax(-1, keepdim=True)
+    same_logits(model, twin, 10, lg.argmax(-1, keepdim=True), graph_a=True, graph_b=False)
 
 
 @pytest.mark.parametrize("name,kw", [("tiny", {}), ("tiny", dict(num_attention_heads=4, num_key_value_heads=1, hidden_size=512,
                                                                 k_bits=4, v_bits=4, group_size=64, residual_length=64))])
-def test_padded_model_matches_tuple_model(name, kw):
+def test_padded_model_matches_tuple_model(name, kw, request):
     """B = 3 left-padded prompts (one shorter than R: its padding reaches the fp16 windows), 40 steps across a K flush:
     the fused padded decode against the tuple path with the 2-D padding mask, both fed the same tokens."""
     model, cfg = tiny_model(0, **kw)
-    model.fused_forward = False                       # forward() = the reference's own 9-tuple path
     R = cfg.residual_length
     n, steps = 2 * R + R - 28 if R < 128 else R + 100, 40
     lengths = [n, n - 60, R // 2 - 5]
     ids, mask = left_padded(cfg, lengths, n, seed=3, low=0)
-    B = len(lengths)
-    pos = mask.long().cumsum(-1) - 1
-    pos.masked_fill_(mask == 0, 1)
-    logits_t, pasts = model(ids, attention_mask=mask, position_ids=pos)
-    model.init_cache(B, n + steps + 4)
-    logits_f = model.prefill(ids, attention_mask=mask)
-    assert torch.allclose(logits_f, logits_t[:, -1], rtol=2e-2, atol=2e-2)
-    tok_t = logits_t[:, -1].argmax(-1, keepdim=True)
-    nxt = pos[:, -1:] + 1
-    agree = 0
-    for s in range(steps):
-        tok = tok_t
-        mask = torch.cat([mask, torch.ones((B, 1), dtype=mask.dtype, device=mask.device)], 1)
-        lt, pasts = model(tok, pasts, attention_mask=mask, position_ids=nxt + s)
-        lf = model.decode_step(tok, use_graph=(s >= 2))
-        d = (lf - lt[:, -1]).abs().max().item()
-        scale = lt[:, -1].abs().max().item()
-        assert d <= 3e-2 * scale + 3e-2, f"step {s}: logits differ by {d} (scale {scale})"
-        agree += int((lf.argmax(-1) == lt[:, -1].argmax(-1)).all())
-        tok_t = lt[:, -1].argmax(-1, keepdim=True)
-    assert agree >= steps - 3
+    bar = TupleBar(request.node.name)
+    model.init_cache(len(lengths), n + steps + 4)
+    pasts = tuple_steps(model, *tuple_prompt(model, ids, bar, mask), steps, bar, mask=mask)
+    bar.done(steps)
     assert model.cache.tk > n - n % R, "the steps crossed a K flush"
-    tup = model.cache.export(0)
-    ref_t = pasts[0]
-    for i in (0, 2, 3, 4, 6, 7):
-        if ref_t[i] is None:
-            assert tup[i] is None
-        else:
-            assert torch.equal(tup[i], ref_t[i].view_as(tup[i])), f"tuple[{i}]"
-    assert tup[8] == ref_t[8]
+    packed_parts_equal(model.cache.export(0), pasts[0], "layer 0")
 
 
 def test_generate_with_masks():

@@ -9,6 +9,8 @@ import pytest
 import torch
 
 from tests._attn import tiny_model
+from tests._model import (graphs, requests, same_logits, same_on_all_ranks, sharded_model, small_cfg,  # noqa: F401
+                          spawn_ranks, world_one_pair)
 from tests._sample import greedy_id, reference_pick, reference_row, uniform24
 
 pytestmark = pytest.mark.gpu
@@ -321,43 +323,29 @@ def test_in_graph_sampler_is_the_stand_alone_call():
     assert draw.tolist() == [new] * B
 
 
-class _CountingGraph(torch.cuda.CUDAGraph):
-    made = 0
-
-    def __init__(self, *a, **kw):
-        super().__init__(*a, **kw)
-        type(self).made += 1
-
-
-def test_mode_flip_keeps_launch_count_and_greedy_bits(monkeypatch):
+def test_mode_flip_keeps_launch_count_and_greedy_bits(graphs):
     """generate() sets the mode it needs and leaves it: the step is recaptured when do_sample changes and only then, the
     launch count is the same in both modes, and greedy decoding after sampling is bit for bit a fresh model's."""
-    monkeypatch.setattr(_CountingGraph, "made", 0)
-    monkeypatch.setattr(torch.cuda, "CUDAGraph", _CountingGraph)
     model, cfg = tiny_model(3)
     fresh, _ = tiny_model(3)
     ids = _prompt(cfg, 2, 33, seed=5)
     g0 = model.generate(ids, max_new_tokens=12)
     greedy_launches = model.launches_per_step
-    assert _CountingGraph.made == 1 and not model._sampling
+    assert graphs.made == 1 and not model._sampling
     model.generate(ids, max_new_tokens=12, seed=1, **SAMPLED)
     assert model.launches_per_step == greedy_launches
-    assert _CountingGraph.made == 2 and model._sampling
+    assert graphs.made == 2 and model._sampling
     model.generate(ids, max_new_tokens=12, seed=2, **SAMPLED)              # other parameters, the same captured step
-    assert _CountingGraph.made == 2
+    assert graphs.made == 2
     g1 = model.generate(ids, max_new_tokens=12)
-    assert _CountingGraph.made == 3 and not model._sampling
+    assert graphs.made == 3 and not model._sampling
     assert torch.equal(g0, g1) and torch.equal(g1, fresh.generate(ids, max_new_tokens=12))
     model.generate(ids, max_new_tokens=12, seed=1, **SAMPLED)
     model.init_cache(2, 33 + 12)                                          # a new cache starts greedy
     fresh.init_cache(2, 33 + 12)
     a, b = model.prefill(ids), fresh.prefill(ids)
     assert torch.equal(a, b)
-    tok = a.argmax(-1).view(2, 1)
-    for step in range(11):
-        la, lb = model.decode_step(tok).clone(), fresh.decode_step(tok).clone()
-        assert torch.equal(la, lb) and torch.equal(model.next_tokens, fresh.next_tokens), step
-        tok = fresh.next_tokens.view(2, 1).clone()
+    same_logits(model, fresh, 11, a.argmax(-1).view(2, 1))
     with pytest.raises(RuntimeError):
         model.set_slot_sampling(0, temperature=1.0)                       # the step is greedy
     with pytest.raises(ValueError):
@@ -381,14 +369,7 @@ def test_p2p_exchange_with_sampling_is_rejected():
     assert model._sampling and model._dist_tokens is not None
 
 
-PROMPTS = [51, 41, 44, 49, 19, 43, 42, 23]
 BUDGETS = [57, 17, 52, 39, 58, 64, 75, 83]
-
-
-def _requests(cfg, params):
-    g = torch.Generator().manual_seed(0)
-    base = [(torch.randint(1, cfg.vocab_size, (n,), generator=g), m) for n, m in zip(PROMPTS, BUDGETS)]
-    return [r if par is None else r + (par,) for r, par in zip(base, params)]
 
 
 def test_serve_mixes_greedy_and_sampled_requests():
@@ -396,11 +377,11 @@ def test_serve_mixes_greedy_and_sampled_requests():
     model, cfg = tiny_model(2)
     par = lambda s: dict(temperature=1.2, top_k=30, top_p=0.9, seed=s)     # noqa: E731
     mixed = [None, par(1), None, par(2), par(3), None, par(4), None]
-    all_greedy = dict(serve(model, _requests(cfg, [None] * 8), 3, 260))
+    all_greedy = dict(serve(model, requests(cfg, BUDGETS, params=[None] * 8), 3, 260))
     stats = {}
-    a = dict(serve(model, _requests(cfg, mixed), 3, 260, stats=stats))
+    a = dict(serve(model, requests(cfg, BUDGETS, params=mixed), 3, 260, stats=stats))
     assert model._sampling                                                # serve() leaves the mode its requests needed
-    b = dict(serve(model, _requests(cfg, mixed), 3, 260))
+    b = dict(serve(model, requests(cfg, BUDGETS, params=mixed), 3, 260))
     assert stats["inserts"] >= 1 and sorted(a) == list(range(8))
     for i in range(8):
         assert a[i].shape == (BUDGETS[i],) and torch.equal(a[i], b[i]), i
@@ -409,33 +390,24 @@ def test_serve_mixes_greedy_and_sampled_requests():
     assert sum(not torch.equal(a[i], all_greedy[i]) for i in range(8) if mixed[i] is not None) >= 3
     others = [None if m is None else par(m["seed"] + 100) for m in mixed]
     others[3] = mixed[3]
-    c = dict(serve(model, _requests(cfg, others), 3, 260))
+    c = dict(serve(model, requests(cfg, BUDGETS, params=others), 3, 260))
     assert torch.equal(c[3], a[3])                                        # its own seed only
     assert sum(not torch.equal(c[i], a[i]) for i in (1, 4, 6)) >= 2
     # params {} is a sampled request with the defaults, not a greedy one
     empty, spelled = list(mixed), list(mixed)
     empty[1], spelled[1] = {}, dict(temperature=1.0, top_k=50, top_p=1.0, seed=0)
-    d, e = dict(serve(model, _requests(cfg, empty), 3, 260)), dict(serve(model, _requests(cfg, spelled), 3, 260))
+    d = dict(serve(model, requests(cfg, BUDGETS, params=empty), 3, 260))
+    e = dict(serve(model, requests(cfg, BUDGETS, params=spelled), 3, 260))
     assert torch.equal(d[1], e[1]) and not torch.equal(d[1], all_greedy[1])
-    again = dict(serve(model, _requests(cfg, [None] * 8), 3, 260))
+    again = dict(serve(model, requests(cfg, BUDGETS, params=[None] * 8), 3, 260))
     assert not model._sampling                                            # a list without params runs the greedy step
     for i in range(8):
         assert torch.equal(again[i], all_greedy[i]), i
 
 
-def _small_cfg():
-    from kivi_b200.llama_kivi import default_config
-    return default_config("tiny", hidden_size=1024, intermediate_size=2816, num_hidden_layers=4, num_attention_heads=8,
-                          num_key_value_heads=4, vocab_size=4096, residual_length=32, group_size=32)
-
-
 def test_tensor_parallel_world_one_samples_like_the_model():
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI
-    cfg = _small_cfg()
-    torch.manual_seed(0)
-    plain = LlamaForCausalLM_KIVI(cfg).half().cuda().eval()
-    tpm = LlamaForCausalLM_KIVI(cfg, tensor_parallel=True).half().cuda().eval()
-    tpm.load_state_dict(plain.state_dict())
+    cfg = small_cfg()
+    plain, tpm = world_one_pair(cfg)
     ids = _prompt(cfg, 3, 40, seed=2)
     mask = torch.ones_like(ids)
     mask[1, :9] = 0
@@ -445,27 +417,12 @@ def test_tensor_parallel_world_one_samples_like_the_model():
     assert plain.launches_per_step == tpm.launches_per_step
 
 
-def _tp_worker(rank, ws, port, out_dir):
-    os.environ.update(RANK=str(rank), WORLD_SIZE=str(ws), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+def _tp_worker(rank, ws, out_dir):
     import torch.distributed as dist
-    from kivi_b200 import dist as kdist, tp
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI
     from kivi_b200.serve import serve
-    kdist.init()
+    cfg = small_cfg()
+    model, _ = sharded_model(cfg, rank, ws)
     dev = torch.device("cuda", rank)
-    torch.cuda.set_device(dev)
-    cfg = _small_cfg()
-    torch.manual_seed(0)
-    full = {k: v.half() for k, v in LlamaForCausalLM_KIVI(cfg).state_dict().items()}
-    model = LlamaForCausalLM_KIVI(cfg, tensor_parallel=True)
-    model.load_state_dict(tp.shard_state_dict(full, cfg, rank, ws))
-    model = model.half().cuda().eval()
-
-    def same_on_all_ranks(t):
-        got = [torch.empty_like(t) for _ in range(ws)]
-        dist.all_gather(got, t.contiguous())
-        return all(torch.equal(got[0], x) for x in got)
-
     prompt = torch.randint(0, cfg.vocab_size, (2, 48), generator=torch.Generator().manual_seed(2)).to(dev)
     out = model.generate(prompt, max_new_tokens=2 * cfg.residual_length + 5, seed=5, **SAMPLED)
     assert same_on_all_ranks(out)
@@ -488,11 +445,4 @@ def test_sharded_sampling_two_gpus(tmp_path):
     """Every rank of a sharded model samples the same ids with no collective: same logits bits, same seeds, same counters."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    mp.spawn(_tp_worker, args=(2, port, str(tmp_path)), nprocs=2, join=True)
-    assert all((tmp_path / f"ok{r}").exists() for r in range(2))
+    spawn_ranks(_tp_worker, 2, tmp_path)

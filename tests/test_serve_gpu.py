@@ -7,6 +7,7 @@ import torch
 
 from oracle import ref
 from tests._attn import assert_e2e, hidden_mask, left_padded, make_cache, rand16, tiny_model, tuple_equal
+from tests._model import PROMPTS, TupleBar, graphs, packed_parts_equal, requests, same_logits, tuple_steps  # noqa: F401
 from tests._util import to_np
 
 pytestmark = pytest.mark.gpu
@@ -162,19 +163,9 @@ def test_shift(kb, vb, g, R, H, Hkv, blocks):
 GQA = dict(num_attention_heads=4, num_key_value_heads=1, hidden_size=512)
 
 
-class _CountingGraph(torch.cuda.CUDAGraph):
-    made = 0
-
-    def __init__(self, *a, **kw):
-        super().__init__(*a, **kw)
-        type(self).made += 1
-
-
-def test_graph_replays_after_refill_and_shift(monkeypatch):
+def test_graph_replays_after_refill_and_shift(graphs):
     """The step captured before an insert and a shift replays after them without a recapture, with logits bit-identical
     to the same model decoding without a graph."""
-    monkeypatch.setattr(_CountingGraph, "made", 0)
-    monkeypatch.setattr(torch.cuda, "CUDAGraph", _CountingGraph)
     model, cfg = tiny_model(5, **GQA)
     twin, _ = tiny_model(5, **GQA)
     twin.load_state_dict(model.state_dict())
@@ -183,10 +174,8 @@ def test_graph_replays_after_refill_and_shift(monkeypatch):
     for m in (model, twin):
         m.init_cache(3, 600)
         m.prefill(ids, attention_mask=mask)
-    for step in range(3):
-        a, b = model.decode_step().clone(), twin.decode_step(use_graph=False).clone()
-        assert torch.equal(a, b), step
-    assert _CountingGraph.made == 1
+    same_logits(model, twin, 3, graph_a=True, graph_b=False)
+    assert graphs.made == 1
     prompt = torch.randint(1, cfg.vocab_size, (40,), device="cuda")
     for m in (model, twin):
         m.release(0)
@@ -196,38 +185,27 @@ def test_graph_replays_after_refill_and_shift(monkeypatch):
     for m in (model, twin):
         m.cache.shift(128)
     assert model.cache.kv_len == n + 3 - 128
-    for step in range(6):
-        a, b = model.decode_step().clone(), twin.decode_step(use_graph=False).clone()
-        assert torch.equal(a, b), f"after the shift, step {step}"
-    assert _CountingGraph.made == 1
+    same_logits(model, twin, 6, graph_a=True, graph_b=False)
+    assert graphs.made == 1
 
 
-# prompt lengths and budgets with which 3 slots and max_tokens = 360 need two shifts (R = 128)
-PROMPTS = [51, 41, 44, 49, 19, 43, 42, 23]
-BUDGETS = [157, 117, 152, 139, 158, 164, 175, 183]
-
-
-def _requests(cfg, seed=0, prompts=PROMPTS):
-    g = torch.Generator().manual_seed(seed)
-    return [(torch.randint(1, cfg.vocab_size, (n,), generator=g), m) for n, m in zip(prompts, BUDGETS)]
+BUDGETS = [157, 117, 152, 139, 158, 164, 175, 183]     # with PROMPTS, 3 slots and max_tokens = 360 need two shifts (R = 128)
 
 
 @pytest.mark.parametrize("kw", [{}, GQA], ids=["tiny", "tiny-gqa"])
-def test_serve(kw, monkeypatch):
+def test_serve(kw, graphs):
     """8 requests through 3 slots: each gets exactly its token budget (or stops at the chosen EOS, which it then ends
     with), the step graph is captured once, and max_tokens forces two shifts."""
     from kivi_b200.serve import serve
-    monkeypatch.setattr(_CountingGraph, "made", 0)
-    monkeypatch.setattr(torch.cuda, "CUDAGraph", _CountingGraph)
     model, cfg = tiny_model(2, **kw)
-    reqs = _requests(cfg)
+    reqs = requests(cfg, BUDGETS)
     stats = {}
     got = dict(serve(model, reqs, 3, 360, stats=stats))
     assert sorted(got) == list(range(len(reqs)))
     for i, (_, m) in enumerate(reqs):
         assert got[i].shape == (m,), i
     assert stats["shifts"] >= 2 and stats["inserts"] == 5 and stats["prefills"] == 1
-    assert _CountingGraph.made == 1
+    assert graphs.made == 1
     eos = int(torch.cat(list(got.values())).bincount().argmax())          # the most frequent token ends some requests
     got_e = dict(serve(model, reqs, 3, 360, eos_token_id=eos))
     assert sorted(got_e) == list(range(len(reqs)))
@@ -238,12 +216,13 @@ def test_serve(kw, monkeypatch):
         assert len(t) == m or t[-1] == eos, i
         stopped += len(t) < m
     assert stopped > 0
-    assert _CountingGraph.made == 1
+    assert graphs.made == 1
 
 
 def test_inserted_request_matches_tuple_path():
     """An inserted sequence continued two ways from the same cache contents: the fused batch (its slot) and the
-    reference's tuple path on that slot's exported 9-tuples with its padding mask, fed the same tokens."""
+    reference's tuple path on that slot's exported 9-tuples with its padding mask, fed the same tokens; the slot's packed
+    cache parts equal the tuple path's after the steps."""
     model, cfg = tiny_model(3, **GQA)
     R = cfg.residual_length
     n = 2 * R + 100                                     # r = 105 after the prompt and 5 steps: the 40 steps flush K
@@ -260,30 +239,19 @@ def test_inserted_request_matches_tuple_path():
     pasts = [tuple(t.clone() if torch.is_tensor(t) else t for t in pk) for pk in pasts]
     pad = torch.zeros((1, T), dtype=torch.long, device="cuda")
     pad[:, T - p:] = 1
-    tok = first.argmax().view(1, 1)
-    model._ids[1] = tok[0, 0]
     model.fused_forward = False
-    steps, agree = 40, 0
-    for s in range(steps):
-        pad = torch.cat([pad, torch.ones((1, 1), dtype=pad.dtype, device="cuda")], 1)
-        lt, pasts = model(tok, pasts, attention_mask=pad, position_ids=torch.tensor([[p + s]], device="cuda"))
-        lf = model.decode_step().clone()
-        lt = lt[:, -1]
-        d = (lf[1] - lt[0]).abs().max().item()
-        scale = lt.abs().max().item()
-        assert d <= 3e-2 * scale + 3e-2, f"step {s}: logits differ by {d} (scale {scale})"
-        agree += int(lf[1].argmax() == lt[0].argmax())
-        tok = lt.argmax(-1, keepdim=True)
-        model._ids[1] = tok[0, 0]                       # both paths continue with the tuple path's token
-    assert agree >= steps - 3
+    bar, steps = TupleBar("test_inserted_request_matches_tuple_path"), 40
+    pasts = tuple_steps(model, pasts, first.argmax().view(1, 1), steps, bar, mask=pad, row=1)
+    bar.done(steps)
     assert model.cache.tk > T - T % R, "the steps crossed a K flush"
+    packed_parts_equal(_row(model.cache.export(0), 1), pasts[0], "slot 1, layer 0")
 
 
 def test_inserted_prompt_does_not_reach_other_requests():
     """Replacing an inserted request's prompt (same length and budget) changes no token of any other request."""
     from kivi_b200.serve import serve
     model, cfg = tiny_model(4)
-    reqs = _requests(cfg, seed=1)
+    reqs = requests(cfg, BUDGETS, seed=1)
     a = dict(serve(model, reqs, 3, 360))
     g = torch.Generator().manual_seed(99)
     swapped = list(reqs)

@@ -8,11 +8,12 @@ Two or more GPUs (one process per GPU, NCCL on 127.0.0.1): the sharded model's d
 sharded step (bit for bit) and against the unsharded model (tolerance), identical tokens on every rank, left-padded generate
 and serve()."""
 import os
-import socket
 from types import SimpleNamespace
 
 import pytest
 import torch
+
+from tests._model import same_logits, same_on_all_ranks, sharded_model, small_cfg, spawn_ranks, world_one_pair
 
 pytestmark = pytest.mark.gpu
 
@@ -124,13 +125,6 @@ def test_argument_errors_launch_nothing():
     torch.cuda.synchronize()
 
 
-def _small_cfg(**kw):
-    from kivi_b200.llama_kivi import default_config
-    return default_config("tiny", **dict(dict(hidden_size=1024, intermediate_size=2816, num_hidden_layers=4,
-                                              num_attention_heads=8, num_key_value_heads=4, vocab_size=4096,
-                                              residual_length=32, group_size=32), **kw))
-
-
 def _fill_cache(model, heads, n, seed, rank=0, world=1):
     """The same n random K/V tokens for every rank (this rank's KV heads of them), packed by the real prefill kernels."""
     c = model.cache
@@ -146,24 +140,15 @@ def _fill_cache(model, heads, n, seed, rank=0, world=1):
 def test_tensor_parallel_model_at_world_one_matches_the_model():
     """tensor_parallel=True on one GPU runs the sharded decode step (partials in the PeerAllReduce slots, the all-reduce
     kernel, the in-graph call counter) with one rank: its logits and tokens equal the plain model's bit for bit."""
-    from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI
-    cfg = _small_cfg()
-    torch.manual_seed(0)
-    plain = LlamaForCausalLM_KIVI(cfg).half().cuda().eval()
-    tpm = LlamaForCausalLM_KIVI(cfg, tensor_parallel=True).half().cuda().eval()
-    tpm.load_state_dict(plain.state_dict())
-    assert tpm.tp_world == 1
+    cfg = small_cfg()
+    plain, tpm = world_one_pair(cfg)
     B, n = 3, 70
     for m in (plain, tpm):
         m.init_cache(B, n + 2 * cfg.residual_length + 8)
         _fill_cache(m, cfg.num_key_value_heads, n, seed=5)
     ids = torch.randint(0, cfg.vocab_size, (B, 1), device="cuda")
-    for step in range(2 * cfg.residual_length + 3):                       # crosses a K flush and a V-ring wrap
-        lp = plain.decode_step(ids, use_graph=step >= 1).clone()
-        lt = tpm.decode_step(ids, use_graph=step >= 1).clone()
-        assert torch.equal(lp, lt), step
-        assert torch.equal(plain.next_tokens, tpm.next_tokens), step
-        ids = tpm.next_tokens.view(B, 1).clone()
+    graph = lambda s: s >= 1                                              # noqa: E731
+    same_logits(plain, tpm, 2 * cfg.residual_length + 3, ids, graph, graph)     # crosses a K flush and a V-ring wrap
     assert int(tpm._allreduce.epoch.item()) == (2 * cfg.residual_length + 3 + 1) * 2 * cfg.num_hidden_layers  # + warm-up
     # prompt pass, left padding and generate on the same path
     prompt = torch.randint(0, cfg.vocab_size, (2, 40), device="cuda")
@@ -181,14 +166,6 @@ def test_tensor_parallel_model_at_world_one_matches_the_model():
 
 
 # ------------------------------------------------------------------------------------------------ two or more GPUs
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 class _Emulation:
     """The sharded decode step of `world` ranks run on one GPU: one KiviCache per rank, the per-rank GEMMs of the same
     shapes as the ranks run, the partials added in fp32 in rank order, then add_rmsnorm."""
@@ -254,27 +231,14 @@ class _Emulation:
         return torch.mm(h, self.lm_head.t()).float()
 
 
-def _tp_worker(rank, ws, port, out_dir):
-    os.environ.update(RANK=str(rank), WORLD_SIZE=str(ws), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+def _tp_worker(rank, ws, out_dir):
     import torch.distributed as dist
-    from kivi_b200 import dist as kdist, tp
+    from kivi_b200 import tp
     from kivi_b200.llama_kivi import LlamaForCausalLM_KIVI
     from kivi_b200.serve import serve
-    kdist.init()
+    cfg = small_cfg()
+    model, full = sharded_model(cfg, rank, ws)
     dev = torch.device("cuda", rank)
-    torch.cuda.set_device(dev)
-    cfg = _small_cfg()
-    torch.manual_seed(0)
-    full = {k: v.half() for k, v in LlamaForCausalLM_KIVI(cfg).state_dict().items()}   # the same seeded weights on every rank
-    model = LlamaForCausalLM_KIVI(cfg, tensor_parallel=True)
-    model.load_state_dict(tp.shard_state_dict(full, cfg, rank, ws))
-    model = model.half().cuda().eval()
-
-    def same_on_all_ranks(t):
-        got = [torch.empty_like(t) for _ in range(ws)]
-        dist.all_gather(got, t.contiguous())
-        return all(torch.equal(got[0], x) for x in got)
-
     B, n, R = 4, 70, cfg.residual_length
     steps = 2 * R + 3                                                     # crosses a K flush and a V-ring wrap
     model.init_cache(B, n + steps + 8)
@@ -323,7 +287,5 @@ def _tp_worker(rank, ws, port, out_dir):
 def test_sharded_decode_multi_gpu(tmp_path, ws):
     if torch.cuda.device_count() < ws:
         pytest.skip(f"needs {ws} GPUs")
-    import torch.multiprocessing as mp
-    mp.spawn(_tp_worker, args=(ws, _free_port(), str(tmp_path)), nprocs=ws, join=True)
-    assert all((tmp_path / f"ok{r}").exists() for r in range(ws))
-    print(f"[tp] world {ws}: max |logits - unsharded| / max|logits| = {(tmp_path / 'ok0').read_text()}")
+    worst = spawn_ranks(_tp_worker, ws, tmp_path)
+    print(f"[tp] world {ws}: max |logits - unsharded| / max|logits| = {worst}")
