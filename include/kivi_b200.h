@@ -270,9 +270,11 @@ int kivi_cache_advance(const kivi_cache_t* cache, void* stream);
  * set instead of touching memory when the device-side lengths exceed what the call declared (max_kv_len, window
  * capacities): KIVI_STATE_ERR_CAPACITY.  kivi_cache_refill_f16 / kivi_cache_shift_f16 / kivi_cache_shift_state set
  * KIVI_STATE_ERR_LENGTHS instead of writing when the device-side lengths are not those the call was given.
+ * kivi_cache_reorder_f16 sets KIVI_STATE_ERR_ROWS instead of writing when a source row lies outside the batch.
  * kivi_cache_prefill_f16 / kivi_cache_import_f16 clear it. */
 #define KIVI_STATE_ERR_CAPACITY 1
 #define KIVI_STATE_ERR_LENGTHS  2
+#define KIVI_STATE_ERR_ROWS     4   /* kivi_cache_reorder_f16: a source row outside [0, batch); nothing was written */
 int kivi_cache_read_state(const kivi_cache_t* cache, int32_t* host_state8, void* stream);
 
 /* ------------------------------------------------------------------------------------------
@@ -308,6 +310,23 @@ int kivi_cache_shift_f16(const kivi_cache_t* cache, int shift, int tk, int tv, v
  * (kv_start: a device int32[B], or NULL).  RoPE positions are per sequence and do not change.  Same requirements on
  * `shift`; if the device-side tk or tv is below it, nothing changes and KIVI_STATE_ERR_LENGTHS is set. */
 int kivi_cache_shift_state(const kivi_cache_t* cache, int shift, int32_t* kv_start, void* stream);
+
+/* Beam search: reorder the batch rows of one layer.  For every b with src[b] != b, the Hkv units of sequence b become a
+ * byte copy of the units of sequence src[b] AS THEY WERE BEFORE THE CALL, for any map (duplicates, swaps, cycles, chains).
+ * A copied row receives the packed K blocks [0, ceil(tk/128)), the packed V blocks [0, ceil(tv/128)), and the whole fp16 K
+ * window and V ring of each unit at full capacity (their win_unit swizzle kept; the ring head vhead is shared by all rows,
+ * so ring slots map one to one).  tk and tv are read from `state` on the device, so a captured call follows the lengths as
+ * they change between replays.  Nothing else is written: not the rows with src[b] == b, not the blocks past the live ones,
+ * not `state`, not kv_start (the caller gathers kv_start[b] = kv_start[src[b]] itself).
+ *   src: device int32[batch], read on the device (it may change between replays of a captured call).  If any entry lies
+ *        outside [0, batch), nothing is written and KIVI_STATE_ERR_ROWS is set in state[6].
+ *   scratch: device memory of at least kivi_cache_reorder_scratch_bytes(cache) bytes, 16-byte aligned.  A row that is
+ *        rewritten AND read by another rewritten row is staged there first (launch 1); then every rewritten row copies
+ *        from the scratch or from the cache (launch 2).  One scratch serves all layers of a model on one stream.
+ * Two launches, no host synchronisation, no allocation; CUDA-graph capturable.  NULL pointers or a scratch that is too
+ * small return KIVI_ERR_* before any launch. */
+int64_t kivi_cache_reorder_scratch_bytes(const kivi_cache_t* cache);   /* one layer's rows at full capacity (< 0: KIVI_ERR_*) */
+int kivi_cache_reorder_f16(const kivi_cache_t* cache, const int32_t* src, void* scratch, int64_t scratch_bytes, void* stream);
 
 /* Copy the cache out in the reference's 9-tuple layout (models/llama_kivi.py:454-455); lengths are
  * passed by the host (it mirrors `state`).  k_code [U,128,tk/fpi] i32, k_scale/k_mn [U,128,tk/g],

@@ -8,6 +8,7 @@ A left-padded batch keeps one length for all sequences; `set_kv_start` names eac
 attention then skips the padding on the device (kivi_decode_attention_ragged_f16).  The same offsets let one batch row
 ("slot") take a new sequence while the others decode: `refill` writes a prompt right-aligned to the shared length,
 `release` idles a slot, and `shift` drops timeline positions that no live sequence sees any more.
+`reorder` makes batch rows copies of other rows on the device (beam search: each beam continues the row it extends).
 A cache built with `sliding_window` = W attends, like transformers' Mistral, to the last W positions only
 (kivi_decode_attention_window_f16): the packed blocks below the window are not read, and `shift` may drop them.
 """
@@ -68,6 +69,8 @@ def _bind():
     _lib.bind("kivi_cache_refill_f16", i32, [P, i32, vp, vp] + [i32] * 6 + [vp])
     _lib.bind("kivi_cache_shift_f16", i32, [P, i32, i32, i32, vp])
     _lib.bind("kivi_cache_shift_state", i32, [P, i32, vp, vp])
+    _lib.bind("kivi_cache_reorder_scratch_bytes", i64, [P])
+    _lib.bind("kivi_cache_reorder_f16", i32, [P, vp, vp, i64, vp])
     _BOUND = True
 
 
@@ -126,6 +129,10 @@ class KiviCache:
         self.kv_start = torch.zeros(batch, dtype=torch.int32, device=self.device)
         self.kv_start_host = [0] * batch                             # host mirror of kv_start (valid while `ragged`)
         self.ragged = False
+        # reorder(): the row map, device-resident so that a captured reorder reads the map written before each replay, and
+        # the staging scratch (allocated on the first reorder)
+        self.reorder_src = torch.arange(batch, dtype=torch.int32, device=self.device)
+        self._reorder_scratch = None
         # host mirror of `state` (its evolution is deterministic)
         self.tk = self.r = self.tv = self.L = self.vhead = self.kv_len = 0
 
@@ -237,6 +244,51 @@ class KiviCache:
         if self.ragged:
             self.kv_start_host = [s - tokens for s in self.kv_start_host]
 
+    # ------------------------------------------------------------------ beam search
+    def reorder(self, src):
+        """Batch row b of every layer becomes a copy of row src[b] as it was before the call (any map: duplicates, swaps,
+        cycles), and so does kv_start[b] while the batch is left-padded.  The lengths do not change.  src: batch ints in
+        [0, batch) (a list or a tensor; ValueError otherwise).  The first call allocates a staging scratch of one layer's
+        rows at full capacity, i.e. 1 / n_layers of nbytes(), kept for later calls."""
+        t = torch.as_tensor(src).reshape(-1)
+        if t.numel() != self.batch:
+            raise ValueError(f"reorder needs {self.batch} source rows, got {t.numel()}")
+        if t.is_floating_point() or t.is_complex() or t.dtype == torch.bool:
+            raise ValueError(f"reorder: source rows must be integers, got {t.dtype}")
+        rows = [int(x) for x in t.tolist()]
+        bad = [x for x in rows if not 0 <= x < self.batch]
+        if bad:
+            raise ValueError(f"reorder: source rows {bad} lie outside the batch of {self.batch}")
+        self.reorder_src.copy_(torch.tensor(rows, dtype=torch.int32))
+        self._enqueue_reorder()
+        self._mirror_reorder(rows)
+
+    def reorder_scratch(self) -> torch.Tensor:
+        """The staging scratch of reorder(), allocated on first use (before capturing _enqueue_reorder, call this)."""
+        if self._reorder_scratch is None:
+            nb = int(_lib.lib().kivi_cache_reorder_scratch_bytes(ctypes.byref(self._structs[0])))
+            if nb < 0:
+                _lib.check(nb, "kivi_cache_reorder_scratch_bytes")
+            self._reorder_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        return self._reorder_scratch
+
+    def _enqueue_reorder(self):
+        """The device half of reorder(), reading the map in `reorder_src`: two launches per layer and, while `ragged`, the
+        kv_start gather.  Capturable in a CUDA graph whose every replay is followed by _mirror_reorder(map)."""
+        scratch = self.reorder_scratch()
+        with torch.cuda.device(self.device):
+            stream = _lib.stream_ptr(self.device)
+            for layer in range(self.n_layers):
+                _lib.check(_lib.lib().kivi_cache_reorder_f16(ctypes.byref(self._structs[layer]), self.reorder_src.data_ptr(),
+                                                             scratch.data_ptr(), scratch.numel(), stream),
+                           "kivi_cache_reorder_f16")
+            if self.ragged:
+                self.kv_start.copy_(self.kv_start.index_select(0, self.reorder_src))
+
+    def _mirror_reorder(self, rows):
+        if self.ragged:
+            self.kv_start_host = [self.kv_start_host[s] for s in rows]
+
     # ------------------------------------------------------------------ operations
     def prefill(self, layer: int, k: torch.Tensor, v: torch.Tensor, kv_start=None):
         """k, v [B, Hkv, n, 128] fp16 (K post-RoPE): models/llama_kivi.py:425-452 in three launches.  kv_start: see
@@ -315,6 +367,9 @@ class KiviCache:
             _lib.check(_lib.lib().kivi_cache_read_state(ctypes.byref(self._structs[0]), host, _lib.stream_ptr(self.device)),
                        "kivi_cache_read_state")
         st = list(host)
+        if st[6] & 4:                                                # KIVI_STATE_ERR_ROWS
+            raise RuntimeError(f"kivi_b200: a row reorder refused to run (state error word {st[6]}): a source row lies "
+                               f"outside the batch of {self.batch}")
         if st[6] & 2:                                                # KIVI_STATE_ERR_LENGTHS
             raise RuntimeError(f"kivi_b200: a refill or shift refused to run (state error word {st[6]}): the device-side "
                                f"lengths {st[:6]} are not the ones the host passed")

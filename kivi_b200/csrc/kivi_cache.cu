@@ -8,6 +8,8 @@
 //   9-tuple               :454-455   -> kivi_cache_export_f16 (tests / interop only)
 // Continuous batching (no counterpart in the reference): kivi_cache_refill_f16 re-runs the prefill kernels for one sequence
 // of a live cache, kivi_cache_shift_f16 / kivi_cache_shift_state drop the oldest blocks of the shared timeline.
+// Beam search (the reference's _reorder_cache, :950-957, without the 9-tuples): kivi_cache_reorder_f16 makes batch rows
+// copies of other rows on the device.
 #include "kivi_decode.cuh"
 
 namespace kivi {
@@ -292,6 +294,80 @@ import_kv_kernel(CacheDesc c, int tk, int tv, int L, int r,
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Row reorder (beam search): sequence b's units become a copy of sequence src[b]'s units as they were before the call.
+// A unit's bytes are four regions: the live packed K blocks, the live packed V blocks (lengths from `state`), the whole
+// fp16 K window and the whole V ring.  The scratch holds one full-capacity slot per (row, unit), regions at the same
+// offsets, so the staging and the copy address source and destination alike.
+//   launch 1 (STAGE): row s is staged when it is rewritten (src[s] != s) and another rewritten row reads it;
+//   launch 2        : every rewritten row b copies from row s = src[b]: from the scratch if s was staged, else from the
+//                     cache, whose row s this call does not write.
+// One CTA per (unit of a row, chunk); grid.y = rows.  Any src outside [0, B) stops every CTA before it writes.
+// ------------------------------------------------------------------------------------------------
+constexpr int kReorderChunks = 4;                                                // CTAs per unit
+
+struct ReorderDesc { int64_t kb, vb, kw, vw; };                                  // bytes of the four full-capacity regions
+
+__device__ __forceinline__ void copy16(uint4* __restrict__ dst, const uint4* __restrict__ src, int64_t n, int lane, int stride)
+{
+    constexpr int kUnroll = 4;                                                   // loads in flight per thread before its stores
+    for (int64_t i = lane; i < n; i += (int64_t)kUnroll * stride) {
+        uint4 t[kUnroll];
+        #pragma unroll
+        for (int e = 0; e < kUnroll; ++e)
+            if (i + (int64_t)e * stride < n) t[e] = src[i + (int64_t)e * stride];
+        #pragma unroll
+        for (int e = 0; e < kUnroll; ++e)
+            if (i + (int64_t)e * stride < n) dst[i + (int64_t)e * stride] = t[e];
+    }
+}
+
+template <bool STAGE>
+__global__ void __launch_bounds__(256)
+reorder_rows_kernel(CacheDesc c, const int32_t* __restrict__ src, uint8_t* __restrict__ scratch, ReorderDesc r)
+{
+    const int row = blockIdx.y, h = blockIdx.x / kReorderChunks, chunk = blockIdx.x % kReorderChunks;
+    bool bad = false, read_by_other = false;
+    for (int b = threadIdx.x; b < c.B; b += blockDim.x) {
+        const int s = src[b];
+        bad |= s < 0 || s >= c.B;
+        read_by_other |= s == row && b != row;
+    }
+    bad = __syncthreads_or(bad);
+    read_by_other = __syncthreads_or(read_by_other);
+    if (bad) {
+        if (!STAGE && blockIdx.x == 0 && row == 0 && threadIdx.x == 0) atomicOr(&c.state[6], KIVI_STATE_ERR_ROWS);
+        return;
+    }
+    const int s = src[row];
+    if (s == row || (STAGE && !read_by_other)) return;                          // nothing to stage / row kept
+    const int64_t slot = r.kb + r.vb + r.kw + r.vw;                              // scratch bytes of one unit
+    const int64_t kbb = lay_block_bytes(c.k_bits, c.g), vbb = lay_block_bytes(c.v_bits, c.g);
+    const int64_t nk = (int64_t)min(cdiv(c.state[ST_TK], kBlockTokens), c.k_cap_blocks) * kbb;
+    const int64_t nv = (int64_t)min(cdiv(c.state[ST_TV], kBlockTokens), c.v_cap_blocks) * vbb;
+    // the unit's four regions in the cache (STAGE: the row itself; else: row s) and in the scratch
+    const int64_t us = (int64_t)(STAGE ? row : s) * c.Hkv + h, ud = (int64_t)row * c.Hkv + h;
+    const bool from_scratch = !STAGE && src[s] != s;                             // s is rewritten too: it was staged
+    const uint8_t* in[4]; uint8_t* out[4];
+    const uint8_t* cache_in[4] = {c.k_store + us * r.kb, c.v_store + us * r.vb,
+                                  reinterpret_cast<const uint8_t*>(c.k_res) + us * r.kw,
+                                  reinterpret_cast<const uint8_t*>(c.v_res) + us * r.vw};
+    uint8_t* sc = scratch + us * slot;
+    uint8_t* sc_regions[4] = {sc, sc + r.kb, sc + r.kb + r.vb, sc + r.kb + r.vb + r.kw};
+    uint8_t* cache_out[4] = {c.k_store + ud * r.kb, c.v_store + ud * r.vb,
+                             reinterpret_cast<uint8_t*>(c.k_res) + ud * r.kw, reinterpret_cast<uint8_t*>(c.v_res) + ud * r.vw};
+    const int64_t bytes[4] = {nk, nv, r.kw, r.vw};
+    #pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        in[i] = STAGE ? cache_in[i] : (from_scratch ? sc_regions[i] : cache_in[i]);
+        out[i] = STAGE ? sc_regions[i] : cache_out[i];
+    }
+    const int lane = chunk * blockDim.x + threadIdx.x, stride = kReorderChunks * blockDim.x;
+    #pragma unroll
+    for (int i = 0; i < 4; ++i)
+        copy16(reinterpret_cast<uint4*>(out[i]), reinterpret_cast<const uint4*>(in[i]), bytes[i] / 16, lane, stride);
+}
+
 int make_desc(const kivi_cache_t* k, CacheDesc* d)
 {
     if (!k) return KIVI_ERR_NULL;
@@ -485,4 +561,37 @@ extern "C" int kivi_cache_read_state(const kivi_cache_t* cache, int32_t* host_st
     cudaError_t e = cudaMemcpyAsync(host_state8, c.state, 8 * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
     return e == cudaSuccess ? KIVI_OK : (int)e;
+}
+
+static ReorderDesc reorder_desc(const CacheDesc& c)
+{
+    return ReorderDesc{(int64_t)c.k_cap_blocks * lay_block_bytes(c.k_bits, c.g), (int64_t)c.v_cap_blocks * lay_block_bytes(c.v_bits, c.g),
+                       (int64_t)c.R * kD * 2, (int64_t)c.v_res_cap * kD * 2};
+}
+
+extern "C" int64_t kivi_cache_reorder_scratch_bytes(const kivi_cache_t* cache)
+{
+    CacheDesc c;
+    int rc = make_desc(cache, &c);
+    if (rc) return rc;
+    const ReorderDesc r = reorder_desc(c);
+    return (int64_t)c.B * c.Hkv * (r.kb + r.vb + r.kw + r.vw);
+}
+
+extern "C" int kivi_cache_reorder_f16(const kivi_cache_t* cache, const int32_t* src, void* scratch, int64_t scratch_bytes,
+                                      void* stream)
+{
+    CacheDesc c;
+    int rc = make_desc(cache, &c);
+    if (rc) return rc;
+    if (!src || !scratch) return KIVI_ERR_NULL;
+    if (scratch_bytes < kivi_cache_reorder_scratch_bytes(cache)) return KIVI_ERR_SHAPE;
+    if (c.B > 65535) return KIVI_ERR_UNSUPPORTED;                                   // grid.y
+    const ReorderDesc r = reorder_desc(c);
+    const dim3 grid(c.Hkv * kReorderChunks, c.B);
+    reorder_rows_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(c, src, (uint8_t*)scratch, r);
+    rc = post_launch();
+    if (rc) return rc;
+    reorder_rows_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(c, src, (uint8_t*)scratch, r);
+    return post_launch();
 }

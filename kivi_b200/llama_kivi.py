@@ -492,6 +492,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self.cache: KiviCache | None = None
         self._graph = None
         self._graph_ragged = False          # the captured step calls the left-padded attention entry
+        self._reorder_graph = None          # beam search: the cache's row reorder + the position gather, captured
+        self.launches_per_reorder = None
         self._fast = None
         self._dist_tokens = None            # [world * B] ids gathered inside the step (greedy sampling, world > 1)
         self._dist_in_graph = True
@@ -702,7 +704,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
     @staticmethod
     def _reorder_cache(past_key_values, beam_idx):
         """models/llama_kivi.py:950-957 (beam search): select batch rows of every tensor of every layer's tuple; the
-        reference's version fails on the None entries and the trailing int of the 9-tuple -- they pass through here."""
+        reference's version fails on the None entries and the trailing int of the 9-tuple -- they pass through here.
+        Views of the fused cache (KiviPast, every layer, one cache at its current length) stay on the fused path: the cache
+        reorders its rows on the device (KiviCache.reorder) and fresh views are returned."""
+        if past_key_values and all(isinstance(p, KiviPast) for p in past_key_values):
+            cache = past_key_values[0].cache
+            if all(p.cache is cache and p.kv_len == cache.kv_len for p in past_key_values):
+                cache.reorder(beam_idx)
+                return tuple(KiviPast(cache, p.layer, cache.kv_len) for p in past_key_values)
         return tuple(tuple(t.index_select(0, beam_idx.to(t.device)) if torch.is_tensor(t) else t for t in layer_past)
                      for layer_past in past_key_values)
 
@@ -727,7 +736,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 from . import dist as kdist
                 self._allreduce = None
                 self._allreduce = kdist.PeerAllReduce(batch, cfg.hidden_size, dev)
-        self._graph, self._graph_ragged = None, False
+        self._graph, self._graph_ragged, self._reorder_graph = None, False, None
         self._pos = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._ids = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._logits = torch.zeros((batch, cfg.vocab_size), dtype=torch.float32, device=dev)
@@ -767,9 +776,15 @@ class LlamaForCausalLM_KIVI(nn.Module):
         assert self.cache is not None, "call init_cache() first"
         return self.lm_head(self._prompt_pass(input_ids, attention_mask)[:, -1]).float()
 
-    def _prompt_pass(self, input_ids, attention_mask=None):
-        """prefill() up to the final norm: the hidden states [B, n, hidden] of every position."""
+    def _prompt_pass(self, input_ids, attention_mask=None, copies: int = 1):
+        """prefill() up to the final norm: the hidden states [B, n, hidden] of every position.  copies = K: the layers run
+        on the B prompts once and the cache's rows b * K .. b * K + K - 1 (the beams or samples of prompt b) each receive
+        prompt b's K / V, starts and positions."""
         B, n = input_ids.shape
+        store = self.cache.prefill
+        if copies > 1:
+            def store(layer, k, v):
+                self.cache.prefill(layer, k.repeat_interleave(copies, 0), v.repeat_interleave(copies, 0))
         starts = None
         if attention_mask is not None:
             starts = kv_start_from_mask(attention_mask)
@@ -778,16 +793,16 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
             mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window, B)
-            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=self.cache.prefill)
+            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store)
             self._pos.fill_(n)
         else:
             am = attention_mask.to(input_ids.device)
             positions = am.long().cumsum(-1) - 1                            # prepare_inputs_for_generation (:908-948)
             positions.masked_fill_(am == 0, 1)
             mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window)
-            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=self.cache.prefill)
-            starts = starts.to(self._pos.device)
-            self._pos.copy_((n - starts).to(torch.long).view(B, 1))
+            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store)
+            starts = starts.to(self._pos.device).repeat_interleave(copies)
+            self._pos.copy_((n - starts).to(torch.long).view(B * copies, 1))
             self.cache.set_kv_start(starts)
         return h
 
@@ -1091,7 +1106,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
     @torch.no_grad()
     def generate(self, input_ids=None, max_new_tokens: int | None = None, use_graph: bool = True, attention_mask=None,
                  max_length: int | None = None, do_sample: bool = False, temperature=1.0, top_k=50, top_p=1.0, seed=0,
-                 **unused):
+                 num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False,
+                 eos_token_id=None, pad_token_id=None, return_dict_in_generate: bool = False, **unused):
         """Decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
         max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Greedy by default;
         do_sample=True samples every token, the first included, on the device with temperature / top_k / top_p (HF's
@@ -1101,7 +1117,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
         (prefill(); the decode steps skip each sequence's padding); right padding raises ValueError.
         A model with a sliding window W rolls its cache: it holds about max(prompt, W) + 2 max(128, R) positions, and
         before a step that would not fit, the positions that fell out of every window are dropped (KiviCache.shift), so
-        the generated length is bounded by the RoPE tables rather than by cache memory."""
+        the generated length is bounded by the RoPE tables rather than by cache memory.
+        num_beams > 1 or num_return_sequences > 1: several sequences per prompt, see _generate_many; the other arguments
+        of that mode (length_penalty, early_stopping, eos_token_id, pad_token_id, return_dict_in_generate) are read there
+        only."""
+        if num_beams != 1 or num_return_sequences != 1:
+            return self._generate_many(input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample,
+                                       temperature, top_k, top_p, seed, num_beams, num_return_sequences, length_penalty,
+                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate)
         if do_sample:
             sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
         if attention_mask is not None:
@@ -1133,6 +1156,122 @@ class LlamaForCausalLM_KIVI(nn.Module):
             tok = self.next_tokens.view(B, 1).clone()
         out.append(tok)
         return torch.cat(out, dim=1)
+
+    def _generate_many(self, input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample, temperature,
+                       top_k, top_p, seed, num_beams, num_return_sequences, length_penalty, early_stopping, eos_token_id,
+                       pad_token_id, return_dict_in_generate):
+        """generate() with K = num_beams (beam search, kivi_b200.beam) or K = num_return_sequences (do_sample) sequences per
+        prompt, in the cache's rows b * K .. b * K + K - 1.  The prompt pass runs once per prompt and its K / V fill the K
+        rows (_prompt_pass(copies=K)).
+        Beam search (transformers' _beam_search semantics: length_penalty, early_stopping True / False / "never",
+        num_return_sequences <= num_beams, EOS = eos_token_id or config.eos_token_id, finished sequences padded with
+        pad_token_id, default the EOS): every step replays the decode-step graph, selects the beams on its logits, reads the
+        chosen rows and tokens back in one copy, and replays a second graph that reorders the cache's rows
+        (KiviCache._enqueue_reorder: launches_per_reorder launches) and their positions.  Returns [B * n, length] ids, or
+        with return_dict_in_generate an object with `sequences` and `sequences_scores`.
+        do_sample: row b * n + j samples from the Philox key seed + b * n + j (set_sampling over the B * n rows), its first
+        token from prompt b's logits.  Returns [B * n, prompt + new] ids.
+        Refused before any work: beam sampling (NotImplementedError), num_return_sequences > num_beams and several greedy
+        sequences per prompt (ValueError), beams with enable_token_allgather replicas (NotImplementedError)."""
+        beams = num_beams > 1
+        if num_beams < 1 or num_return_sequences < 1:
+            raise ValueError(f"num_beams ({num_beams}) and num_return_sequences ({num_return_sequences}) must be >= 1")
+        if beams and do_sample:
+            raise NotImplementedError("beam sampling (num_beams > 1 with do_sample=True) is not supported")
+        if beams and num_return_sequences > num_beams:
+            raise ValueError(f"num_return_sequences ({num_return_sequences}) must not exceed num_beams ({num_beams})")
+        if not beams and not do_sample:
+            raise ValueError(f"greedy decoding returns one sequence per prompt, num_return_sequences is "
+                             f"{num_return_sequences}: use do_sample=True or num_beams >= num_return_sequences")
+        if beams and early_stopping not in (True, False, "never"):
+            raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
+        if beams and (self._exchange is not None or self._dist_tokens is not None):
+            raise NotImplementedError("beam search with enable_token_allgather data-parallel replicas is not supported")
+        K = num_beams if beams else num_return_sequences
+        B, n = input_ids.shape
+        rows = B * K
+        if do_sample:
+            sampling_rows(rows, temperature, top_k, top_p, seed)                # ValueError before any work
+        if attention_mask is not None:
+            kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
+        if max_new_tokens is None:
+            if max_length is None:
+                raise ValueError("generate() needs max_new_tokens or max_length")
+            max_new_tokens = max_length - n
+        cap = n + max_new_tokens
+        if self.sliding_window is not None:
+            cap = min(cap, max(n, self.sliding_window) + 2 * max(128, self.config.residual_length))
+        if self.cache is None or self.cache.batch != rows or self.cache.max_tokens < cap:
+            self.init_cache(rows, cap)
+        self._tables(self.cache.device, n + max_new_tokens)
+        if do_sample:
+            self.set_sampling(temperature, top_k, top_p, seed)
+        else:
+            self.set_sampling(None)
+        logits = self.lm_head(self._prompt_pass(input_ids, attention_mask, copies=K)[:, -1]).float()    # [B, vocab]
+        if do_sample:
+            out = [input_ids.repeat_interleave(K, 0)]
+            tok = self.sample_first(logits.repeat_interleave(K, 0)).view(rows, 1)
+            for _ in range(max_new_tokens - 1):
+                out.append(tok)
+                if self.cache.kv_len + 1 > self.cache.max_tokens:
+                    self._roll()
+                self.decode_step(tok, use_graph=use_graph)
+                tok = self.next_tokens.view(rows, 1).clone()
+            out.append(tok)
+            seq, scores = torch.cat(out, dim=1), None
+        else:
+            from .beam import BeamSearch
+            if eos_token_id is None:
+                eos_token_id = getattr(self.config, "eos_token_id", None)
+            search = BeamSearch(input_ids, K, n + max_new_tokens, eos_token_id, pad_token_id, length_penalty,
+                                early_stopping, num_return_sequences)
+            self.cache.reorder_scratch()
+            first = True
+            while True:
+                beam_idx, tok, done = search.step(logits)
+                host = torch.cat([beam_idx, done.view(1).long()]).tolist()   # the one device-to-host read of a step
+                if host[-1]:
+                    break
+                self._ids.copy_(tok.view(rows, 1))
+                if not first:        # after the prompt pass the K rows of a prompt hold the same bytes: nothing to copy
+                    self._reorder_rows(beam_idx, host[:-1], use_graph)
+                first = False
+                if self.cache.kv_len + 1 > self.cache.max_tokens:
+                    self._roll()
+                logits = self.decode_step(use_graph=use_graph)
+            seq, scores = search.finalize()
+        if not return_dict_in_generate:
+            return seq
+        from transformers.generation.utils import GenerateBeamDecoderOnlyOutput, GenerateDecoderOnlyOutput
+        if scores is None:
+            return GenerateDecoderOnlyOutput(sequences=seq)
+        return GenerateBeamDecoderOnlyOutput(sequences=seq, sequences_scores=scores)
+
+    def _reorder_rows(self, beam_idx, rows, use_graph: bool = True):
+        """Row r of the cache and of the positions becomes a copy of row beam_idx[r] (device [B], any integer dtype; `rows`:
+        the same map on the host).  The copy (KiviCache._enqueue_reorder, reading cache.reorder_src) and the position gather
+        are captured once in a CUDA graph: the first call runs them eagerly, which also loads the kernels, then captures."""
+        c = self.cache
+        c.reorder_src.copy_(beam_idx)
+
+        def body():
+            c._enqueue_reorder()
+            self._pos.copy_(self._pos.index_select(0, c.reorder_src))
+        if not use_graph:
+            body()
+        elif self._reorder_graph is not None and self._reorder_graph[1] == c.ragged:
+            self._reorder_graph[0].replay()
+        else:
+            body()
+            from . import _lib
+            n0 = _lib.launch_count()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                body()
+            self.launches_per_reorder = _lib.launch_count() - n0
+            self._reorder_graph = (g, c.ragged)
+        c._mirror_reorder(rows)
 
 
 MistralForCausalLM_KIVI = LlamaForCausalLM_KIVI       # models/mistral_kivi.py:921 -- same hook; GQA is handled in-kernel
