@@ -363,6 +363,28 @@ int kivi_rope_split_f16(const void* qkv, const void* cos_table, const void* sin_
                         void* stream);
 int kivi_silu_mul_f16(const void* gate_up, void* out, int rows, int intermediate, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Prompt attention: the attention of a prompt over itself, in the prompt pass (not over the cache).
+ *   q [B, H, n, 128], k / v [B, Hkv, n, 128] fp16 with a contiguous head dimension and element strides
+ *     q_sb / q_sh / q_st (batch, head, token) and kv_sb / kv_sh / kv_st (shared by k and v): the strided views of
+ *     the q / k / v projections.  K after RoPE.
+ *   out [B, n, H, 128] fp16 contiguous (the layout o_proj reads).
+ * Query head h reads KV head h / (H / Hkv); K and V are never expanded.  Query i of sequence b sees the keys
+ *   lo <= j <= i,   lo = max(s_b, window > 0 ? i - window + 1 : 0),   s_b = clamp(kv_start[b], 0, n)
+ * (kv_start NULL = 0; transformers' kv_idx > q_idx - window).  A query with no visible key (i < s_b) gets zeros.
+ * Scale 1/sqrt(128); logits and the softmax in fp32 with a running maximum and sum; P rounded to fp16 for the P.V
+ * product; fp32 accumulators.  Offsets are 64-bit.  Key tiles with no visible key for any query of a tile are not read,
+ * so the work and the K / V bytes follow the visible pairs.
+ * Requirements: q, k, v, out non-NULL and 16-byte aligned, every stride a multiple of 8 elements, kv_start 4-byte
+ * aligned; batch in [1, 65535], num_heads >= 1, n >= 1, window >= 0 (KIVI_ERR_SHAPE), num_heads % num_kv_heads == 0
+ * (KIVI_ERR_GQA).  One launch, no allocation, no synchronisation; CUDA-graph capturable.
+ * ------------------------------------------------------------------------------------------ */
+int kivi_prompt_attention_f16(const void* q, const void* k, const void* v, void* out,
+                              int batch, int num_heads, int num_kv_heads, int n,
+                              int64_t q_sb, int64_t q_sh, int64_t q_st,
+                              int64_t kv_sb, int64_t kv_sh, int64_t kv_st,
+                              const int32_t* kv_start, int window, void* stream);
+
 /* Greedy sampling fused with its collective (the only exchange of the data-parallel decode, SURVEY 8e; the reference has
  * none).  next_local[b] = argmax_v logits[b, v] (first index among equal maxima, as torch.argmax; logits fp32 [batch, vocab],
  * models/llama_kivi.py:881); ids_feedback (may be NULL) receives the same ids (the next step's input buffer).

@@ -48,6 +48,8 @@ inline int ensure_dynamic_smem(F kernel, int bytes, int ordinal, std::atomic<uns
 struct Tuning { int gqa_g, ctas_per_sm, stages_per_warp, no_pdl, no_mma_gemv; };
 const Tuning& tuning();
 
+inline bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
+
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -597,8 +597,6 @@ allreduce_add_rmsnorm_kernel(const __half* const* __restrict__ peer, __half* __r
 
 using namespace kivi;
 
-static bool aligned_to(const void* p, uintptr_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
-
 // the checks both residual-add + RMSNorm entry points begin with
 static int check_rmsnorm_args(const void* residual, const void* weight, const void* out, int rows, int hidden)
 {

@@ -1,5 +1,6 @@
 """ctypes wrappers of the decode-step glue kernels (csrc/kivi_model.cu): residual-add + RMSNorm,
-RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), greedy and sampled next-token selection (fp32 logits); each wrapper checks device, dtype, contiguity and shapes
+RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), greedy and sampled next-token selection (fp32 logits), and of the prompt
+pass's attention (csrc/kivi_prompt.cu); each wrapper checks device, dtype, contiguity and shapes
 before the call (ValueError, or RuntimeError for a CPU tensor)."""
 from __future__ import annotations
 
@@ -24,6 +25,8 @@ def _bind():
     _lib.bind("kivi_sample_f32", i32, [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
     _lib.bind("kivi_allreduce_add_rmsnorm_f16", i32,
               [vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, i32, i32, i32, i32, vp, vp, i32, vp])
+    i64 = ctypes.c_int64
+    _lib.bind("kivi_prompt_attention_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32] + [i64] * 6 + [vp, i32, vp])
     _B = True
 
 
@@ -157,3 +160,38 @@ def sample(logits, temperature, top_k, top_p, seed, draw, next_local, ids_feedba
         next_local.data_ptr(), ptr(ids_feedback), ptr(dbg_u), ptr(dbg_kept), _lib.stream_ptr(logits.device)),
         "kivi_sample_f32")
     return next_local
+
+
+def prompt_attention(q, k, v, out, kv_start=None, window=None):
+    """Attention of a prompt over itself (kivi_prompt_attention_f16): q [B, H, n, 128], k / v [B, Hkv, n, 128] fp16 with
+    a contiguous head dimension -- the strided [B, heads, n, 128] views of the q / k / v projections -- and k, v of equal
+    strides; out [B, n, H, 128] fp16 contiguous.  Query i of sequence b sees the keys max(s_b, i - window + 1) <= j <= i
+    with s_b = kv_start[b] (int32 [B] on the device, clamped into [0, n]; None = 0) and window None or 0 = no window.
+    A query with no visible key gets zeros.  Returns out."""
+    _bind()
+    _lib.require_cuda(q, k, v, out, kv_start)
+    for name, t in (("q", q), ("k", k), ("v", v)):
+        if t.dtype != torch.float16:
+            raise ValueError(f"{name}: expected torch.float16, got {t.dtype}")
+        if t.dim() != 4 or t.shape[-1] != 128 or t.stride(-1) != 1:
+            raise ValueError(f"{name}: expected [B, heads, n, 128] with a contiguous last dimension, got shape "
+                             f"{tuple(t.shape)}, strides {t.stride()}")
+    B, H, n, _ = q.shape
+    Hkv = k.shape[1]
+    if k.shape != (B, Hkv, n, 128) or v.shape != k.shape:
+        raise ValueError(f"k, v: expected [{B}, Hkv, {n}, 128] each, got {tuple(k.shape)}, {tuple(v.shape)}")
+    # the stride of a dimension of size 1 is never used (its index is 0): 0, so that views differing there agree
+    q_str, k_str, v_str = ([0 if t.shape[i] == 1 else t.stride(i) for i in range(3)] for t in (q, k, v))
+    if v_str != k_str:
+        raise ValueError(f"k, v: expected equal strides, got {k.stride()}, {v.stride()}")
+    _check("out", out, torch.float16, (B, n, H, 128))
+    if kv_start is not None:
+        _check("kv_start", kv_start, torch.int32, (B,))
+    for name, t in (("k", k), ("v", v), ("out", out), ("kv_start", kv_start)):
+        if t is not None and t.device != q.device:
+            raise ValueError(f"{name}: on {t.device}, q on {q.device}")
+    _lib.check(_lib.lib().kivi_prompt_attention_f16(
+        q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, H, Hkv, n, *q_str, *k_str,
+        kv_start.data_ptr() if kv_start is not None else None, int(window or 0), _lib.stream_ptr(q.device)),
+        "kivi_prompt_attention_f16")
+    return out

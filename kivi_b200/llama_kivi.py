@@ -20,11 +20,13 @@ from __future__ import annotations
 
 import math
 from types import SimpleNamespace
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import glue
 from .cache import KiviCache, kv_start_from_mask
 from .matmul import cuda_bmm_fA_qB_outer
 from .new_pack import triton_quantize_and_pack_along_last_dim
@@ -235,6 +237,20 @@ def _rotate_half(x):
     return torch.cat((-x2, x1), dim=-1)
 
 
+# Rows of B * n that the per-token part of a prompt pass (norms, projections, RoPE, MLP) runs on at a time: a longer prompt
+# holds one chunk's [rows, intermediate] temporaries instead of the whole prompt's.  Every model-level prompt of the test
+# suite (B * n <= 1500) stays one chunk and runs the unchunked code.
+PROMPT_CHUNK_ROWS = 16384
+
+
+class PromptMask(NamedTuple):
+    """The mask of a prompt pass in the form kivi_prompt_attention_f16 takes it, in place of an additive [B, 1, n, n]
+    tensor: query i of sequence b sees the keys max(kv_start[b], i - window + 1) <= j <= i.  kv_start: int32 [B] on the
+    device, or None (no padding); window: 0 = none."""
+    kv_start: torch.Tensor | None
+    window: int
+
+
 class LlamaFlashAttention_KIVI(nn.Module):
     """Attention layer of the reference (models/llama_kivi.py:264-466), KIVI ops on libkivi_b200."""
 
@@ -264,35 +280,56 @@ class LlamaFlashAttention_KIVI(nn.Module):
         k = k * cos + _rotate_half(k) * sin
         return q, k, v
 
+    def _qkv_rows(self, x, cos, sin):
+        """_qkv on rows of tokens: x [rows, hidden], cos / sin [rows, 1, D] -> q [rows, H, D], k and v [rows, Hkv, D],
+        q and k rotated."""
+        rows = x.shape[0]
+        q = self.q_proj(x).view(rows, self.num_heads, self.head_dim)
+        k = self.k_proj(x).view(rows, self.num_key_value_heads, self.head_dim)
+        v = self.v_proj(x).view(rows, self.num_key_value_heads, self.head_dim)
+        return q * cos + _rotate_half(q) * sin, k * cos + _rotate_half(k) * sin, v
+
     def _prompt_attention(self, q, k, v, attention_mask):
-        """Attention over the prompt itself (the reference calls flash-attn here, models/llama_kivi.py:401-423; off the
-        decode hot path): causal, plus the additive mask [B, 1, q_len, q_len] when the batch is padded or a sliding window
-        cuts the prompt (_additive_mask; the mask takes q_len^2 elements per sequence)."""
+        """Attention over the prompt itself (the reference calls flash-attn here, models/llama_kivi.py:401-423) -> [B,
+        q_len, H * D].  A PromptMask (a left-padded batch or a sliding window that cuts the prompt, fp16 on CUDA) runs
+        kivi_prompt_attention_f16 on the strided q / k / v, with no mask tensor and no K / V copy per query head.
+        Otherwise SDPA: causal, plus an additive mask [B, 1, q_len, q_len] when one is given."""
+        B, H, n, D = q.shape
+        if isinstance(attention_mask, PromptMask):
+            out = torch.empty((B, n, H, D), dtype=q.dtype, device=q.device)
+            glue.prompt_attention(q, k, v, out, attention_mask.kv_start, attention_mask.window)
+            return out.view(B, n, H * D)
         kk, vv = repeat_kv(k, self.num_key_value_groups), repeat_kv(v, self.num_key_value_groups)
         if attention_mask is None:
-            return F.scaled_dot_product_attention(q, kk, vv, is_causal=True)
-        return F.scaled_dot_product_attention(q, kk, vv, attn_mask=attention_mask.to(q.dtype))
+            o = F.scaled_dot_product_attention(q, kk, vv, is_causal=True)
+        else:
+            o = F.scaled_dot_product_attention(q, kk, vv, attn_mask=attention_mask.to(q.dtype))
+        return o.transpose(1, 2).reshape(B, n, H * D)
+
+    def _prompt_core(self, q, k, v, attention_mask, store_kv):
+        """The prompt pass between the projections and o_proj: attention ([B, q_len, H * D]) and the 9-tuple, or
+        store_kv(layer, k, v) and None."""
+        attn_output = self._prompt_attention(q, k, v, attention_mask)
+        if store_kv is None:
+            return attn_output, kivi_prefill_tuple(k, v, self.group_size, self.k_bits, self.v_bits, self.residual_length)
+        store_kv(self.layer_idx, k, v)
+        return attn_output, None
 
     def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None):
         """hidden_states [B, q_len, hidden]; cos/sin broadcastable to [B, 1, q_len, D].
         past_key_value: None (a prompt pass, returns a 9-tuple) or the reference's 9-tuple (decode, returns the next one).
         store_kv: with a prompt pass, a callable store_kv(layer, k, v) that takes the rotated K and V [B, Hkv, q_len, D] in
         place of the 9-tuple (the fused cache: KiviCache.prefill, or a refill of one slot); the pass then returns None.
-        attention_mask: None or additive [B, 1, q_len, kv_len] (models/llama_kivi.py:364-372)."""
+        attention_mask: None or additive [B, 1, q_len, kv_len] (models/llama_kivi.py:364-372); in a prompt pass also a
+        PromptMask."""
         bsz, q_len, _ = hidden_states.shape
         q, k, v = self._qkv(hidden_states, cos, sin)
         if past_key_value is not None:                                      # reference 9-tuple, decode
             attn_output, past = kivi_decode_attention_tuple(q, k, v, past_key_value, self.group_size, self.k_bits,
                                                             self.v_bits, self.residual_length, attention_mask)
-            attn_output = attn_output.transpose(1, 2).contiguous()
+            attn_output = attn_output.transpose(1, 2).contiguous().reshape(bsz, q_len, self.num_heads * self.head_dim)
         else:                                                               # prompt (:401-455)
-            attn_output = self._prompt_attention(q, k, v, attention_mask).transpose(1, 2)
-            if store_kv is None:
-                past = kivi_prefill_tuple(k, v, self.group_size, self.k_bits, self.v_bits, self.residual_length)
-            else:
-                store_kv(self.layer_idx, k, v)
-                past = None
-        attn_output = attn_output.reshape(bsz, q_len, self.num_heads * self.head_dim)
+            attn_output, past = self._prompt_core(q, k, v, attention_mask, store_kv)
         return self.o_proj(attn_output), None, past
 
 
@@ -321,6 +358,8 @@ class LlamaDecoderLayer_KIVI(nn.Module):
         self.tp_world = tp_world
 
     def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None):
+        if past_key_value is None and hidden_states.shape[0] * hidden_states.shape[1] > PROMPT_CHUNK_ROWS:
+            return self._prompt_in_chunks(hidden_states, cos, sin, attention_mask, store_kv)
         residual = hidden_states
         h, _, past = self.self_attn(self.input_layernorm(hidden_states), cos, sin, past_key_value, attention_mask,
                                     store_kv)
@@ -332,6 +371,38 @@ class LlamaDecoderLayer_KIVI(nn.Module):
             h = sum_partials(h)
         hidden_states = hidden_states + h
         return hidden_states, past
+
+    def _prompt_in_chunks(self, x, cos, sin, attention_mask, store_kv):
+        """forward() of a prompt pass in bounded memory: the per-token work -- input norm, q|k|v, RoPE; after the
+        attention o_proj, the residual add, the post-attention norm, the MLP and its residual add -- runs on
+        PROMPT_CHUNK_ROWS rows of B * n at a time, the attention between the two halves on the whole prompt.  The layer
+        holds the residual stream, q, k, v, the attention output and one chunk's temporaries.  x [B, n, hidden] is the
+        residual stream, updated in place."""
+        a = self.self_attn
+        B, n, hidden = x.shape
+        rows, D = B * n, a.head_dim
+        flat = x.view(rows, hidden)
+        cos, sin = (t.expand(B, 1, n, D).reshape(rows, 1, D) for t in (cos, sin))
+        q = x.new_empty((rows, a.num_heads, D))
+        k = x.new_empty((rows, a.num_key_value_heads, D))
+        v = torch.empty_like(k)
+        chunks = [slice(lo, min(lo + PROMPT_CHUNK_ROWS, rows)) for lo in range(0, rows, PROMPT_CHUNK_ROWS)]
+        for c in chunks:
+            q[c], k[c], v[c] = a._qkv_rows(self.input_layernorm(flat[c]), cos[c], sin[c])
+        heads = lambda t: t.view(B, n, -1, D).transpose(1, 2)                # noqa: E731 ([B, heads, n, D], as _qkv)
+        attn, past = a._prompt_core(heads(q), heads(k), heads(v), attention_mask, store_kv)
+        del q, k, v
+        attn = attn.view(rows, -1)
+        for c in chunks:
+            h = a.o_proj(attn[c])
+            if self.tp_world > 1:
+                h = sum_partials(h)
+            r = flat[c] + h
+            h = self.mlp(self.post_attention_layernorm(r))
+            if self.tp_world > 1:
+                h = sum_partials(h)
+            flat[c] = r + h
+        return x, past
 
 
 class LlamaModel_KIVI(nn.Module):
@@ -598,7 +669,13 @@ class LlamaForCausalLM_KIVI(nn.Module):
         for i, layer in enumerate(self.model.layers):
             h, past = layer(h, cos, sin, pasts[i] if pasts is not None else None, attention_mask, store_kv)
             new_pasts.append(past)
-        h = self.model.norm(h)
+        rows = h.shape[0] * h.shape[1]
+        if rows > PROMPT_CHUNK_ROWS:                   # a long prompt: the norm's fp32 temporaries one chunk at a time
+            flat = h.view(rows, -1)
+            for lo in range(0, rows, PROMPT_CHUNK_ROWS):
+                flat[lo:lo + PROMPT_CHUNK_ROWS] = self.model.norm(flat[lo:lo + PROMPT_CHUNK_ROWS])
+        else:
+            h = self.model.norm(h)
         return h, new_pasts
 
     # ------------------------------------------------------------------ reference-style forward (9-tuples)
@@ -628,7 +705,11 @@ class LlamaForCausalLM_KIVI(nn.Module):
             if start + q_len > rows:            # the slow path's index_select would raise; say why
                 raise ValueError(f"{start + q_len} positions exceed config.max_position_embeddings = {rows}")
             dtype = self.lm_head.weight.dtype
-            mask = _additive_mask(attention_mask, q_len, start + q_len, dtype, input_ids.device, self.sliding_window, B)
+            mask = None
+            if past_key_values is None:                                   # the prompt: the kernel's mask where it applies
+                mask = self._tuple_prompt_mask(attention_mask, B, q_len, input_ids.device)
+            if mask is None:
+                mask = _additive_mask(attention_mask, q_len, start + q_len, dtype, input_ids.device, self.sliding_window, B)
             h, pasts = self._run_layers(input_ids, position_ids, past_key_values, mask)
             logits = self.lm_head(h).float()                                     # logits.float() (:881)
         if return_dict is None:
@@ -637,6 +718,34 @@ class LlamaForCausalLM_KIVI(nn.Module):
             from transformers.modeling_outputs import CausalLMOutputWithPast
             return CausalLMOutputWithPast(loss=None, logits=logits, past_key_values=tuple(pasts))
         return _Output((logits, pasts))
+
+    def _kernel_mask(self, starts, n: int, device):
+        """The PromptMask of a prompt at positions 0 .. n-1 whose sequences start at `starts` (int32 [B] on `device`, or
+        None: no padding), or None where the prompt-attention kernel does not apply: weights other than fp16 on CUDA, a
+        head_dim other than 128, or nothing to mask (no padding, and no sliding window shorter than the prompt).  The
+        masks the model would otherwise build with _additive_mask -- left padding, a window that cuts the prompt, or
+        both -- are exactly these."""
+        cut = self.sliding_window is not None and n > self.sliding_window
+        if (device.type != "cuda" or self.lm_head.weight.dtype != torch.float16
+                or self.model.layers[0].self_attn.head_dim != 128 or (starts is None and not cut)):
+            return None
+        return PromptMask(None if starts is None else starts.to(device), self.sliding_window if cut else 0)
+
+    def _tuple_prompt_mask(self, attention_mask, B: int, n: int, device):
+        """The PromptMask of forward()'s prompt on the 9-tuple path, or None to keep the additive mask.  Only masks the
+        kernel's rule states exactly go to it: no mask, an all-ones [B, n] mask, or a left-padding [B, n] mask (then with
+        the sequences' starts) -- each with the window when it cuts the prompt.  A 4-D mask, a 2-D mask that is not left
+        padding (right padding, holes, a row with no real token) or of another shape keeps _additive_mask, which applies
+        it as given together with the window."""
+        if attention_mask is None:
+            return self._kernel_mask(None, n, device)
+        if attention_mask.dim() != 2 or tuple(attention_mask.shape) != (B, n):
+            return None
+        try:
+            starts = kv_start_from_mask(attention_mask)
+        except ValueError:
+            return None
+        return self._kernel_mask(starts if bool(starts.any()) else None, n, device)
 
     # ------------------------------------------------------------------ forward() on the fused cache path
     fused_forward = True        # False: forward() always uses the reference's own 9-tuples (torch.cat growth, per-op launches)
@@ -770,7 +879,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
     def prefill(self, input_ids, attention_mask=None):
         """Run the prompt, fill the cache (models/llama_kivi.py:401-452), return last-position logits.
         attention_mask: None or an HF padding mask [B, n] of a LEFT-padded batch (ValueError otherwise).  The prompt
-        attention then takes the additive mask of the tuple path, positions follow HF (cumsum - 1, pad positions 1), and
+        attention then skips each sequence's padding (kivi_prompt_attention_f16 with the sequences' starts; the additive
+        mask of the tuple path for weights other than fp16), positions follow HF (cumsum - 1, pad positions 1), and
         the decode steps skip each sequence's padding (KiviCache.set_kv_start).  An all-ones mask is no mask.  Every
         prompt, a one-token one included, replaces what the cache held."""
         assert self.cache is not None, "call init_cache() first"
@@ -792,14 +902,18 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 starts = None
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
-            mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window, B)
+            mask = self._kernel_mask(None, n, input_ids.device)
+            if mask is None:
+                mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window, B)
             h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store)
             self._pos.fill_(n)
         else:
             am = attention_mask.to(input_ids.device)
             positions = am.long().cumsum(-1) - 1                            # prepare_inputs_for_generation (:908-948)
             positions.masked_fill_(am == 0, 1)
-            mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window)
+            mask = self._kernel_mask(starts, n, input_ids.device)
+            if mask is None:
+                mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window)
             h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store)
             starts = starts.to(self._pos.device).repeat_interleave(copies)
             self._pos.copy_((n - starts).to(torch.long).view(B * copies, 1))
@@ -818,7 +932,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if not 1 <= n <= T:
             raise ValueError(f"a prompt of {n} tokens does not fit the shared length {T} (1 <= n <= length)")
         positions = torch.arange(n, device=ids.device).unsqueeze(0)
-        mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, ids.device, self.sliding_window)
+        mask = self._kernel_mask(None, n, ids.device)
+        if mask is None:
+            mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, ids.device, self.sliding_window)
         h, _ = self._run_layers(ids, positions, None, mask,
                                 store_kv=lambda layer, k, v: self.cache.refill(layer, seq, k, v))
         self._pos[seq] = n
