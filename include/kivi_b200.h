@@ -426,6 +426,40 @@ int kivi_sample_f32(const void* logits, int batch, int vocab, const float* tempe
                     const uint64_t* seed, uint64_t* draw, void* next_local, void* ids_feedback, float* dbg_u, int32_t* dbg_kept,
                     void* stream);
 
+/* Logits processing: scores = the logits after repetition, presence and frequency penalties, EOS suppression below a
+ * minimum length and the masking of finished rows, for the greedy kernel or kivi_sample_f32 to choose from.  logits and
+ * scores are fp32 [batch, vocab], distinct buffers; logits is only read.  Per-row state and parameters are DEVICE arrays, read
+ * by the kernel, so a captured call follows later changes:
+ *   counts   int32 [batch, vocab]       how many times each token was generated (kivi_logits_record)
+ *   seen     uint32 [batch, ceil(vocab / 32)]   the prompt's tokens, bit v & 31 of word v >> 5
+ *   n_new    int32 [batch], finished uint8 [batch]   (kivi_logits_record)
+ *   repetition, presence, frequency   fp32 [batch];  min_new int32 [batch]
+ *   eos_ids  int64 [n_eos], 0 <= n_eos <= 8 (may be NULL when n_eos = 0); ids outside [0, vocab) match no token
+ * For each token v of row b, with x = logits[b, v], c = counts[b, v], in this order, every step one IEEE fp32 operation
+ * rounded to nearest (no contraction):
+ *   1. repetition (transformers' RepetitionPenaltyLogitsProcessor): if v is in seen or c > 0:  x = x < 0 ? x * p : x / p
+ *   2. frequency, then presence (vLLM's order, generated tokens only):  x = x - f * float(c);  if c > 0: x = x - pres
+ *   3. if n_new[b] < min_new[b]: x = -inf for every v in eos_ids (MinLength / MinNewTokensLength LogitsProcessor)
+ *   4. if finished[b]: x = 0 at v = pad_id, -inf everywhere else (the rule of the `unfinished` mask of HF's greedy and
+ *      sampling loops: both selection kernels then pick pad_id -- the greedy one as the only maximum, the sampler as
+ *      the one finite token, which it keeps whatever its top-k and top-p; it consumes a draw like any sampled row)
+ * A row with p == 1 and presence, frequency +0 skips steps 1-2 and reads neither counts nor seen (its scores equal its logits
+ * bit for bit, NaN payloads included); a finished row reads nothing but its flag.  Parameter VALUES are the caller's
+ * responsibility (kivi_b200's processing_rows validates them on the host).
+ * Requirements: 0 <= batch <= 65535, vocab >= 1, 0 <= pad_id < vocab, seen 4-byte aligned; 128-bit accesses when vocab % 4 == 0
+ * and logits / scores / counts are 16-byte aligned.  Argument errors return KIVI_ERR_* before any launch.  One launch,
+ * graph-capturable. */
+int kivi_logits_process_f32(const void* logits, void* scores, int batch, int vocab, const int32_t* counts, const uint32_t* seen,
+                            const int32_t* n_new, const uint8_t* finished, const float* repetition, const float* presence,
+                            const float* frequency, const int32_t* min_new, const int64_t* eos_ids, int n_eos, int64_t pad_id,
+                            void* stream);
+
+/* The state update after the token choice: t = tokens[b] (int64 [batch], e.g. next_local of the selection kernel):
+ * counts[b, t] += 1 (t in [0, vocab)), n_new[b] += 1, finished[b] = 1 if t is one of eos_ids[0 .. n_eos).  One thread per row;
+ * the same state layout and requirements as kivi_logits_process_f32 (batch >= 0).  One launch, graph-capturable. */
+int kivi_logits_record(const void* tokens, int batch, int vocab, int32_t* counts, int32_t* n_new, uint8_t* finished,
+                       const int64_t* eos_ids, int n_eos, void* stream);
+
 /* Tensor-parallel residual-add + RMSNorm: the all-reduce after o_proj / down_proj fused into the norm that follows it.
  * With the rows of the attention heads and of the MLP columns sharded over `world` ranks, rank p holds a partial sum
  * partial_p [rows, hidden] fp16 of the projection.  Every rank computes the same bits:

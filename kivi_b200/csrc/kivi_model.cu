@@ -532,6 +532,91 @@ sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
+// Logits processing between lm_head and the token choice, contract in include/kivi_b200.h (kivi_logits_process_f32).
+// logits_process_kernel: an element-wise pass, 4 tokens per thread (one 128-bit load of logits and of counts when the
+// rows are 16-byte aligned, VEC), grid (chunks of the row, rows), so one row already fills the GPU.  The 4 tokens of a
+// thread lie in one 32-bit word of the prompt bits.  A row whose penalties are neutral reads neither counts nor bits;
+// a finished row reads nothing but its flag.  Every operation is an IEEE fp32 operation with round-to-nearest and no
+// contraction, so a torch restatement of the same sequence gives the same bits.
+// logits_record_kernel: one thread per row, after the token choice.
+// ------------------------------------------------------------------------------------------------
+constexpr int kProcThreads = 128, kProcMaxEos = 8;
+
+template <bool VEC>
+__global__ void __launch_bounds__(kProcThreads)
+logits_process_kernel(const float* __restrict__ logits, float* __restrict__ scores, int V, const int* __restrict__ counts,
+                      const uint32_t* __restrict__ seen, int words, const int* __restrict__ n_new,
+                      const uint8_t* __restrict__ finished, const float* __restrict__ repetition,
+                      const float* __restrict__ presence, const float* __restrict__ frequency,
+                      const int* __restrict__ min_new, const long long* __restrict__ eos, int n_eos, long long pad)
+{
+    const int b = blockIdx.y;
+    const int v0 = (blockIdx.x * kProcThreads + threadIdx.x) * 4;
+    if (v0 >= V) return;
+    const long long off = (long long)b * V + v0;
+    float x[4];
+    if (finished[b]) {                                                   // only the pad id stays finite: it is chosen
+        #pragma unroll
+        for (int e = 0; e < 4; ++e) x[e] = v0 + e == pad ? 0.f : -INFINITY;
+    } else {
+        if (VEC) {
+            const float4 l = *reinterpret_cast<const float4*>(logits + off);
+            x[0] = l.x; x[1] = l.y; x[2] = l.z; x[3] = l.w;
+        } else {
+            #pragma unroll
+            for (int e = 0; e < 4; ++e) x[e] = v0 + e < V ? logits[off + e] : 0.f;
+        }
+        const float p = repetition[b], pr = presence[b], f = frequency[b];
+        // neutral: p == 1 and both penalties +0 (a -0 frequency is not neutral: x - (-0 * 0) turns -0 into +0)
+        if (p != 1.f || __float_as_uint(pr) != 0u || __float_as_uint(f) != 0u) {
+            int c[4];
+            if (VEC) {
+                const int4 ci = *reinterpret_cast<const int4*>(counts + off);
+                c[0] = ci.x; c[1] = ci.y; c[2] = ci.z; c[3] = ci.w;
+            } else {
+                #pragma unroll
+                for (int e = 0; e < 4; ++e) c[e] = v0 + e < V ? counts[off + e] : 0;
+            }
+            const uint32_t bits = seen[(long long)b * words + (v0 >> 5)] >> (v0 & 31);
+            #pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float y = x[e];
+                if (((bits >> e) & 1u) || c[e] > 0) y = y < 0.f ? __fmul_rn(y, p) : __fdiv_rn(y, p);
+                y = __fsub_rn(y, __fmul_rn(f, (float)c[e]));
+                if (c[e] > 0) y = __fsub_rn(y, pr);
+                x[e] = y;
+            }
+        }
+        if (n_new[b] < min_new[b]) {
+            for (int k = 0; k < n_eos; ++k) {
+                const long long d = eos[k] - v0;
+                if (d >= 0 && d < 4) x[d] = -INFINITY;
+            }
+        }
+    }
+    if (VEC) {
+        *reinterpret_cast<float4*>(scores + off) = make_float4(x[0], x[1], x[2], x[3]);
+    } else {
+        #pragma unroll
+        for (int e = 0; e < 4; ++e) if (v0 + e < V) scores[off + e] = x[e];
+    }
+}
+
+__global__ void __launch_bounds__(kProcThreads)
+logits_record_kernel(const long long* __restrict__ tokens, int B, int V, int* __restrict__ counts, int* __restrict__ n_new,
+                     uint8_t* __restrict__ finished, const long long* __restrict__ eos, int n_eos)
+{
+    const int b = blockIdx.x * kProcThreads + threadIdx.x;
+    if (b >= B) return;
+    const long long t = tokens[b];
+    if (t >= 0 && t < V) counts[(long long)b * V + t] += 1;
+    n_new[b] += 1;
+    bool stop = false;
+    for (int k = 0; k < n_eos; ++k) stop |= eos[k] == t;
+    if (stop) finished[b] = 1;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Tensor-parallel residual-add + RMSNorm: the all-reduce of the o_proj / down_proj partial sums fused into the norm that
 // consumes them.  Every rank reads the `world` partials of this call straight from the peers' symmetric buffers (layout in
 // include/kivi_b200.h), sums them in fp32 in rank order, rounds to fp16 and runs add_rmsnorm_row on that addend, the body of
@@ -681,6 +766,41 @@ extern "C" int kivi_sample_f32(const void* logits, int batch, int vocab, const f
     kernel<<<batch, kSampleThreads, staged ? row_bytes : 0, (cudaStream_t)stream>>>(
         (const float*)logits, vocab, temperature, top_k, top_p, (const unsigned long long*)seed, (unsigned long long*)draw,
         (long long*)next_local, (long long*)ids_feedback, dbg_u, dbg_kept);
+    return post_launch();
+}
+
+extern "C" int kivi_logits_process_f32(const void* logits, void* scores, int batch, int vocab, const int32_t* counts,
+                                       const uint32_t* seen, const int32_t* n_new, const uint8_t* finished,
+                                       const float* repetition, const float* presence, const float* frequency,
+                                       const int32_t* min_new, const int64_t* eos_ids, int n_eos, int64_t pad_id,
+                                       void* stream)
+{
+    if (!logits || !scores || !counts || !seen || !n_new || !finished || !repetition || !presence || !frequency || !min_new)
+        return KIVI_ERR_NULL;
+    if (n_eos > 0 && !eos_ids) return KIVI_ERR_NULL;
+    if (batch < 0 || batch > 65535 || vocab < 1 || n_eos < 0 || n_eos > kProcMaxEos || pad_id < 0 || pad_id >= vocab)
+        return KIVI_ERR_SHAPE;
+    if (!aligned_to(seen, 4)) return KIVI_ERR_ALIGN;
+    if (batch == 0) return KIVI_OK;
+    // 128-bit accesses when every row starts on a 16-byte boundary
+    const bool vec = vocab % 4 == 0 && aligned_to(logits, 16) && aligned_to(scores, 16) && aligned_to(counts, 16);
+    const dim3 grid(cdiv(cdiv(vocab, 4), kProcThreads), batch);
+    auto kernel = vec ? logits_process_kernel<true> : logits_process_kernel<false>;
+    kernel<<<grid, kProcThreads, 0, (cudaStream_t)stream>>>(
+        (const float*)logits, (float*)scores, vocab, counts, seen, cdiv(vocab, 32), n_new, finished, repetition, presence,
+        frequency, min_new, (const long long*)eos_ids, n_eos, (long long)pad_id);
+    return post_launch();
+}
+
+extern "C" int kivi_logits_record(const void* tokens, int batch, int vocab, int32_t* counts, int32_t* n_new,
+                                  uint8_t* finished, const int64_t* eos_ids, int n_eos, void* stream)
+{
+    if (!tokens || !counts || !n_new || !finished) return KIVI_ERR_NULL;
+    if (n_eos > 0 && !eos_ids) return KIVI_ERR_NULL;
+    if (batch < 0 || vocab < 1 || n_eos < 0 || n_eos > kProcMaxEos) return KIVI_ERR_SHAPE;
+    if (batch == 0) return KIVI_OK;
+    logits_record_kernel<<<cdiv(batch, kProcThreads), kProcThreads, 0, (cudaStream_t)stream>>>(
+        (const long long*)tokens, batch, vocab, counts, n_new, finished, (const long long*)eos_ids, n_eos);
     return post_launch();
 }
 

@@ -1,5 +1,6 @@
 """ctypes wrappers of the decode-step glue kernels (csrc/kivi_model.cu): residual-add + RMSNorm,
-RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), greedy and sampled next-token selection (fp32 logits), and of the prompt
+RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), logits processing and greedy and sampled next-token selection (fp32
+logits), and of the prompt
 pass's attention (csrc/kivi_prompt.cu); each wrapper checks device, dtype, contiguity and shapes
 before the call (ValueError, or RuntimeError for a CPU tensor)."""
 from __future__ import annotations
@@ -26,6 +27,8 @@ def _bind():
     _lib.bind("kivi_allreduce_add_rmsnorm_f16", i32,
               [vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, i32, i32, i32, i32, vp, vp, i32, vp])
     i64 = ctypes.c_int64
+    _lib.bind("kivi_logits_process_f32", i32, [vp, vp, i32, i32] + [vp] * 9 + [i32, i64, vp])
+    _lib.bind("kivi_logits_record", i32, [vp, i32, i32, vp, vp, vp, vp, i32, vp])
     _lib.bind("kivi_prompt_attention_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32] + [i64] * 6 + [vp, i32, vp])
     _B = True
 
@@ -160,6 +163,69 @@ def sample(logits, temperature, top_k, top_p, seed, draw, next_local, ids_feedba
         next_local.data_ptr(), ptr(ids_feedback), ptr(dbg_u), ptr(dbg_kept), _lib.stream_ptr(logits.device)),
         "kivi_sample_f32")
     return next_local
+
+
+def _check_state(B, V, device, counts, n_new, finished, eos, seen=None):
+    """The per-row processing state of B rows of a vocabulary of V tokens, on `device`; returns the number of EOS ids."""
+    for name, t, dtype, shape in (("counts", counts, torch.int32, (B, V)), ("n_new", n_new, torch.int32, (B,)),
+                                  ("finished", finished, torch.uint8, (B,)),
+                                  ("seen", seen, torch.int32, (B, (V + 31) // 32))):
+        if t is not None:
+            _check(name, t, dtype, shape)
+            if t.device != device:
+                raise ValueError(f"{name}: on {t.device}, expected {device}")
+    if eos is None:
+        return 0
+    if eos.dim() != 1 or eos.numel() > 8:
+        raise ValueError(f"eos: expected at most 8 ids in a 1-D tensor, got shape {tuple(eos.shape)}")
+    _check("eos", eos, torch.int64, eos.shape)
+    if eos.device != device:
+        raise ValueError(f"eos: on {eos.device}, expected {device}")
+    return eos.numel()
+
+
+def logits_process(logits, scores, counts, seen, n_new, finished, repetition, presence, frequency, min_new, eos, pad_id: int):
+    """scores = logits (fp32 [B, vocab]) after the repetition penalty over the prompt bits `seen` (int32 [B, ceil(vocab / 32)]
+    holding the uint32 words) and the generated `counts` (int32 [B, vocab]), the frequency and presence penalties, EOS
+    suppression while n_new[b] < min_new[b], and the masking of `finished` rows to pad_id; include/kivi_b200.h
+    (kivi_logits_process_f32) has the exact rules.  repetition / presence / frequency fp32 [B], min_new / n_new int32 [B],
+    finished uint8 [B], eos int64 [<= 8] or None.  The kernel reads every state and parameter on the device, so a captured
+    call follows later changes; the parameter VALUES are checked on the host by llama_kivi.processing_rows."""
+    _bind()
+    if logits.dim() != 2:
+        raise ValueError(f"logits: expected [B, vocab], got shape {tuple(logits.shape)}")
+    B, V = logits.shape
+    _check("logits", logits, torch.float32, (B, V))
+    _check("scores", scores, torch.float32, (B, V))
+    if scores.data_ptr() == logits.data_ptr():
+        raise ValueError("scores: expected a buffer distinct from logits")
+    n_eos = _check_state(B, V, logits.device, counts, n_new, finished, eos, seen)
+    for name, t, dtype in (("repetition", repetition, torch.float32), ("presence", presence, torch.float32),
+                           ("frequency", frequency, torch.float32), ("min_new", min_new, torch.int32)):
+        _check(name, t, dtype, (B,))
+        if t.device != logits.device:
+            raise ValueError(f"{name}: on {t.device}, logits on {logits.device}")
+    if not 0 <= int(pad_id) < V:
+        raise ValueError(f"pad_id {pad_id} outside the vocabulary of {V}")
+    _lib.check(_lib.lib().kivi_logits_process_f32(
+        logits.data_ptr(), scores.data_ptr(), B, V, counts.data_ptr(), seen.data_ptr(), n_new.data_ptr(), finished.data_ptr(),
+        repetition.data_ptr(), presence.data_ptr(), frequency.data_ptr(), min_new.data_ptr(),
+        eos.data_ptr() if n_eos else None, n_eos, int(pad_id), _lib.stream_ptr(logits.device)), "kivi_logits_process_f32")
+    return scores
+
+
+def logits_record(tokens, counts, n_new, finished, eos):
+    """After the token choice: counts[b, tokens[b]] += 1, n_new[b] += 1, finished[b] = 1 when tokens[b] is one of `eos`
+    (int64 [<= 8] or None).  tokens int64 [B]; the state as in logits_process (kivi_logits_record)."""
+    _bind()
+    if counts.dim() != 2:
+        raise ValueError(f"counts: expected [B, vocab], got shape {tuple(counts.shape)}")
+    B, V = counts.shape
+    _check("tokens", tokens, torch.int64, (B,))
+    n_eos = _check_state(B, V, tokens.device, counts, n_new, finished, eos)
+    _lib.check(_lib.lib().kivi_logits_record(
+        tokens.data_ptr(), B, V, counts.data_ptr(), n_new.data_ptr(), finished.data_ptr(), eos.data_ptr() if n_eos else None,
+        n_eos, _lib.stream_ptr(tokens.device)), "kivi_logits_record")
 
 
 def prompt_attention(q, k, v, out, kv_start=None, window=None):

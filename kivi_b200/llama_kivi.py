@@ -530,6 +530,71 @@ def sampling_rows(n: int, temperature=1.0, top_k=50, top_p=1.0, seed=0):
     return t, k, p, sd
 
 
+PROCESSING_KEYS = ("repetition_penalty", "presence_penalty", "frequency_penalty", "min_new_tokens")
+
+
+def processing_rows(n: int, repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_new_tokens=0,
+                    eos_token_id=None, vocab: int | None = None):
+    """The logits-processing parameters of n batch rows as four lists (repetition, presence, frequency, min_new), from
+    scalars or length-n sequences, and the EOS ids as a list (an int, a sequence of at most 8, or None = []).
+    repetition_penalty > 0 and finite (1 = off), presence_penalty and frequency_penalty in [-2, 2] (0 = off),
+    min_new_tokens an int >= 0, EOS ids integers inside [0, vocab) (vocab None: >= 0); anything else is a ValueError."""
+    import math
+
+    def rows(name, v, conv):
+        vals = list(v) if isinstance(v, (list, tuple)) or (torch.is_tensor(v) and v.dim() > 0) else [v] * n
+        if len(vals) != n:
+            raise ValueError(f"{name}: expected a scalar or {n} values, got {len(vals)}")
+        try:
+            return [conv(x) for x in vals]
+        except (TypeError, OverflowError, ValueError) as e:
+            raise ValueError(f"{name}: {e}") from None
+
+    def integer(x):
+        if isinstance(x, bool) or int(x) != x:
+            raise ValueError(f"expected an integer, got {x!r}")
+        return int(x)
+
+    rep, pres = rows("repetition_penalty", repetition_penalty, float), rows("presence_penalty", presence_penalty, float)
+    freq, mn = rows("frequency_penalty", frequency_penalty, float), rows("min_new_tokens", min_new_tokens, integer)
+    for b in range(n):
+        if not (math.isfinite(rep[b]) and rep[b] > 0.0):
+            raise ValueError(f"repetition_penalty: expected a finite value > 0 (1 = off), got {rep[b]}")
+        for name, v in (("presence_penalty", pres[b]), ("frequency_penalty", freq[b])):
+            if not -2.0 <= v <= 2.0:
+                raise ValueError(f"{name}: expected a value in [-2, 2], got {v}")
+        if not 0 <= mn[b] < 2 ** 31:
+            raise ValueError(f"min_new_tokens: expected an int32 >= 0, got {mn[b]}")
+    eos = [] if eos_token_id is None else eos_token_id
+    eos = list(eos) if isinstance(eos, (list, tuple)) or (torch.is_tensor(eos) and eos.dim() > 0) else [eos]
+    try:
+        eos = [integer(e) for e in eos]
+    except (TypeError, OverflowError, ValueError) as e:
+        raise ValueError(f"eos_token_id: {e}") from None
+    if len(eos) > 8:
+        raise ValueError(f"eos_token_id: at most 8 ids, got {len(eos)}")
+    for e in eos:
+        if e < 0 or (vocab is not None and e >= vocab):
+            raise ValueError(f"eos_token_id: {e} is outside the vocabulary" + (f" [0, {vocab})" if vocab else ""))
+    return rep, pres, freq, mn, eos
+
+
+def _processing_args(n: int, repetition_penalty=None, min_length=None, min_new_tokens=None, eos_token_id=None,
+                     pad_token_id=None):
+    """generate()'s logits-processing arguments (prompt of n positions, left padding included, as transformers counts
+    min_length) as set_processing keyword arguments, or None when they ask for nothing: no repetition penalty other than 1,
+    and no eos_token_id.  min_length / min_new_tokens without eos_token_id is a ValueError."""
+    floors = [m for m in (min_new_tokens, None if min_length is None else min_length - n) if m is not None]
+    min_new = max(floors + [0])
+    if eos_token_id is None and (min_new_tokens or min_length):
+        raise ValueError("min_length and min_new_tokens suppress eos_token_id until they are reached: pass eos_token_id "
+                         "(the config's EOS is not used as a default)")
+    rep = 1.0 if repetition_penalty is None else repetition_penalty
+    if rep == 1.0 and eos_token_id is None:
+        return None
+    return dict(repetition_penalty=rep, min_new_tokens=min_new, eos_token_id=eos_token_id, pad_token_id=pad_token_id)
+
+
 class LlamaForCausalLM_KIVI(nn.Module):
     """models/llama_kivi.py:785.  `forward` keeps the reference's contract (HF argument names, per-layer 9-tuples as
     past_key_values, fp32 logits, `prepare_inputs_for_generation`, `_reorder_cache`); `decode_step` / `generate` use
@@ -858,7 +923,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                      top_p=torch.ones(batch, dtype=torch.float32, device=dev),
                                      seed=torch.zeros(batch, dtype=torch.long, device=dev),
                                      draw=torch.zeros(batch, dtype=torch.long, device=dev))
-        self._tables(dev)                                    # rows for every position the cache can reach
+        # logits processing (set_processing): off, and its per-row state unallocated, until asked for
+        self._processing, self._proc = False, None
+        self._tables(dev)                                   # rows for every position the cache can reach
         return self.cache
 
     def import_cache(self, past_key_values, max_tokens: int | None = None):
@@ -900,6 +967,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
             starts = kv_start_from_mask(attention_mask)
             if not bool(starts.any()):
                 starts = None
+        if self._processing:
+            self._mark_prompt(input_ids, starts, slice(None), copies)
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
             mask = self._kernel_mask(None, n, input_ids.device)
@@ -939,12 +1008,37 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                 store_kv=lambda layer, k, v: self.cache.refill(layer, seq, k, v))
         self._pos[seq] = n
         self.cache.set_seq_start(seq, T - n)
+        if self._processing:
+            self._mark_prompt(ids, None, slice(seq, seq + 1))
         return self.lm_head(h[0, -1]).float()
 
     def release(self, seq: int):
         """Make slot `seq` idle (KiviCache.release): it keeps its row of every step but reads no cached byte."""
         self.cache.release(seq)
         self._pos[seq] = 0
+        if self._processing:
+            p = self._proc
+            for t in (p.seen, p.counts, p.n_new, p.finished):
+                t[seq].zero_()
+
+    def _mark_prompt(self, ids, starts, rows, copies: int = 1):
+        """Logits processing: the prompt ids [r, n] become the prompt bits of the batch rows `rows` (a slice of r * copies
+        rows; row j gets prompt j // copies), counting position i of prompt j only when i >= starts[j] (None: 0), so left
+        padding is not penalised.  The rows' generated counts, n_new and finished flags start from 0."""
+        p, V = self._proc, self.config.vocab_size
+        r, n = ids.shape
+        words = p.seen.shape[1]
+        live = ids.clamp(0, V - 1)
+        if starts is not None:
+            pos = torch.arange(n, device=ids.device).view(1, n)
+            live = torch.where(pos >= starts.to(ids.device).view(r, 1), live, words * 32)    # a column past the bits
+        hit = torch.zeros((r, words * 32 + 1), dtype=torch.bool, device=ids.device)
+        hit.scatter_(1, live, True)
+        w = (hit[:, :-1].view(r, words, 32).long() << torch.arange(32, device=ids.device)).sum(-1)
+        w = torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)                    # the uint32 words' bits
+        p.seen[rows] = w.repeat_interleave(copies, 0)
+        for t in (p.counts, p.n_new, p.finished):
+            t[rows].zero_()
 
     @torch.no_grad()
     def prefill_synthetic(self, n: int, seed: int = 0):
@@ -1029,6 +1123,82 @@ class LlamaForCausalLM_KIVI(nn.Module):
             dist.broadcast(tok, src=0)
         return tok if seq is None else tok[0]
 
+    # ------------------------------------------------------------------ logits processing
+    def set_processing(self, repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_new_tokens=0,
+                       eos_token_id=None, pad_token_id=None):
+        """Process the logits of every decode step on the device before the token choice (kivi_logits_process_f32 and, after
+        the choice, kivi_logits_record, inside the step's CUDA graph): the repetition penalty over the prompt's and the
+        generated tokens, the frequency and presence penalties over the generated ones, EOS suppression while a row has
+        fewer than min_new_tokens new tokens, and after a row's EOS only pad_token_id (default: the first EOS id).  The
+        greedy kernel or the sampler then chooses from the processed scores; decode_step still returns the raw logits.
+        Scalars, or one value per batch row (processing_rows); eos_token_id: an int or up to 8 ids, for every row.
+        Call before prefill() / insert(): they record the prompt tokens and reset the rows' counts, lengths and flags.
+        set_processing(None) returns the step to what it was without processing and frees the state.  The captured step is
+        dropped when processing turns on or off or pad_token_id changes, not when the other parameters do.  Under tensor
+        parallelism every rank calls this with the same arguments."""
+        assert self.cache is not None, "call init_cache() first"
+        on = repetition_penalty is not None
+        if on:
+            B, V, dev = self.cache.batch, self.config.vocab_size, self.cache.device
+            rep, pres, freq, mn, eos = processing_rows(B, repetition_penalty, presence_penalty, frequency_penalty,
+                                                       min_new_tokens, eos_token_id, V)
+            pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
+            if isinstance(pad, bool) or int(pad) != pad or not 0 <= int(pad) < V:
+                raise ValueError(f"pad_token_id: expected an id inside the vocabulary [0, {V}), got {pad!r}")
+            p = self._proc
+            if p is None:
+                i32 = dict(dtype=torch.int32, device=dev)
+                p = self._proc = SimpleNamespace(
+                    counts=torch.zeros((B, V), **i32), seen=torch.zeros((B, (V + 31) // 32), **i32),
+                    n_new=torch.zeros(B, **i32), finished=torch.zeros(B, dtype=torch.uint8, device=dev),
+                    repetition=torch.ones(B, dtype=torch.float32, device=dev),
+                    presence=torch.zeros(B, dtype=torch.float32, device=dev),
+                    frequency=torch.zeros(B, dtype=torch.float32, device=dev), min_new=torch.zeros(B, **i32),
+                    eos=torch.full((8,), -1, dtype=torch.long, device=dev),   # -1 matches no token: a fixed-size list
+                    scores=torch.empty((B, V), dtype=torch.float32, device=dev), pad=None, stops=False)
+            p.repetition.copy_(torch.tensor(rep, dtype=torch.float32).to(dev))
+            p.presence.copy_(torch.tensor(pres, dtype=torch.float32).to(dev))
+            p.frequency.copy_(torch.tensor(freq, dtype=torch.float32).to(dev))
+            p.min_new.copy_(torch.tensor(mn, dtype=torch.int32).to(dev))
+            p.eos.copy_(torch.tensor(eos + [-1] * (8 - len(eos)), dtype=torch.long).to(dev))
+            p.stops = bool(eos)
+            if p.pad != int(pad):
+                p.pad, self._graph = int(pad), None
+        else:
+            self._proc = None
+        if on != self._processing:
+            self._processing, self._graph = on, None
+
+    def set_slot_processing(self, seq: int, repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0,
+                            min_new_tokens=0):
+        """The processing parameters of batch row `seq` alone (a slot given to a new request); its counts, length and flag
+        are reset by insert().  The captured step reads them on the device: no recapture."""
+        if not self._processing:
+            raise RuntimeError("set_slot_processing: processing is off; call set_processing() first")
+        if not 0 <= seq < self.cache.batch:
+            raise ValueError(f"seq {seq} outside the batch of {self.cache.batch}")
+        rep, pres, freq, mn, _ = processing_rows(1, repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens)
+        p = self._proc
+        p.repetition[seq], p.presence[seq], p.frequency[seq], p.min_new[seq] = rep[0], pres[0], freq[0], mn[0]
+
+    def choose_first(self, logits, seq: int | None = None):
+        """The first token(s) from the prompt's last-position logits ([B, vocab] of prefill, or [vocab] of insert(seq)), as
+        the decode step chooses: processed (set_processing) with the rows' state, then the argmax (first_tokens) or a draw
+        (sample_first), then recorded.  Returns [B] ids, or a 0-d id for `seq`."""
+        from . import glue
+        p = self._proc if self._processing else None
+        rows = slice(None) if seq is None else slice(seq, seq + 1)
+        if p is not None:
+            flat = logits.reshape(-1, logits.shape[-1]).float().contiguous()
+            scores = torch.empty_like(flat)
+            glue.logits_process(flat, scores, p.counts[rows], p.seen[rows], p.n_new[rows], p.finished[rows],
+                                p.repetition[rows], p.presence[rows], p.frequency[rows], p.min_new[rows], p.eos, p.pad)
+            logits = scores if seq is None else scores[0]
+        tok = self.sample_first(logits, seq) if self._sampling else self.first_tokens(logits)
+        if p is not None:
+            glue.logits_record(tok.reshape(-1), p.counts[rows], p.n_new[rows], p.finished[rows], p.eos)
+        return tok
+
     @property
     def all_tokens(self):
         if self._exchange is not None:
@@ -1083,7 +1253,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
     def _step_body(self):
         """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split,
         fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels; then lm_head, the cache advance and the argmax
-        or sampling kernel.  A model with attention biases adds them in the q|k|v and o GEMMs (addmm).
+        or sampling kernel, which set_processing() frames with the logits-processing kernel before it and the record
+        kernel after it.  A model with attention biases adds them in the q|k|v and o GEMMs (addmm).
         Tensor-parallel (self._allreduce is a PeerAllReduce): the same launches on this rank's heads and channels, but o_proj
         and down_proj write their partial sums into the PeerAllReduce slots, and the two residual-add + RMSNorm kernels of a
         layer become kivi_allreduce_add_rmsnorm_f16 (calls 2i and 2i + 1 of the step), which add up every rank's partials.
@@ -1129,18 +1300,26 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._logits.copy_(f.logits16)                                       # logits.float() (:881)
         cache._enqueue_advance()                             # decode_step advances the host mirror after each replay
         self._pos.add_(1)
+        logits, p = self._logits, self._proc if self._processing else None
+        if p is not None:
+            # logits processing (set_processing): the choice reads the processed scores, decode_step returns the raw logits
+            glue.logits_process(logits, p.scores, p.counts, p.seen, p.n_new, p.finished, p.repetition, p.presence,
+                                p.frequency, p.min_new, p.eos, p.pad)
+            logits = p.scores
         # greedy sampling inside the step (and inside its CUDA graph): the argmax of a sequence needs only that
         # sequence's logits, so with data-parallel replicas the exchange is the sampled ids, 8 B per sequence
         if self._sampling:
             # in the argmax kernel's place, one kernel as well: a draw per sequence from its own parameters, seed and counter
             s = self._samp
-            glue.sample(self._logits, s.temperature, s.top_k, s.top_p, s.seed, s.draw, self.next_tokens, self._ids.view(-1))
+            glue.sample(logits, s.temperature, s.top_k, s.top_p, s.seed, s.draw, self.next_tokens, self._ids.view(-1))
         else:
             if self._exchange is not None:
                 self._exchange.step.add_(1)                  # the step number the peers' arrival counters are compared with
             # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight
             # into every peer's buffer over NVLink + arrival counters
-            glue.greedy_sample(self._logits, self.next_tokens, self._ids.view(-1), self._exchange)
+            glue.greedy_sample(logits, self.next_tokens, self._ids.view(-1), self._exchange)
+        if p is not None:
+            glue.logits_record(self.next_tokens, p.counts, p.n_new, p.finished, p.eos)
         if self._dist_tokens is not None and self._dist_in_graph:
             from . import dist as kdist
             kdist.gather_tokens(self.next_tokens, out=self._dist_tokens)
@@ -1176,6 +1355,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 state = self.cache.state.clone()
                 pos, ids0 = self._pos.clone(), self._ids.clone()
                 draw = self._samp.draw.clone() if self._sampling else None
+                proc = self._proc if self._processing else None
+                proc_state = [proc.counts.clone(), proc.n_new.clone(), proc.finished.clone()] if proc is not None else None
                 s = torch.cuda.Stream()
                 s.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(s):
@@ -1190,6 +1371,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 self._ids.copy_(ids0)
                 if draw is not None:
                     self._samp.draw.copy_(draw)                              # the warm-up step consumed a draw per row
+                if proc_state is not None:                                   # and recorded a token per row
+                    for t, saved in zip((proc.counts, proc.n_new, proc.finished), proc_state):
+                        t.copy_(saved)
                 from . import _lib
                 n0 = _lib.launch_count()
                 g = torch.cuda.CUDAGraph()
@@ -1223,7 +1407,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
     def generate(self, input_ids=None, max_new_tokens: int | None = None, use_graph: bool = True, attention_mask=None,
                  max_length: int | None = None, do_sample: bool = False, temperature=1.0, top_k=50, top_p=1.0, seed=0,
                  num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False,
-                 eos_token_id=None, pad_token_id=None, return_dict_in_generate: bool = False, **unused):
+                 eos_token_id=None, pad_token_id=None, return_dict_in_generate: bool = False, repetition_penalty=None,
+                 min_length: int | None = None, min_new_tokens: int | None = None, **unused):
         """Decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
         max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Greedy by default;
         do_sample=True samples every token, the first included, on the device with temperature / top_k / top_p (HF's
@@ -1235,14 +1420,31 @@ class LlamaForCausalLM_KIVI(nn.Module):
         before a step that would not fit, the positions that fell out of every window are dropped (KiviCache.shift), so
         the generated length is bounded by the RoPE tables rather than by cache memory.
         num_beams > 1 or num_return_sequences > 1: several sequences per prompt, see _generate_many; the other arguments
-        of that mode (length_penalty, early_stopping, eos_token_id, pad_token_id, return_dict_in_generate) are read there
-        only."""
+        of that mode (length_penalty, early_stopping, return_dict_in_generate) are read there only.
+        Logits processing (greedy and sampled decoding, set_processing): repetition_penalty (transformers'
+        RepetitionPenaltyLogitsProcessor over the prompt, left padding excluded, and the generated tokens), min_length
+        (counted as transformers does, from the padded prompt length) and min_new_tokens (EOS suppressed until then), and
+        EOS stopping: with eos_token_id (an int or a list) a row that emits one of them is finished and continues with
+        pad_token_id (default: the first EOS id), and decoding stops once every row has finished; the ids are then as long
+        as transformers' greedy or sampled generate returns them.  Unlike transformers, the config's EOS is not a default:
+        without eos_token_id the output has max_new_tokens new tokens, as it always had.  min_length or min_new_tokens
+        without eos_token_id is a ValueError, and beam search with a processor a NotImplementedError (transformers applies
+        them to log-probabilities there), both before any work.  Without these arguments the step is the one without
+        processing, launch for launch."""
+        proc = _processing_args(input_ids.shape[1], repetition_penalty, min_length, min_new_tokens, eos_token_id,
+                                pad_token_id)
         if num_beams != 1 or num_return_sequences != 1:
+            if num_beams > 1 and proc is not None and (proc["repetition_penalty"] != 1.0 or proc["min_new_tokens"]):
+                raise NotImplementedError("repetition_penalty, min_length and min_new_tokens in beam search are not "
+                                          "supported: transformers applies them to log-probabilities there")
             return self._generate_many(input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample,
                                        temperature, top_k, top_p, seed, num_beams, num_return_sequences, length_penalty,
-                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate)
+                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate, proc)
         if do_sample:
             sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
+        if proc is not None:
+            processing_rows(input_ids.shape[0], proc["repetition_penalty"], eos_token_id=proc["eos_token_id"],
+                            vocab=self.config.vocab_size)
         if attention_mask is not None:
             kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
         B, n = input_ids.shape
@@ -1261,21 +1463,44 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.set_sampling(temperature, top_k, top_p, seed)
         else:
             self.set_sampling(None)
+        if proc is not None:
+            self.set_processing(**proc)
+        else:
+            self.set_processing(None)
         logits = self.prefill(input_ids, attention_mask)
-        out = [input_ids]
-        tok = (self.sample_first(logits) if do_sample else self.first_tokens(logits)).view(B, 1)
-        for _ in range(max_new_tokens - 1):
-            out.append(tok)
+        return torch.cat([input_ids, self._decode(self.choose_first(logits).view(B, 1), max_new_tokens, use_graph)], 1)
+
+    def _decode(self, tok, max_new_tokens: int, use_graph: bool):
+        """The new tokens [rows, k] of a greedy or sampled generate(), from the first ones tok [rows, 1]: k = max_new_tokens,
+        or, when processing stops rows at EOS, the number of steps until every row had finished.  The finished flags of
+        token i are copied to the host asynchronously and read after step i + 1 has been launched, so the device never
+        waits for the host; the step launched past the last row's EOS is dropped."""
+        out = [tok]
+        stops = self._processing and self._proc.stops
+        if stops:
+            flags = [torch.empty(tok.shape[0], dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+            events = [torch.cuda.Event(), torch.cuda.Event()]
+
+            def copy_flags(i):
+                flags[i & 1].copy_(self._proc.finished, non_blocking=True)
+                events[i & 1].record()
+            copy_flags(0)
+        for i in range(1, max_new_tokens):
             if self.cache.kv_len + 1 > self.cache.max_tokens:
                 self._roll()
-            self.decode_step(tok, use_graph=use_graph)
-            tok = self.next_tokens.view(B, 1).clone()
-        out.append(tok)
+            self.decode_step(out[-1], use_graph=use_graph)
+            out.append(self.next_tokens.view(-1, 1).clone())
+            if stops:
+                copy_flags(i)
+                events[(i - 1) & 1].synchronize()
+                if bool(flags[(i - 1) & 1].all()):
+                    out.pop()                                        # every row had finished at token i - 1
+                    break
         return torch.cat(out, dim=1)
 
     def _generate_many(self, input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample, temperature,
                        top_k, top_p, seed, num_beams, num_return_sequences, length_penalty, early_stopping, eos_token_id,
-                       pad_token_id, return_dict_in_generate):
+                       pad_token_id, return_dict_in_generate, proc=None):
         """generate() with K = num_beams (beam search, kivi_b200.beam) or K = num_return_sequences (do_sample) sequences per
         prompt, in the cache's rows b * K .. b * K + K - 1.  The prompt pass runs once per prompt and its K / V fill the K
         rows (_prompt_pass(copies=K)).
@@ -1286,7 +1511,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         (KiviCache._enqueue_reorder: launches_per_reorder launches) and their positions.  Returns [B * n, length] ids, or
         with return_dict_in_generate an object with `sequences` and `sequences_scores`.
         do_sample: row b * n + j samples from the Philox key seed + b * n + j (set_sampling over the B * n rows), its first
-        token from prompt b's logits.  Returns [B * n, prompt + new] ids.
+        token from prompt b's logits, with the logits processing `proc` (generate()'s, set_processing) on every row.
+        Returns [B * n, prompt + new] ids.
         Refused before any work: beam sampling (NotImplementedError), num_return_sequences > num_beams and several greedy
         sequences per prompt (ValueError), beams with enable_token_allgather replicas (NotImplementedError)."""
         beams = num_beams > 1
@@ -1306,8 +1532,11 @@ class LlamaForCausalLM_KIVI(nn.Module):
         K = num_beams if beams else num_return_sequences
         B, n = input_ids.shape
         rows = B * K
+        proc = proc if do_sample else None                  # beam search reads eos_token_id itself
         if do_sample:
             sampling_rows(rows, temperature, top_k, top_p, seed)                # ValueError before any work
+        if proc is not None:
+            processing_rows(rows, proc["repetition_penalty"], eos_token_id=proc["eos_token_id"], vocab=self.config.vocab_size)
         if attention_mask is not None:
             kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
         if max_new_tokens is None:
@@ -1324,18 +1553,15 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.set_sampling(temperature, top_k, top_p, seed)
         else:
             self.set_sampling(None)
+        if proc is not None:
+            self.set_processing(**proc)
+        else:
+            self.set_processing(None)
         logits = self.lm_head(self._prompt_pass(input_ids, attention_mask, copies=K)[:, -1]).float()    # [B, vocab]
         if do_sample:
-            out = [input_ids.repeat_interleave(K, 0)]
-            tok = self.sample_first(logits.repeat_interleave(K, 0)).view(rows, 1)
-            for _ in range(max_new_tokens - 1):
-                out.append(tok)
-                if self.cache.kv_len + 1 > self.cache.max_tokens:
-                    self._roll()
-                self.decode_step(tok, use_graph=use_graph)
-                tok = self.next_tokens.view(rows, 1).clone()
-            out.append(tok)
-            seq, scores = torch.cat(out, dim=1), None
+            tok = self.choose_first(logits.repeat_interleave(K, 0)).view(rows, 1)
+            seq = torch.cat([input_ids.repeat_interleave(K, 0), self._decode(tok, max_new_tokens, use_graph)], 1)
+            scores = None
         else:
             from .beam import BeamSearch
             if eos_token_id is None:

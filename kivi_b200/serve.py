@@ -7,6 +7,8 @@ finished slot is released (kv_start beyond every length: it reads no cached byte
 that no live sequence sees any more are dropped from the front in multiples of max(128, R) (KiviCache.shift), so the
 timeline stays inside the cache.  A request decodes greedily, or samples with its own temperature / top-k / top-p / seed:
 the sampling kernel of the step reads each slot's parameters on the device, so both kinds share a batch and one step graph.
+A request may also carry a repetition, presence and frequency penalty and a minimum number of new tokens (logits processing
+inside the step, LlamaForCausalLM_KIVI.set_processing), read per slot on the device in the same way.
 """
 from __future__ import annotations
 
@@ -15,14 +17,33 @@ from collections import deque
 import torch
 
 from .cache import kv_start_from_mask
-from .llama_kivi import sampling_rows
+from .llama_kivi import PROCESSING_KEYS, processing_rows, sampling_rows
 
 GREEDY = dict(temperature=0.0, top_k=0, top_p=1.0, seed=0)            # the slot parameters of a request without params
+SAMPLING_KEYS = ("temperature", "top_k", "top_p", "seed")
+NEUTRAL = dict(repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_new_tokens=0)   # no processing
+
+
+def sampling_params(par):
+    """The sampling parameters of a request's params: None (greedy) for a request without params or whose params hold
+    processing keys only, else its sampling keys (the missing ones take generate(do_sample=True)'s defaults)."""
+    if par is None or (not any(k in par for k in SAMPLING_KEYS) and any(k in par for k in PROCESSING_KEYS)):
+        return None
+    return {k: v for k, v in par.items() if k in SAMPLING_KEYS}
+
+
+def processing_params(par):
+    """The logits-processing parameters of a request's params (None when it has none of the keys)."""
+    if par is None or not any(k in par for k in PROCESSING_KEYS):
+        return None
+    return {k: v for k, v in par.items() if k in PROCESSING_KEYS}
 
 
 def parse_requests(requests):
     """requests: (prompt ids, max_new_tokens) or (prompt ids, max_new_tokens, params) with params a dict of temperature,
-    top_k, top_p, seed (missing keys: 1.0, 50, 1.0, 0, as generate(do_sample=True); the seed is the request's Philox key).
+    top_k, top_p, seed (missing keys: 1.0, 50, 1.0, 0, as generate(do_sample=True); the seed is the request's Philox key)
+    and of repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens (missing keys: 1.0, 0.0, 0.0, 0;
+    processing_rows).  A request whose params hold processing keys only is greedy.
     Returns ([(prompt int64 1-D on the host, max_new_tokens)], [params or None]); ValueError for an empty prompt, a budget
     below 1, an unknown key or a value outside its range."""
     reqs, params = [], []
@@ -35,10 +56,11 @@ def parse_requests(requests):
         reqs.append((p, int(r[1])))
         par = r[2] if len(r) == 3 else None
         if par is not None:
-            unknown = set(par) - {"temperature", "top_k", "top_p", "seed"}
+            unknown = set(par) - set(SAMPLING_KEYS) - set(PROCESSING_KEYS)
             if unknown:
                 raise ValueError(f"request {i}: unknown sampling parameters {sorted(unknown)}")
-            sampling_rows(1, **par)                                       # ValueError for a value outside its range
+            sampling_rows(1, **{k: v for k, v in par.items() if k in SAMPLING_KEYS})   # ValueError outside its range
+            processing_rows(1, **{k: v for k, v in par.items() if k in PROCESSING_KEYS})
             par = dict(par)
         params.append(par)
     return reqs, params
@@ -66,14 +88,17 @@ def plan_admission(T: int, tv: int, max_tokens: int, quantum: int, live_starts, 
 
 
 @torch.no_grad()
-def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None = None, use_graph: bool = True,
+def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_graph: bool = True,
           stats: dict | None = None):
     """Decoding of a stream of requests with `batch` slots on one cache of `max_tokens` positions.
     requests: a list of (prompt ids 1-D, max_new_tokens), greedy, or (prompt ids, max_new_tokens, params), sampled on the
-    device with params = a dict of temperature, top_k, top_p, seed (parse_requests).  A sampled request's tokens depend on
-    its own prompt, parameters and seed only, not on its slot or on the other requests.  When no request has params the
-    step is the greedy one throughout.  serve() sets the model's mode (set_sampling) for its requests and leaves it so.
-    Yields (index into requests, new token ids [k] int64 on the host) as each request finishes: after max_new_tokens tokens, or after eos_token_id (included, as in HF).
+    device with params = a dict of temperature, top_k, top_p, seed, and of the logits-processing keys repetition_penalty,
+    presence_penalty, frequency_penalty, min_new_tokens (parse_requests; min_new_tokens suppresses eos_token_id).  A
+    request's tokens depend on its own prompt, parameters and seed only, not on its slot or on the other requests.  When no
+    request has sampling parameters the step is the greedy one throughout, and when none has processing keys the step has
+    no processing.  serve() sets the model's modes (set_sampling, set_processing) for its requests and leaves them so.
+    Yields (index into requests, new token ids [k] int64 on the host) as each request finishes: after max_new_tokens
+    tokens, or after an id of eos_token_id (an int or a list; included, as in HF).
     The first `batch` requests start with one left-padded prefill, padded to the longest prompt of the whole list, so every
     later prompt fits under the shared length.  Each step is one decode_step (its CUDA graph is captured once: the batch
     is ragged from the start) and one device-to-host read of the sampled ids; finished slots are released and refilled
@@ -82,7 +107,10 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
     reqs, params = parse_requests(requests)
     if not reqs:
         return
-    sampling = any(par is not None for par in params)
+    samp = [sampling_params(par) for par in params]
+    proc = [processing_params(par) for par in params]
+    sampling, processing = any(s is not None for s in samp), any(p is not None for p in proc)
+    eos = set() if eos_token_id is None else set(torch.as_tensor(eos_token_id).reshape(-1).tolist())
     longest = max(p.numel() for p, _ in reqs)
     for i, (p, m) in enumerate(reqs):
         if longest + m > max_tokens:
@@ -102,15 +130,22 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
         model.set_sampling(**GREEDY)
     else:
         model.set_sampling(None)
+    # the same for processing: neutral in every slot until a request with processing keys takes it (its scores are then
+    # its logits, bit for bit); EOS ends a request on the host (emit), and its slot's state is reset when it is released
+    if processing:
+        model.set_processing(**NEUTRAL, eos_token_id=eos_token_id)
+    else:
+        model.set_processing(None)
 
     def first_token(logits, slot=None, rows=None):
         """The first token(s) from prompt logits: of slot `slot` (insert) or of the whole batch, whose row b holds request
         rows[b] (prefill); a slot gets its request's parameters and a fresh draw counter here."""
-        if not sampling:
-            return model.first_tokens(logits)
         for b, i in enumerate(rows) if slot is None else [(slot, rows)]:
-            model.set_slot_sampling(b, **(GREEDY if params[i] is None else params[i]))
-        return model.sample_first(logits, slot)
+            if sampling:
+                model.set_slot_sampling(b, **(GREEDY if samp[i] is None else samp[i]))
+            if processing:
+                model.set_slot_processing(b, **(NEUTRAL if proc[i] is None else proc[i]))
+        return model.choose_first(logits, slot)
 
     queue = deque(range(len(reqs)))
     owner = [None] * batch                  # request index decoding in each slot
@@ -121,7 +156,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id: int | None
         """Append a token to the slot's output; finish (release) the slot on EOS or on its token budget."""
         outs[slot].append(tok)
         i = owner[slot]
-        if tok == eos_token_id or len(outs[slot]) >= reqs[i][1]:
+        if tok in eos or len(outs[slot]) >= reqs[i][1]:
             done.append((i, torch.tensor(outs[slot], dtype=torch.long)))
             owner[slot], outs[slot] = None, []
             model.release(slot)
