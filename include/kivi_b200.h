@@ -460,6 +460,24 @@ int kivi_logits_process_f32(const void* logits, void* scores, int batch, int voc
 int kivi_logits_record(const void* tokens, int batch, int vocab, int32_t* counts, int32_t* n_new, uint8_t* finished,
                        const int64_t* eos_ids, int n_eos, void* stream);
 
+/* Log-probabilities of chosen tokens under the softmax of their row, and the row's top N.  x = logits fp32 [batch, vocab]
+ * (only read), tokens int64 [batch] (e.g. next_local of the selection kernel), 0 <= n_top = N <= 20.  Per row b:
+ *   lse_b = m + log(sum_v exp(x[b, v] - m)), m the row's maximum (exp in fp32, the sum, the log and lse in fp64)
+ *   logprob[b]            = float(x[b, t] - lse_b), t = tokens[b]; NaN when t is outside [0, vocab)
+ *   top_ids[b, 0 .. N)    the N largest x[b, .] in descending order, ties by ascending id; a NaN ranks above +inf (all NaNs
+ *                         first, by id, as torch.topk orders them) and -0 equals +0.  N > vocab: entries vocab .. N-1 are -1
+ *   top_logprobs[b, j]    = float(x[b, top_ids[b, j]] - lse_b) (-inf for an id of -1), each value rounded once from fp64,
+ *                         so the chosen token's logprob equals its entry in the list bit for bit when it appears there.
+ * Special values give what torch.log_softmax(row.double()) gives: a NaN or +inf anywhere in the row, or a row with no finite
+ * value, makes every value of the row NaN (ids are still ranked); a -inf token of a row with a finite maximum gets -inf.
+ * Bound against the fp64 log_softmax r of the same row: |value - r| <= 2^-24 |r| + 2^-22 + 2^-24 * 104 (DESIGN.md: the final
+ * rounding, exp's error, and the rounding of x - m for the terms exp does not flush to 0).
+ * Row b's outputs depend only on row b and tokens[b] (every sum has a fixed order), and are bit-identical from run to run.
+ * top_ids / top_logprobs ([batch, N]) may be NULL when N = 0.  Requirements: batch >= 0, 1 <= vocab <= 2^22; argument errors
+ * return KIVI_ERR_* before any launch.  One launch, no scratch buffer, graph-capturable. */
+int kivi_token_logprobs_f32(const void* logits, int batch, int vocab, const int64_t* tokens, int n_top, float* logprob,
+                            int64_t* top_ids, float* top_logprobs, void* stream);
+
 /* Tensor-parallel residual-add + RMSNorm: the all-reduce after o_proj / down_proj fused into the norm that follows it.
  * With the rows of the attention heads and of the MLP columns sharded over `world` ranks, rank p holds a partial sum
  * partial_p [rows, hidden] fp16 of the projection.  Every rank computes the same bits:

@@ -617,6 +617,134 @@ logits_record_kernel(const long long* __restrict__ tokens, int B, int V, int* __
 }
 
 // ------------------------------------------------------------------------------------------------
+// Log-probabilities of the chosen tokens and the top-N of each row, contract in include/kivi_b200.h (kivi_token_logprobs_f32).
+// One CTA of kSampleThreads per row, the sampler's shape, so the top-N threshold is sample_select<false> itself: the N-th
+// largest key of the row.  Pass 1 reads the row for its maximum m; pass 2 sums exp(x - m) (fp32 exp, fp64 sum in a fixed
+// order: per thread in id order, then a fixed shuffle tree, then the 32 warp sums in warp order), so the bits depend on the
+// row alone.  lse = m + log(S) stays in fp64 and every value is rounded once: float(double(x) - lse).
+// The selection ranks ranked(x): a NaN becomes one positive NaN, whose key lies above that of +inf (NaN first, ties by id,
+// like torch.topk), and -0 becomes +0.  A row with a NaN passes xmax = NaN and one with +inf has xmax = +inf: every token
+// then falls in sample_bucket's bin 0, still monotone in the key, and the three key levels decide alone.
+// With the threshold key t: the tokens above t (fewer than N) are listed unordered, and each warp lists the first N tokens
+// AT t of its contiguous id segment in id order; thread 0 sorts the first list (at most 19 entries) and fills the rest from
+// the warps' lists in warp order, i.e. the smallest ids of the tie.
+// ------------------------------------------------------------------------------------------------
+constexpr int kLogprobMaxTop = 20;
+constexpr uint32_t kRankedNaN = 0x7fc00000u;
+
+__device__ __forceinline__ float logprob_ranked(float v)
+{
+    return (v != v) ? __uint_as_float(kRankedNaN) : (v == 0.f ? 0.f : v);
+}
+
+__device__ __forceinline__ float logprob_value(float v, double lse)
+{
+    return __double2float_rn((double)v - lse);
+}
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+token_logprobs_kernel(const float* __restrict__ logits, int V, const long long* __restrict__ tokens, int N,
+                      float* __restrict__ logprob, long long* __restrict__ top_ids, float* __restrict__ top_logprobs)
+{
+    __shared__ SampleShared s;
+    __shared__ double warp_S[kSampleWarps];
+    __shared__ int order[kLogprobMaxTop];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float* row = logits + (long long)b * V;
+
+    // pass 1: the maximum over the non-NaN values, and whether a NaN or +inf is present
+    float m = -INFINITY;
+    int nan = 0;
+    #pragma unroll 4
+    for (int i = tid; i < V; i += kSampleThreads) {
+        const float v = __ldg(row + i);
+        m = fmaxf(m, v);
+        nan |= v != v;
+    }
+    #pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    nan = __any_sync(0xffffffffu, nan);
+    if (lane == 0) { s.warp_max[warp] = m; s.warp_idx[warp] = nan; }
+    __syncthreads();
+    m = -INFINITY;
+    for (int w = 0; w < kSampleWarps; ++w) { m = fmaxf(m, s.warp_max[w]); nan |= s.warp_idx[w]; }
+    const bool bad = nan || !(m > -INFINITY) || m == INFINITY;                     // no finite maximum: every value is NaN
+
+    // pass 2: S = sum exp(x - m), the row's second read (from L2)
+    double lse = __longlong_as_double(0x7ff8000000000000ll);             // NaN
+    if (!bad) {
+        double acc = 0.0;
+        #pragma unroll 4
+        for (int i = tid; i < V; i += kSampleThreads) acc += (double)expf(__fsub_rn(__ldg(row + i), m));
+        #pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if (lane == 0) warp_S[warp] = acc;
+        __syncthreads();
+        double S = 0.0;
+        for (int w = 0; w < kSampleWarps; ++w) S += warp_S[w];
+        lse = (double)m + log(S);
+    }
+    if (tid == 0) {
+        const long long t = tokens[b];
+        logprob[b] = (t >= 0 && t < V) ? logprob_value(__ldg(row + t), lse) : __uint_as_float(kRankedNaN);
+    }
+    if (N == 0) return;
+
+    // the threshold: the key of the N-th largest ranked value (every token when N >= V)
+    auto x = [=](int i) { return logprob_ranked(__ldg(row + i)); };
+    const uint32_t thr = N < V ? sample_select<false>(x, V, 0u, nan ? __uint_as_float(kRankedNaN) : m,
+                                                      (unsigned long long)N, s) : 0u;
+    int* above = s.cand;                                                 // [kLogprobMaxTop] the tokens with key > thr
+    int* ties = s.cand + kLogprobMaxTop;                                 // [warp][N] each warp's first tokens at thr
+    if (tid == 0) s.cand_n = 0;
+    __syncthreads();
+    const int seg = cdiv(cdiv(V, kSampleWarps), 32) * 32;
+    const int end = min(V, (warp + 1) * seg);
+    int tied = 0;
+    for (int base = warp * seg; base < end; base += 32) {
+        const int i = base + lane;
+        uint32_t key = 0;
+        if (i < end) key = sample_key(x(i));
+        if (i < end && key > thr) {
+            const int at = atomicAdd(&s.cand_n, 1);
+            if (at < kLogprobMaxTop) above[at] = i;
+        }
+        const uint32_t eq = __ballot_sync(0xffffffffu, i < end && key == thr);
+        const int at = tied + __popc(eq & ((1u << lane) - 1));
+        if (((eq >> lane) & 1u) && at < N) ties[warp * N + at] = i;
+        tied += __popc(eq);
+    }
+    if (lane == 0) s.warp_cnt[warp] = min(tied, N);
+    __syncthreads();
+
+    if (tid == 0) {
+        const int na = min(s.cand_n, kLogprobMaxTop);
+        int n = 0;
+        for (int j = 0; j < na; ++j) {                                   // insertion sort: key descending, id ascending
+            const int id = above[j];
+            const uint32_t k = sample_key(x(id));
+            int p = n++;
+            for (; p > 0; --p) {
+                const int q = order[p - 1];
+                const uint32_t kq = sample_key(x(q));
+                if (kq > k || (kq == k && q < id)) break;
+                order[p] = q;
+            }
+            order[p] = id;
+        }
+        for (int w = 0; w < kSampleWarps && n < N; ++w)
+            for (int j = 0; j < s.warp_cnt[w] && n < N; ++j) order[n++] = ties[w * N + j];
+        for (; n < N; ++n) order[n] = -1;                                // N > vocab: no token
+    }
+    __syncthreads();
+    if (tid < N) {
+        const int id = order[tid];
+        top_ids[(long long)b * N + tid] = id;
+        top_logprobs[(long long)b * N + tid] = id >= 0 ? logprob_value(__ldg(row + id), lse) : -INFINITY;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Tensor-parallel residual-add + RMSNorm: the all-reduce of the o_proj / down_proj partial sums fused into the norm that
 // consumes them.  Every rank reads the `world` partials of this call straight from the peers' symmetric buffers (layout in
 // include/kivi_b200.h), sums them in fp32 in rank order, rounds to fp16 and runs add_rmsnorm_row on that addend, the body of
@@ -801,6 +929,18 @@ extern "C" int kivi_logits_record(const void* tokens, int batch, int vocab, int3
     if (batch == 0) return KIVI_OK;
     logits_record_kernel<<<cdiv(batch, kProcThreads), kProcThreads, 0, (cudaStream_t)stream>>>(
         (const long long*)tokens, batch, vocab, counts, n_new, finished, (const long long*)eos_ids, n_eos);
+    return post_launch();
+}
+
+extern "C" int kivi_token_logprobs_f32(const void* logits, int batch, int vocab, const int64_t* tokens, int n_top,
+                                       float* logprob, int64_t* top_ids, float* top_logprobs, void* stream)
+{
+    if (!logits || !tokens || !logprob) return KIVI_ERR_NULL;
+    if (n_top > 0 && (!top_ids || !top_logprobs)) return KIVI_ERR_NULL;
+    if (batch < 0 || vocab < 1 || vocab > kSampleMaxVocab || n_top < 0 || n_top > kLogprobMaxTop) return KIVI_ERR_SHAPE;
+    if (batch == 0) return KIVI_OK;
+    token_logprobs_kernel<<<batch, kSampleThreads, 0, (cudaStream_t)stream>>>(
+        (const float*)logits, vocab, (const long long*)tokens, n_top, logprob, (long long*)top_ids, top_logprobs);
     return post_launch();
 }
 

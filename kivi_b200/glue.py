@@ -1,6 +1,6 @@
 """ctypes wrappers of the decode-step glue kernels (csrc/kivi_model.cu): residual-add + RMSNorm,
-RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), logits processing and greedy and sampled next-token selection (fp32
-logits), and of the prompt
+RoPE + q/k/v split, SiLU*mul (fp16 CUDA tensors), logits processing, greedy and sampled next-token selection and the
+log-probabilities of chosen tokens (fp32 logits), and of the prompt
 pass's attention (csrc/kivi_prompt.cu); each wrapper checks device, dtype, contiguity and shapes
 before the call (ValueError, or RuntimeError for a CPU tensor)."""
 from __future__ import annotations
@@ -29,6 +29,7 @@ def _bind():
     i64 = ctypes.c_int64
     _lib.bind("kivi_logits_process_f32", i32, [vp, vp, i32, i32] + [vp] * 9 + [i32, i64, vp])
     _lib.bind("kivi_logits_record", i32, [vp, i32, i32, vp, vp, vp, vp, i32, vp])
+    _lib.bind("kivi_token_logprobs_f32", i32, [vp, i32, i32, vp, i32, vp, vp, vp, vp])
     _lib.bind("kivi_prompt_attention_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32] + [i64] * 6 + [vp, i32, vp])
     _B = True
 
@@ -226,6 +227,43 @@ def logits_record(tokens, counts, n_new, finished, eos):
     _lib.check(_lib.lib().kivi_logits_record(
         tokens.data_ptr(), B, V, counts.data_ptr(), n_new.data_ptr(), finished.data_ptr(), eos.data_ptr() if n_eos else None,
         n_eos, _lib.stream_ptr(tokens.device)), "kivi_logits_record")
+
+
+MAX_TOP_LOGPROBS = 20
+
+
+def token_logprobs(logits, tokens, logprob, top_ids=None, top_logprobs=None):
+    """logprob[b] = log_softmax(logits[b])[tokens[b]] (NaN for an id outside the vocabulary) and, with N = top_ids.shape[1]
+    (0 <= N <= 20), the row's N most likely ids in top_ids[b] (descending, ties by ascending id) and their log-probabilities
+    in top_logprobs[b].  logits fp32 [B, vocab], tokens int64 [B], logprob fp32 [B], top_ids int64 [B, N], top_logprobs fp32
+    [B, N] (both None for N = 0); include/kivi_b200.h (kivi_token_logprobs_f32) has the rules for NaN and infinities and
+    the error bound.  One launch, nothing allocated: a captured call reads new logits and tokens on every replay."""
+    _bind()
+    if logits.dim() != 2:
+        raise ValueError(f"logits: expected [B, vocab], got shape {tuple(logits.shape)}")
+    B, V = logits.shape
+    _check("logits", logits, torch.float32, (B, V))
+    if (top_ids is None) != (top_logprobs is None):
+        raise ValueError("top_ids and top_logprobs: expected both or neither")
+    N = 0
+    if top_ids is not None:
+        if top_ids.dim() != 2:
+            raise ValueError(f"top_ids: expected [B, N], got shape {tuple(top_ids.shape)}")
+        N = top_ids.shape[1]
+        if not 0 <= N <= MAX_TOP_LOGPROBS:
+            raise ValueError(f"top_ids: expected at most {MAX_TOP_LOGPROBS} columns, got {N}")
+    for name, t, dtype, shape in (("tokens", tokens, torch.int64, (B,)), ("logprob", logprob, torch.float32, (B,)),
+                                  ("top_ids", top_ids, torch.int64, (B, N)),
+                                  ("top_logprobs", top_logprobs, torch.float32, (B, N))):
+        if t is not None:
+            _check(name, t, dtype, shape)
+            if t.device != logits.device:
+                raise ValueError(f"{name}: on {t.device}, logits on {logits.device}")
+    ptr = lambda t: t.data_ptr() if t is not None else None             # noqa: E731
+    _lib.check(_lib.lib().kivi_token_logprobs_f32(
+        logits.data_ptr(), B, V, tokens.data_ptr(), N, logprob.data_ptr(), ptr(top_ids), ptr(top_logprobs),
+        _lib.stream_ptr(logits.device)), "kivi_token_logprobs_f32")
+    return logprob
 
 
 def prompt_attention(q, k, v, out, kv_start=None, window=None):

@@ -595,6 +595,38 @@ def _processing_args(n: int, repetition_penalty=None, min_length=None, min_new_t
     return dict(repetition_penalty=rep, min_new_tokens=min_new, eos_token_id=eos_token_id, pad_token_id=pad_token_id)
 
 
+def _trace_add(trace, logits, scores, clone: bool = False):
+    """One new token's entries of generate()'s output_logits / output_scores lists (either may be None: not asked for);
+    clone: the tensors are the step's static buffers.  With processing off the scores are the logits: one copy serves both."""
+    if trace is None:
+        return
+    lg = logits.reshape(-1, logits.shape[-1])
+    if clone and trace.logits is not None:
+        lg = lg.clone()
+    if trace.logits is not None:
+        trace.logits.append(lg)
+    if trace.scores is not None:
+        sc = scores.reshape(-1, scores.shape[-1])
+        if scores is logits:
+            sc = lg.clone() if clone and trace.logits is None else lg
+        elif clone:
+            sc = sc.clone()
+        trace.scores.append(sc)
+
+
+def _trace_pop(trace):
+    for t in (trace.scores, trace.logits):
+        if t is not None:
+            t.pop()
+
+
+def _generate_output(sequences, trace):
+    """transformers' GenerateDecoderOnlyOutput of a greedy or sampled generate(): the fields not asked for are None."""
+    from transformers.generation.utils import GenerateDecoderOnlyOutput
+    tup = lambda t: None if t is None else tuple(t)                       # noqa: E731
+    return GenerateDecoderOnlyOutput(sequences=sequences, scores=tup(trace.scores), logits=tup(trace.logits))
+
+
 class LlamaForCausalLM_KIVI(nn.Module):
     """models/llama_kivi.py:785.  `forward` keeps the reference's contract (HF argument names, per-layer 9-tuples as
     past_key_values, fp32 logits, `prepare_inputs_for_generation`, `_reorder_cache`); `decode_step` / `generate` use
@@ -636,6 +668,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._exchange = None               # kivi_b200.dist.PeerTokenExchange: ids stored into the peers' buffers by the sampling kernel
         self._allreduce = None              # kivi_b200.dist.PeerAllReduce of the tensor-parallel decode step
         self._sampling = False              # the step's last kernel samples (set_sampling) instead of taking the argmax
+        self._logprobs_n = None             # set_logprobs(): the step's top-N logprobs (None: off)
+        self.logprobs = self.top_ids = self.top_logprobs = None
 
     # ------------------------------------------------------------------ HF-style construction
     @classmethod
@@ -925,7 +959,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                      draw=torch.zeros(batch, dtype=torch.long, device=dev))
         # logits processing (set_processing): off, and its per-row state unallocated, until asked for
         self._processing, self._proc = False, None
+        # log-probabilities of the chosen tokens (set_logprobs): the mode outlives the cache, its buffers take the new batch
+        n_top, self._logprobs_n = self._logprobs_n, None
+        self.logprobs = self.top_ids = self.top_logprobs = None
         self._tables(dev)                                   # rows for every position the cache can reach
+        if n_top is not None:
+            self.set_logprobs(n_top)
         return self.cache
 
     def import_cache(self, past_key_values, max_tokens: int | None = None):
@@ -1181,13 +1220,16 @@ class LlamaForCausalLM_KIVI(nn.Module):
         p = self._proc
         p.repetition[seq], p.presence[seq], p.frequency[seq], p.min_new[seq] = rep[0], pres[0], freq[0], mn[0]
 
-    def choose_first(self, logits, seq: int | None = None):
+    def choose_first(self, logits, seq: int | None = None, return_scores: bool = False):
         """The first token(s) from the prompt's last-position logits ([B, vocab] of prefill, or [vocab] of insert(seq)), as
         the decode step chooses: processed (set_processing) with the rows' state, then the argmax (first_tokens) or a draw
-        (sample_first), then recorded.  Returns [B] ids, or a 0-d id for `seq`."""
+        (sample_first), then recorded; with set_logprobs() on, the rows' logprobs buffers receive the raw log-probabilities
+        of these tokens.  Returns [B] ids, or a 0-d id for `seq`; return_scores: (ids, the scores the choice read, in the
+        shape of `logits`: the processed ones, or `logits` itself with processing off)."""
         from . import glue
         p = self._proc if self._processing else None
         rows = slice(None) if seq is None else slice(seq, seq + 1)
+        raw = logits
         if p is not None:
             flat = logits.reshape(-1, logits.shape[-1]).float().contiguous()
             scores = torch.empty_like(flat)
@@ -1197,7 +1239,40 @@ class LlamaForCausalLM_KIVI(nn.Module):
         tok = self.sample_first(logits, seq) if self._sampling else self.first_tokens(logits)
         if p is not None:
             glue.logits_record(tok.reshape(-1), p.counts[rows], p.n_new[rows], p.finished[rows], p.eos)
-        return tok
+        if self._logprobs_n is not None:
+            top = self._logprobs_n > 0
+            glue.token_logprobs(raw.reshape(-1, raw.shape[-1]).float().contiguous(), tok.reshape(-1),
+                                self.logprobs[rows], self.top_ids[rows] if top else None,
+                                self.top_logprobs[rows] if top else None)
+        return (tok, logits) if return_scores else tok
+
+    # ------------------------------------------------------------------ log-probabilities
+    def set_logprobs(self, n_top=0):
+        """Log-probabilities of the chosen tokens, computed inside every decode step (kivi_token_logprobs_f32, after the
+        token choice, inside the step's CUDA graph) and by choose_first for the first token: `logprobs` [B] fp32 receives
+        each row's log-probability of its new token and `top_ids` [B, n_top] int64 / `top_logprobs` [B, n_top] fp32 the row's
+        n_top most likely tokens (descending, ties by ascending id), 0 <= n_top <= 20.  These are raw log-probabilities, the
+        log-softmax of the logits decode_step() returns: before logits processing, temperature, top-k and top-p.  The
+        buffers are static, overwritten by the next step, and reallocated for the new batch by init_cache(), which keeps
+        the mode (so does generate(), which may call it).  set_logprobs(None) turns the mode off and frees them; the
+        captured step is dropped when the mode turns on or off or n_top changes.  Under tensor parallelism every rank
+        computes the same values (the logits are replicated)."""
+        assert self.cache is not None, "call init_cache() first"
+        if n_top is not None:
+            from .glue import MAX_TOP_LOGPROBS
+            if isinstance(n_top, bool) or int(n_top) != n_top or not 0 <= int(n_top) <= MAX_TOP_LOGPROBS:
+                raise ValueError(f"n_top: expected an int in [0, {MAX_TOP_LOGPROBS}], got {n_top!r}")
+            n_top = int(n_top)
+        if n_top == self._logprobs_n:
+            return
+        self._logprobs_n, self._graph = n_top, None
+        if n_top is None:
+            self.logprobs = self.top_ids = self.top_logprobs = None
+        else:
+            B, dev = self.cache.batch, self.cache.device
+            self.logprobs = torch.zeros(B, dtype=torch.float32, device=dev)
+            self.top_ids = torch.zeros((B, n_top), dtype=torch.long, device=dev)
+            self.top_logprobs = torch.zeros((B, n_top), dtype=torch.float32, device=dev)
 
     @property
     def all_tokens(self):
@@ -1254,7 +1329,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split,
         fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels; then lm_head, the cache advance and the argmax
         or sampling kernel, which set_processing() frames with the logits-processing kernel before it and the record
-        kernel after it.  A model with attention biases adds them in the q|k|v and o GEMMs (addmm).
+        kernel after it; set_logprobs() adds the log-probability kernel after the choice.  A model with attention biases adds them in the q|k|v and o GEMMs (addmm).
         Tensor-parallel (self._allreduce is a PeerAllReduce): the same launches on this rank's heads and channels, but o_proj
         and down_proj write their partial sums into the PeerAllReduce slots, and the two residual-add + RMSNorm kernels of a
         layer become kivi_allreduce_add_rmsnorm_f16 (calls 2i and 2i + 1 of the step), which add up every rank's partials.
@@ -1318,6 +1393,11 @@ class LlamaForCausalLM_KIVI(nn.Module):
             # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight
             # into every peer's buffer over NVLink + arrival counters
             glue.greedy_sample(logits, self.next_tokens, self._ids.view(-1), self._exchange)
+        if self._logprobs_n is not None:
+            # log-probabilities of the chosen ids under the raw logits (set_logprobs); one more launch
+            top = self._logprobs_n > 0
+            glue.token_logprobs(self._logits, self.next_tokens, self.logprobs, self.top_ids if top else None,
+                                self.top_logprobs if top else None)
         if p is not None:
             glue.logits_record(self.next_tokens, p.counts, p.n_new, p.finished, p.eos)
         if self._dist_tokens is not None and self._dist_in_graph:
@@ -1408,7 +1488,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
                  max_length: int | None = None, do_sample: bool = False, temperature=1.0, top_k=50, top_p=1.0, seed=0,
                  num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False,
                  eos_token_id=None, pad_token_id=None, return_dict_in_generate: bool = False, repetition_penalty=None,
-                 min_length: int | None = None, min_new_tokens: int | None = None, **unused):
+                 min_length: int | None = None, min_new_tokens: int | None = None, output_scores: bool = False,
+                 output_logits: bool = False, **unused):
         """Decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
         max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Greedy by default;
         do_sample=True samples every token, the first included, on the device with temperature / top_k / top_p (HF's
@@ -1430,7 +1511,23 @@ class LlamaForCausalLM_KIVI(nn.Module):
         without eos_token_id the output has max_new_tokens new tokens, as it always had.  min_length or min_new_tokens
         without eos_token_id is a ValueError, and beam search with a processor a NotImplementedError (transformers applies
         them to log-probabilities there), both before any work.  Without these arguments the step is the one without
-        processing, launch for launch."""
+        processing, launch for launch.
+        return_dict_in_generate=True returns transformers' GenerateDecoderOnlyOutput(sequences, scores, logits), its
+        unrequested fields None.  output_logits=True: a tuple with one fp32 [rows, vocab] tensor per new token, the raw
+        logits it was chosen from (the prompt's last position for the first token, then each decode_step's logits).
+        output_scores=True (greedy only): the scores the argmax read, i.e. the processed scores with logits processing on
+        and the logits without it; unlike transformers, a row that has finished gets the pad-only scores of the processing
+        kernel (0 at the pad id, -inf elsewhere) rather than further processed logits.  Both tuples have exactly one entry
+        per new token, also when decoding stops at EOS.  They stay on the device: rows * vocab * 4 bytes per new token
+        each, as in transformers.  compute_transition_scores() turns them into per-token scores.  output_scores with
+        do_sample=True (transformers returns the scores after its warpers, which the sampler never materialises) and either
+        output with beam search are NotImplementedError, before any work."""
+        if (output_scores or output_logits) and num_beams > 1:
+            raise NotImplementedError("output_scores and output_logits in beam search are not supported")
+        if output_scores and do_sample:
+            raise NotImplementedError("output_scores with do_sample=True is not supported: the sampler never materialises "
+                                      "the warped scores transformers returns; use output_logits")
+        trace = SimpleNamespace(scores=[] if output_scores else None, logits=[] if output_logits else None)
         proc = _processing_args(input_ids.shape[1], repetition_penalty, min_length, min_new_tokens, eos_token_id,
                                 pad_token_id)
         if num_beams != 1 or num_return_sequences != 1:
@@ -1439,7 +1536,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                           "supported: transformers applies them to log-probabilities there")
             return self._generate_many(input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample,
                                        temperature, top_k, top_p, seed, num_beams, num_return_sequences, length_penalty,
-                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate, proc)
+                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate, proc, trace)
         if do_sample:
             sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
         if proc is not None:
@@ -1468,13 +1565,32 @@ class LlamaForCausalLM_KIVI(nn.Module):
         else:
             self.set_processing(None)
         logits = self.prefill(input_ids, attention_mask)
-        return torch.cat([input_ids, self._decode(self.choose_first(logits).view(B, 1), max_new_tokens, use_graph)], 1)
+        tok, scores = self.choose_first(logits, return_scores=True)
+        _trace_add(trace, logits, scores)
+        seq = torch.cat([input_ids, self._decode(tok.view(B, 1), max_new_tokens, use_graph, trace)], 1)
+        return _generate_output(seq, trace) if return_dict_in_generate else seq
 
-    def _decode(self, tok, max_new_tokens: int, use_graph: bool):
+    def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits: bool = False):
+        """transformers' GenerationMixin.compute_transition_scores for greedy and sampled outputs: the score of each
+        generated token, [rows, len(scores)], from generate()'s `scores` (or `logits`) tuple.  normalize_logits=True takes
+        the log-softmax of every step's row first (then, with output_logits, these are the tokens' raw log-probabilities).
+        On the host's torch, in the tensors' own dtype and device.  beam_indices (beam search) is NotImplementedError."""
+        if beam_indices is not None:
+            raise NotImplementedError("compute_transition_scores with beam_indices: beam search returns no per-step scores")
+        V, steps = self.config.vocab_size, len(scores)
+        s = torch.stack(scores).reshape(steps, -1).transpose(0, 1)          # [rows * vocab, steps], transformers' layout
+        if normalize_logits:
+            s = torch.nn.functional.log_softmax(s.reshape(-1, V, steps), dim=1).reshape(-1, steps)
+        rows = torch.arange(s.shape[0] // V, device=sequences.device).view(-1, 1) * V
+        return s.gather(0, sequences[:, sequences.shape[-1] - steps:] + rows)
+
+    def _decode(self, tok, max_new_tokens: int, use_graph: bool, trace=None):
         """The new tokens [rows, k] of a greedy or sampled generate(), from the first ones tok [rows, 1]: k = max_new_tokens,
         or, when processing stops rows at EOS, the number of steps until every row had finished.  The finished flags of
         token i are copied to the host asynchronously and read after step i + 1 has been launched, so the device never
-        waits for the host; the step launched past the last row's EOS is dropped."""
+        waits for the host; the step launched past the last row's EOS is dropped.  trace (generate's output_scores /
+        output_logits lists, already holding the first token's entries): each step's scores and logits are cloned after
+        its replay, and dropped with the step that is."""
         out = [tok]
         stops = self._processing and self._proc.stops
         if stops:
@@ -1488,19 +1604,23 @@ class LlamaForCausalLM_KIVI(nn.Module):
         for i in range(1, max_new_tokens):
             if self.cache.kv_len + 1 > self.cache.max_tokens:
                 self._roll()
-            self.decode_step(out[-1], use_graph=use_graph)
+            logits = self.decode_step(out[-1], use_graph=use_graph)
             out.append(self.next_tokens.view(-1, 1).clone())
+            if trace is not None:
+                _trace_add(trace, logits, self._proc.scores if self._processing else logits, clone=True)
             if stops:
                 copy_flags(i)
                 events[(i - 1) & 1].synchronize()
                 if bool(flags[(i - 1) & 1].all()):
                     out.pop()                                        # every row had finished at token i - 1
+                    if trace is not None:
+                        _trace_pop(trace)
                     break
         return torch.cat(out, dim=1)
 
     def _generate_many(self, input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample, temperature,
                        top_k, top_p, seed, num_beams, num_return_sequences, length_penalty, early_stopping, eos_token_id,
-                       pad_token_id, return_dict_in_generate, proc=None):
+                       pad_token_id, return_dict_in_generate, proc=None, trace=None):
         """generate() with K = num_beams (beam search, kivi_b200.beam) or K = num_return_sequences (do_sample) sequences per
         prompt, in the cache's rows b * K .. b * K + K - 1.  The prompt pass runs once per prompt and its K / V fill the K
         rows (_prompt_pass(copies=K)).
@@ -1512,7 +1632,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         with return_dict_in_generate an object with `sequences` and `sequences_scores`.
         do_sample: row b * n + j samples from the Philox key seed + b * n + j (set_sampling over the B * n rows), its first
         token from prompt b's logits, with the logits processing `proc` (generate()'s, set_processing) on every row.
-        Returns [B * n, prompt + new] ids.
+        Returns [B * n, prompt + new] ids, or with return_dict_in_generate generate()'s GenerateDecoderOnlyOutput (`trace`:
+        its output_logits, per row).
         Refused before any work: beam sampling (NotImplementedError), num_return_sequences > num_beams and several greedy
         sequences per prompt (ValueError), beams with enable_token_allgather replicas (NotImplementedError)."""
         beams = num_beams > 1
@@ -1559,8 +1680,11 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.set_processing(None)
         logits = self.lm_head(self._prompt_pass(input_ids, attention_mask, copies=K)[:, -1]).float()    # [B, vocab]
         if do_sample:
-            tok = self.choose_first(logits.repeat_interleave(K, 0)).view(rows, 1)
-            seq = torch.cat([input_ids.repeat_interleave(K, 0), self._decode(tok, max_new_tokens, use_graph)], 1)
+            first = logits.repeat_interleave(K, 0)
+            tok = self.choose_first(first).view(rows, 1)
+            if trace is not None:
+                _trace_add(trace, first, first)
+            seq = torch.cat([input_ids.repeat_interleave(K, 0), self._decode(tok, max_new_tokens, use_graph, trace)], 1)
             scores = None
         else:
             from .beam import BeamSearch
@@ -1585,9 +1709,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
             seq, scores = search.finalize()
         if not return_dict_in_generate:
             return seq
-        from transformers.generation.utils import GenerateBeamDecoderOnlyOutput, GenerateDecoderOnlyOutput
+        from transformers.generation.utils import GenerateBeamDecoderOnlyOutput
         if scores is None:
-            return GenerateDecoderOnlyOutput(sequences=seq)
+            return _generate_output(seq, trace)
         return GenerateBeamDecoderOnlyOutput(sequences=seq, sequences_scores=scores)
 
     def _reorder_rows(self, beam_idx, rows, use_graph: bool = True):

@@ -8,11 +8,15 @@ that no live sequence sees any more are dropped from the front in multiples of m
 timeline stays inside the cache.  A request decodes greedily, or samples with its own temperature / top-k / top-p / seed:
 the sampling kernel of the step reads each slot's parameters on the device, so both kinds share a batch and one step graph.
 A request may also carry a repetition, presence and frequency penalty and a minimum number of new tokens (logits processing
-inside the step, LlamaForCausalLM_KIVI.set_processing), read per slot on the device in the same way.
+inside the step, LlamaForCausalLM_KIVI.set_processing), read per slot on the device in the same way, and ask for the
+log-probabilities of its tokens (`logprobs`, LlamaForCausalLM_KIVI.set_logprobs), computed inside the step as well.
 """
 from __future__ import annotations
 
 from collections import deque
+from typing import NamedTuple
+
+from types import SimpleNamespace
 
 import torch
 
@@ -22,6 +26,29 @@ from .llama_kivi import PROCESSING_KEYS, processing_rows, sampling_rows
 GREEDY = dict(temperature=0.0, top_k=0, top_p=1.0, seed=0)            # the slot parameters of a request without params
 SAMPLING_KEYS = ("temperature", "top_k", "top_p", "seed")
 NEUTRAL = dict(repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_new_tokens=0)   # no processing
+MAX_LOGPROBS = 20
+
+
+class TokenLogprobs(NamedTuple):
+    """The raw log-probabilities of a request's k new tokens, on the host: `token` fp32 [k] of each chosen token, and the
+    request's N most likely tokens at each position, `top_ids` int64 [k, N] (descending, ties by ascending id) with their
+    log-probabilities `top` fp32 [k, N]."""
+    token: torch.Tensor
+    top_ids: torch.Tensor
+    top: torch.Tensor
+
+
+def logprobs_param(par):
+    """The number of top log-probabilities a request's params ask for (0: the chosen token's only), or None."""
+    return None if par is None else par.get("logprobs")
+
+
+def decoding_params(par):
+    """A request's params without `logprobs`, which never changes its tokens: None (greedy) when that was its only key."""
+    if par is None or "logprobs" not in par:
+        return par
+    rest = {k: v for k, v in par.items() if k != "logprobs"}
+    return rest or None
 
 
 def sampling_params(par):
@@ -43,7 +70,8 @@ def parse_requests(requests):
     """requests: (prompt ids, max_new_tokens) or (prompt ids, max_new_tokens, params) with params a dict of temperature,
     top_k, top_p, seed (missing keys: 1.0, 50, 1.0, 0, as generate(do_sample=True); the seed is the request's Philox key)
     and of repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens (missing keys: 1.0, 0.0, 0.0, 0;
-    processing_rows).  A request whose params hold processing keys only is greedy.
+    processing_rows), and `logprobs`: an int N, 0 <= N <= 20, the number of top log-probabilities wanted with each token.
+    A request whose params hold processing keys or `logprobs` only is greedy.
     Returns ([(prompt int64 1-D on the host, max_new_tokens)], [params or None]); ValueError for an empty prompt, a budget
     below 1, an unknown key or a value outside its range."""
     reqs, params = [], []
@@ -56,9 +84,12 @@ def parse_requests(requests):
         reqs.append((p, int(r[1])))
         par = r[2] if len(r) == 3 else None
         if par is not None:
-            unknown = set(par) - set(SAMPLING_KEYS) - set(PROCESSING_KEYS)
+            unknown = set(par) - set(SAMPLING_KEYS) - set(PROCESSING_KEYS) - {"logprobs"}
             if unknown:
                 raise ValueError(f"request {i}: unknown sampling parameters {sorted(unknown)}")
+            n = par.get("logprobs", 0)
+            if isinstance(n, bool) or not isinstance(n, int) or not 0 <= n <= MAX_LOGPROBS:
+                raise ValueError(f"request {i}: logprobs: expected an int in [0, {MAX_LOGPROBS}], got {n!r}")
             sampling_rows(1, **{k: v for k, v in par.items() if k in SAMPLING_KEYS})   # ValueError outside its range
             processing_rows(1, **{k: v for k, v in par.items() if k in PROCESSING_KEYS})
             par = dict(par)
@@ -98,7 +129,11 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     request has sampling parameters the step is the greedy one throughout, and when none has processing keys the step has
     no processing.  serve() sets the model's modes (set_sampling, set_processing) for its requests and leaves them so.
     Yields (index into requests, new token ids [k] int64 on the host) as each request finishes: after max_new_tokens
-    tokens, or after an id of eos_token_id (an int or a list; included, as in HF).
+    tokens, or after an id of eos_token_id (an int or a list; included, as in HF).  When a request of the call has a
+    `logprobs` key, every yield is (index, ids, lp) instead: lp is None for a request without the key, else a
+    TokenLogprobs of its k tokens with its own N columns -- the raw log-probabilities (before processing, temperature,
+    top-k and top-p) that the step computes at the largest N asked for (set_logprobs) and returns under the step's one
+    device-to-host read.  `logprobs` never changes a request's tokens.
     The first `batch` requests start with one left-padded prefill, padded to the longest prompt of the whole list, so every
     later prompt fits under the shared length.  Each step is one decode_step (its CUDA graph is captured once: the batch
     is ragged from the start) and one device-to-host read of the sampled ids; finished slots are released and refilled
@@ -107,8 +142,11 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     reqs, params = parse_requests(requests)
     if not reqs:
         return
+    lp_n = [logprobs_param(par) for par in params]
+    params = [decoding_params(par) for par in params]
     samp = [sampling_params(par) for par in params]
     proc = [processing_params(par) for par in params]
+    want_lp = any(n is not None for n in lp_n)
     sampling, processing = any(s is not None for s in samp), any(p is not None for p in proc)
     eos = set() if eos_token_id is None else set(torch.as_tensor(eos_token_id).reshape(-1).tolist())
     longest = max(p.numel() for p, _ in reqs)
@@ -136,6 +174,27 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
         model.set_processing(**NEUTRAL, eos_token_id=eos_token_id)
     else:
         model.set_processing(None)
+    if want_lp:
+        n_top = max(n for n in lp_n if n is not None)
+        model.set_logprobs(n_top)
+        host = SimpleNamespace(ids=torch.empty(batch, dtype=torch.long, pin_memory=True),
+                               lp=torch.empty(batch, dtype=torch.float32, pin_memory=True),
+                               top_ids=torch.empty((batch, n_top), dtype=torch.long, pin_memory=True),
+                               top=torch.empty((batch, n_top), dtype=torch.float32, pin_memory=True),
+                               done=torch.cuda.Event())
+    else:
+        model.set_logprobs(None)
+
+    def read(ids):
+        """The ids [batch] (device) to the host, with the logprobs buffers when they are on: one synchronisation."""
+        if not want_lp:
+            return ids.tolist()
+        for dst, src in ((host.ids, ids), (host.lp, model.logprobs), (host.top_ids, model.top_ids),
+                         (host.top, model.top_logprobs)):
+            dst.copy_(src, non_blocking=True)
+        host.done.record()
+        host.done.synchronize()
+        return host.ids.tolist()
 
     def first_token(logits, slot=None, rows=None):
         """The first token(s) from prompt logits: of slot `slot` (insert) or of the whole batch, whose row b holds request
@@ -150,15 +209,26 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     queue = deque(range(len(reqs)))
     owner = [None] * batch                  # request index decoding in each slot
     outs = [[] for _ in range(batch)]
+    lps = [[] for _ in range(batch)]        # the slot's rows of the host logprobs buffers, one per token
     done = []
 
     def emit(slot, tok):
         """Append a token to the slot's output; finish (release) the slot on EOS or on its token budget."""
         outs[slot].append(tok)
         i = owner[slot]
+        if want_lp and lp_n[i] is not None:
+            n = lp_n[i]
+            lps[slot].append((host.lp[slot].clone(), host.top_ids[slot, :n].clone(), host.top[slot, :n].clone()))
         if tok in eos or len(outs[slot]) >= reqs[i][1]:
-            done.append((i, torch.tensor(outs[slot], dtype=torch.long)))
-            owner[slot], outs[slot] = None, []
+            ids = torch.tensor(outs[slot], dtype=torch.long)
+            if not want_lp:
+                done.append((i, ids))
+            elif lp_n[i] is None:
+                done.append((i, ids, None))
+            else:
+                t, top_ids, top = zip(*lps[slot])
+                done.append((i, ids, TokenLogprobs(torch.stack(t), torch.stack(top_ids), torch.stack(top))))
+            owner[slot], outs[slot], lps[slot] = None, [], []
             model.release(slot)
 
     def start_group():
@@ -176,7 +246,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
         cache.set_kv_start(kv_start_from_mask(mask))                      # ragged from the start: one step graph
         first = first_token(logits, rows=rows)
         model._ids.copy_(first.view(batch, 1))
-        first = first.tolist()
+        first = read(first)
         stats["prefills"] += 1
         for b in range(batch):
             if b < len(rows):
@@ -201,7 +271,8 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
                         stats["shifts"] += 1
                         stats["shifted_tokens"] += plan[0]
                     i = queue.popleft()
-                    tok = int(first_token(model.insert(slot, p.to(dev)), slot, i))
+                    tok = first_token(model.insert(slot, p.to(dev)), slot, i)
+                    tok = read(tok.view(1).expand(batch))[0] if want_lp else int(tok)
                     model._ids[slot] = tok
                     owner[slot] = i
                     stats["inserts"] += 1
@@ -214,7 +285,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
         if not live:
             continue
         model.decode_step(use_graph=use_graph)
-        toks = model.next_tokens.tolist()                                 # the step's one device-to-host read
+        toks = read(model.next_tokens)                                    # the step's one device-to-host read
         stats["steps"] += 1
         stats["slot_steps"] += len(live)
         for b in live:
