@@ -385,6 +385,27 @@ int kivi_prompt_attention_f16(const void* q, const void* k, const void* v, void*
                               int64_t kv_sb, int64_t kv_sh, int64_t kv_st,
                               const int32_t* kv_start, int window, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Suffix prompt attention: the last m tokens of a prompt over the whole prompt, whose first n - m tokens' K / V were
+ * computed earlier (a stored prefix).
+ *   q [B, H, m, 128]: the queries at positions n - m .. n - 1; k / v [B, Hkv, n, 128]; out [B, m, H, 128] fp16
+ *   contiguous; strides, kv_start and window as in kivi_prompt_attention_f16.
+ * Query t sits at position i = n - m + t and sees the keys max(s_b, i - window + 1) <= j <= i: the rule above with i
+ * counted from the start of the keys.  The same kernel runs both entries and visits key tiles in ascending absolute
+ * position, so a row meets the tiles where it sees a key in the same order in both.  Where n - m is not a multiple of a
+ * CTA's tokens, a row may also visit tiles in which it sees nothing; those leave its online softmax exactly unchanged
+ * (alpha 0 with no key seen yet, 1 after; every p 0).  Row t therefore equals row n - m + t of kivi_prompt_attention_f16
+ * on the same q / k / v bit for bit (m = n: the same output).  Tiles below the window of a CTA's first query and below kv_start are never read, so the work
+ * follows the suffix's visible pairs, not n^2.
+ * Requirements: those of kivi_prompt_attention_f16, and 1 <= m <= n (KIVI_ERR_SHAPE).  One launch, no allocation, no
+ * synchronisation; CUDA-graph capturable.
+ * ------------------------------------------------------------------------------------------ */
+int kivi_prompt_attention_suffix_f16(const void* q, const void* k, const void* v, void* out,
+                                     int batch, int num_heads, int num_kv_heads, int m, int n,
+                                     int64_t q_sb, int64_t q_sh, int64_t q_st,
+                                     int64_t kv_sb, int64_t kv_sh, int64_t kv_st,
+                                     const int32_t* kv_start, int window, void* stream);
+
 /* Greedy sampling fused with its collective (the only exchange of the data-parallel decode, SURVEY 8e; the reference has
  * none).  next_local[b] = argmax_v logits[b, v] (first index among equal maxima, as torch.argmax; logits fp32 [batch, vocab],
  * models/llama_kivi.py:881); ids_feedback (may be NULL) receives the same ids (the next step's input buffer).

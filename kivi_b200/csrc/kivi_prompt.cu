@@ -7,6 +7,16 @@
 // accumulators), with an online (running) maximum and sum in fp32.  K / V tiles are staged by cp.async into two stages
 // while the previous tile is contracted.  Tiles with no visible key for any row of the CTA -- after its last token, below
 // the sequence's first real token, below the window of its first token -- are never loaded.
+//
+// The queries may be the last m of the n keys' positions (a prompt's suffix over a stored prefix and itself): query t
+// then sits at position n - m + t, the masks and the key tiles follow that position, and a CTA's tiles run from the
+// window of its first query to its last query in absolute key positions, in ascending order.  Every tile in which a row
+// sees a key is therefore visited, in the same order, as in the pass over all n queries.  The CTAs group the rows
+// differently when n - m is not a multiple of the tokens per CTA, so a row may visit extra tiles before its first
+// visible key or after its last; such a tile leaves the row's state exactly as it was: before any visible key m stays
+// -inf, m_use = 0, alpha = exp2(-inf) = 0 and every p = 0, so o and l stay 0; after one, m is unchanged, alpha =
+// exp2(0) = 1 and every p = exp2(-inf) = 0.  The output is thus the full pass's row bit for bit -- a property that rests
+// on the m_use guard below and on P.V adding exact zeros.
 #include "kivi_decode.cuh"
 
 namespace kivi {
@@ -42,10 +52,11 @@ struct PromptArgs {
     const __half* q;
     const __half* k;
     const __half* v;
-    __half* out;                          // [B, n, H, 128]
+    __half* out;                          // [B, q_len, H, 128]
     int64_t q_sb, q_sh, q_st, kv_sb, kv_sh, kv_st;
     const int32_t* kv_start;              // NULL or [B]
     int H, G, n, window;
+    int q_len, q_off;                     // queries: the positions q_off .. q_off + q_len - 1 = n - 1 of the keys
     int hc;                               // query heads per CTA, min(G, 64)
     int mt;                               // tokens per CTA, 64 / hc
     int chunks;                           // CTAs per KV head and token tile, ceil(G / hc)
@@ -62,13 +73,14 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
     const int h0 = (blockIdx.y % a.chunks) * a.hc;    // this CTA's first query head within the group
     const int nh = min(a.hc, a.G - h0);
     const int t0 = (gridDim.x - 1 - blockIdx.x) * a.mt;   // the tiles with the most keys start first
-    const int t1 = min(t0 + a.mt, a.n) - 1;
+    const int t1 = min(t0 + a.mt, a.q_len) - 1;           // this CTA's queries t0 .. t1, at positions i0 .. i1
+    const int i0 = a.q_off + t0, i1 = a.q_off + t1;
     const int s_b = a.kv_start ? min(max(__ldg(a.kv_start + b), 0), a.n) : 0;
     auto lo_of = [&](int i) { return max(s_b, a.window > 0 ? i - a.window + 1 : 0); };
 
-    // keys any row of this CTA sees: [lo_of(t0), t1] (lo_of is non-decreasing in the token); none if t1 < s_b
-    const int jt0 = lo_of(t0) / kKeys;
-    const int n_tiles = t1 < s_b ? 0 : t1 / kKeys - jt0 + 1;
+    // keys any row of this CTA sees: [lo_of(i0), i1] (lo_of is non-decreasing in the position); none if i1 < s_b
+    const int jt0 = lo_of(i0) / kKeys;
+    const int n_tiles = i1 < s_b ? 0 : i1 / kKeys - jt0 + 1;
 
     const __half* kbase = a.k + (int64_t)b * a.kv_sb + (int64_t)kvh * a.kv_sh;
     const __half* vbase = a.v + (int64_t)b * a.kv_sb + (int64_t)kvh * a.kv_sh;
@@ -90,7 +102,7 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
         for (int it = 0; it < 8; ++it) {
             const int idx = tid + it * kThreads, r = idx >> 4, c = idx & 15;
             const int t = t0 + r / a.hc, hg = r % a.hc;
-            const bool ok = r < a.mt * a.hc && t < a.n && hg < nh;
+            const bool ok = r < a.mt * a.hc && t < a.q_len && hg < nh;
             const __half* src = a.q + (int64_t)b * a.q_sb + (int64_t)(kvh * a.G + h0 + (ok ? hg : 0)) * a.q_sh +
                                 (int64_t)(ok ? t : 0) * a.q_st + c * 8;
             cp16(sQ + prompt_swz(r, c), src, ok);
@@ -105,8 +117,8 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
     const int g = lane >> 2, tq = lane & 3;
     int tok[2];
     #pragma unroll
-    for (int x = 0; x < 2; ++x) tok[x] = t0 + (warp * 16 + g + 8 * x) / a.hc;
-    const int lo_max = lo_of(t1);
+    for (int x = 0; x < 2; ++x) tok[x] = i0 + (warp * 16 + g + 8 * x) / a.hc;
+    const int lo_max = lo_of(i1);
 
     float o[16][4];
     #pragma unroll
@@ -141,7 +153,7 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
         }
 
         // keys outside a row's [lo, i] -> -inf; a tile wholly inside every row's range needs no test
-        if (j * kKeys < lo_max || j * kKeys + kKeys - 1 > t0) {
+        if (j * kKeys < lo_max || j * kKeys + kKeys - 1 > i0) {
             #pragma unroll
             for (int x = 0; x < 2; ++x) {
                 const int i = tok[x], lo = lo_of(i);
@@ -205,7 +217,7 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
     }
 
     // O / l -> fp16, staged through the warp's own 16 rows of the Q tile (read only by this warp, at tile 0), then
-    // written as 16-byte rows of out [B, n, H, 128].  A row with no visible key is exactly zero.
+    // written as 16-byte rows of out [B, q_len, H, 128].  A row with no visible key is exactly zero.
     #pragma unroll
     for (int x = 0; x < 2; ++x) {
         l[x] += __shfl_xor_sync(0xffffffffu, l[x], 1);
@@ -228,11 +240,11 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
     for (int it = 0; it < 8; ++it) {
         const int idx = lane + 32 * it, r = warp * 16 + (idx >> 4), c = idx & 15;
         const int t = t0 + r / a.hc, hg = r % a.hc;
-        if (r < a.mt * a.hc && t < a.n && hg < nh) {
+        if (r < a.mt * a.hc && t < a.q_len && hg < nh) {
             uint4 w;
             asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];"
                          : "=r"(w.x), "=r"(w.y), "=r"(w.z), "=r"(w.w) : "r"(sQ + prompt_swz(r, c)) : "memory");
-            const int64_t row = ((int64_t)b * a.n + t) * a.H + (int64_t)kvh * a.G + h0 + hg;
+            const int64_t row = ((int64_t)b * a.q_len + t) * a.H + (int64_t)kvh * a.G + h0 + hg;
             *reinterpret_cast<uint4*>(a.out + row * kD + c * 8) = w;
         }
     }
@@ -242,14 +254,13 @@ __global__ void __launch_bounds__(kThreads, 2) prompt_attention_kernel(const Pro
 
 using namespace kivi;
 
-extern "C" int kivi_prompt_attention_f16(const void* q, const void* k, const void* v, void* out,
-                                         int batch, int num_heads, int num_kv_heads, int n,
-                                         int64_t q_sb, int64_t q_sh, int64_t q_st,
-                                         int64_t kv_sb, int64_t kv_sh, int64_t kv_st,
-                                         const int32_t* kv_start, int window, void* stream)
+// The queries are the last m of the n key positions (m = n: the whole prompt).  Argument errors return before any CUDA call.
+static int prompt_attention(const void* q, const void* k, const void* v, void* out, int batch, int num_heads,
+                            int num_kv_heads, int m, int n, int64_t q_sb, int64_t q_sh, int64_t q_st, int64_t kv_sb,
+                            int64_t kv_sh, int64_t kv_st, const int32_t* kv_start, int window, void* stream)
 {
     if (!q || !k || !v || !out) return KIVI_ERR_NULL;
-    if (batch <= 0 || batch > 65535 || num_heads <= 0 || n <= 0 || window < 0) return KIVI_ERR_SHAPE;
+    if (batch <= 0 || batch > 65535 || num_heads <= 0 || n <= 0 || m <= 0 || m > n || window < 0) return KIVI_ERR_SHAPE;
     if (num_kv_heads <= 0 || num_heads % num_kv_heads != 0) return KIVI_ERR_GQA;
     PromptArgs a;
     a.G = num_heads / num_kv_heads;
@@ -272,7 +283,28 @@ extern "C" int kivi_prompt_attention_f16(const void* q, const void* k, const voi
     a.q_sb = q_sb; a.q_sh = q_sh; a.q_st = q_st; a.kv_sb = kv_sb; a.kv_sh = kv_sh; a.kv_st = kv_st;
     a.kv_start = kv_start;
     a.H = num_heads; a.n = n; a.window = window;
-    const dim3 grid((unsigned)((n + a.mt - 1) / a.mt), (unsigned)(num_kv_heads * a.chunks), (unsigned)batch);
+    a.q_len = m; a.q_off = n - m;
+    const dim3 grid((unsigned)((m + a.mt - 1) / a.mt), (unsigned)(num_kv_heads * a.chunks), (unsigned)batch);
     prompt_attention_kernel<<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(a);
     return post_launch();
+}
+
+extern "C" int kivi_prompt_attention_f16(const void* q, const void* k, const void* v, void* out,
+                                         int batch, int num_heads, int num_kv_heads, int n,
+                                         int64_t q_sb, int64_t q_sh, int64_t q_st,
+                                         int64_t kv_sb, int64_t kv_sh, int64_t kv_st,
+                                         const int32_t* kv_start, int window, void* stream)
+{
+    return prompt_attention(q, k, v, out, batch, num_heads, num_kv_heads, n, n, q_sb, q_sh, q_st, kv_sb, kv_sh, kv_st,
+                            kv_start, window, stream);
+}
+
+extern "C" int kivi_prompt_attention_suffix_f16(const void* q, const void* k, const void* v, void* out,
+                                                int batch, int num_heads, int num_kv_heads, int m, int n,
+                                                int64_t q_sb, int64_t q_sh, int64_t q_st,
+                                                int64_t kv_sb, int64_t kv_sh, int64_t kv_st,
+                                                const int32_t* kv_start, int window, void* stream)
+{
+    return prompt_attention(q, k, v, out, batch, num_heads, num_kv_heads, m, n, q_sb, q_sh, q_st, kv_sb, kv_sh, kv_st,
+                            kv_start, window, stream);
 }

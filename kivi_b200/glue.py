@@ -31,6 +31,8 @@ def _bind():
     _lib.bind("kivi_logits_record", i32, [vp, i32, i32, vp, vp, vp, vp, i32, vp])
     _lib.bind("kivi_token_logprobs_f32", i32, [vp, i32, i32, vp, i32, vp, vp, vp, vp])
     _lib.bind("kivi_prompt_attention_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32] + [i64] * 6 + [vp, i32, vp])
+    _lib.bind("kivi_prompt_attention_suffix_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32] + [i64] * 6 +
+              [vp, i32, vp])
     _B = True
 
 
@@ -266,12 +268,8 @@ def token_logprobs(logits, tokens, logprob, top_ids=None, top_logprobs=None):
     return logprob
 
 
-def prompt_attention(q, k, v, out, kv_start=None, window=None):
-    """Attention of a prompt over itself (kivi_prompt_attention_f16): q [B, H, n, 128], k / v [B, Hkv, n, 128] fp16 with
-    a contiguous head dimension -- the strided [B, heads, n, 128] views of the q / k / v projections -- and k, v of equal
-    strides; out [B, n, H, 128] fp16 contiguous.  Query i of sequence b sees the keys max(s_b, i - window + 1) <= j <= i
-    with s_b = kv_start[b] (int32 [B] on the device, clamped into [0, n]; None = 0) and window None or 0 = no window.
-    A query with no visible key gets zeros.  Returns out."""
+def _prompt_operands(q, k, v, out, kv_start):
+    """The checks and strides shared by the prompt-attention entries -> (B, H, Hkv, m, n, q strides, k / v strides)."""
     _bind()
     _lib.require_cuda(q, k, v, out, kv_start)
     for name, t in (("q", q), ("k", k), ("v", v)):
@@ -280,22 +278,48 @@ def prompt_attention(q, k, v, out, kv_start=None, window=None):
         if t.dim() != 4 or t.shape[-1] != 128 or t.stride(-1) != 1:
             raise ValueError(f"{name}: expected [B, heads, n, 128] with a contiguous last dimension, got shape "
                              f"{tuple(t.shape)}, strides {t.stride()}")
-    B, H, n, _ = q.shape
-    Hkv = k.shape[1]
+    B, H, m, _ = q.shape
+    Hkv, n = k.shape[1], k.shape[2]
     if k.shape != (B, Hkv, n, 128) or v.shape != k.shape:
-        raise ValueError(f"k, v: expected [{B}, Hkv, {n}, 128] each, got {tuple(k.shape)}, {tuple(v.shape)}")
+        raise ValueError(f"k, v: expected [{B}, Hkv, n, 128] each, got {tuple(k.shape)}, {tuple(v.shape)}")
     # the stride of a dimension of size 1 is never used (its index is 0): 0, so that views differing there agree
     q_str, k_str, v_str = ([0 if t.shape[i] == 1 else t.stride(i) for i in range(3)] for t in (q, k, v))
     if v_str != k_str:
         raise ValueError(f"k, v: expected equal strides, got {k.stride()}, {v.stride()}")
-    _check("out", out, torch.float16, (B, n, H, 128))
+    _check("out", out, torch.float16, (B, m, H, 128))
     if kv_start is not None:
         _check("kv_start", kv_start, torch.int32, (B,))
     for name, t in (("k", k), ("v", v), ("out", out), ("kv_start", kv_start)):
         if t is not None and t.device != q.device:
             raise ValueError(f"{name}: on {t.device}, q on {q.device}")
+    return B, H, Hkv, m, n, q_str, k_str
+
+
+def prompt_attention(q, k, v, out, kv_start=None, window=None):
+    """Attention of a prompt over itself (kivi_prompt_attention_f16): q [B, H, n, 128], k / v [B, Hkv, n, 128] fp16 with
+    a contiguous head dimension -- the strided [B, heads, n, 128] views of the q / k / v projections -- and k, v of equal
+    strides; out [B, n, H, 128] fp16 contiguous.  Query i of sequence b sees the keys max(s_b, i - window + 1) <= j <= i
+    with s_b = kv_start[b] (int32 [B] on the device, clamped into [0, n]; None = 0) and window None or 0 = no window.
+    A query with no visible key gets zeros.  Returns out."""
+    B, H, Hkv, m, n, q_str, k_str = _prompt_operands(q, k, v, out, kv_start)
+    if m != n:
+        raise ValueError(f"q: expected {n} tokens, as k and v, got {m} (prompt_attention_suffix takes fewer)")
     _lib.check(_lib.lib().kivi_prompt_attention_f16(
         q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, H, Hkv, n, *q_str, *k_str,
         kv_start.data_ptr() if kv_start is not None else None, int(window or 0), _lib.stream_ptr(q.device)),
         "kivi_prompt_attention_f16")
+    return out
+
+
+def prompt_attention_suffix(q, k, v, out, kv_start=None, window=None):
+    """The last m tokens of a prompt over the whole prompt (kivi_prompt_attention_suffix_f16): q [B, H, m, 128] holds the
+    queries at positions n - m .. n - 1 of k / v [B, Hkv, n, 128]; out [B, m, H, 128].  Layouts, kv_start and window as
+    prompt_attention, whose rows n - m .. n - 1 this returns bit for bit.  1 <= m <= n.  Returns out."""
+    B, H, Hkv, m, n, q_str, k_str = _prompt_operands(q, k, v, out, kv_start)
+    if not 1 <= m <= n:
+        raise ValueError(f"q: expected 1 <= m <= n = {n} tokens, got {m}")
+    _lib.check(_lib.lib().kivi_prompt_attention_suffix_f16(
+        q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, H, Hkv, m, n, *q_str, *k_str,
+        kv_start.data_ptr() if kv_start is not None else None, int(window or 0), _lib.stream_ptr(q.device)),
+        "kivi_prompt_attention_suffix_f16")
     return out

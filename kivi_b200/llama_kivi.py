@@ -20,7 +20,7 @@ from __future__ import annotations
 
 import math
 from types import SimpleNamespace
-from typing import NamedTuple
+from typing import Callable, NamedTuple
 
 import torch
 import torch.nn as nn
@@ -251,6 +251,15 @@ class PromptMask(NamedTuple):
     window: int
 
 
+class PrefixMask(NamedTuple):
+    """The mask of a prompt pass over tokens r .. n-1 of a prompt whose K / V at positions 0 .. r-1 are stored
+    (LlamaForCausalLM_KIVI.insert with a PrefixCache).  Each layer places its suffix K / V after the prefix's in one
+    [1, Hkv, n, 128] buffer (`extend`(layer, k, v) -> (k, v)), runs kivi_prompt_attention_suffix_f16 on it with `mask`
+    (query t at position r + t) and stores that buffer."""
+    mask: PromptMask
+    extend: Callable
+
+
 class LlamaFlashAttention_KIVI(nn.Module):
     """Attention layer of the reference (models/llama_kivi.py:264-466), KIVI ops on libkivi_b200."""
 
@@ -297,7 +306,8 @@ class LlamaFlashAttention_KIVI(nn.Module):
         B, H, n, D = q.shape
         if isinstance(attention_mask, PromptMask):
             out = torch.empty((B, n, H, D), dtype=q.dtype, device=q.device)
-            glue.prompt_attention(q, k, v, out, attention_mask.kv_start, attention_mask.window)
+            run = glue.prompt_attention if k.shape[2] == n else glue.prompt_attention_suffix     # a stored prefix
+            run(q, k, v, out, attention_mask.kv_start, attention_mask.window)
             return out.view(B, n, H * D)
         kk, vv = repeat_kv(k, self.num_key_value_groups), repeat_kv(v, self.num_key_value_groups)
         if attention_mask is None:
@@ -308,7 +318,10 @@ class LlamaFlashAttention_KIVI(nn.Module):
 
     def _prompt_core(self, q, k, v, attention_mask, store_kv):
         """The prompt pass between the projections and o_proj: attention ([B, q_len, H * D]) and the 9-tuple, or
-        store_kv(layer, k, v) and None."""
+        store_kv(layer, k, v) and None.  With a PrefixMask, k and v first take the stored prefix in front."""
+        if isinstance(attention_mask, PrefixMask):
+            k, v = attention_mask.extend(self.layer_idx, k, v)
+            attention_mask = attention_mask.mask
         attn_output = self._prompt_attention(q, k, v, attention_mask)
         if store_kv is None:
             return attn_output, kivi_prefill_tuple(k, v, self.group_size, self.k_bits, self.v_bits, self.residual_length)
@@ -321,7 +334,7 @@ class LlamaFlashAttention_KIVI(nn.Module):
         store_kv: with a prompt pass, a callable store_kv(layer, k, v) that takes the rotated K and V [B, Hkv, q_len, D] in
         place of the 9-tuple (the fused cache: KiviCache.prefill, or a refill of one slot); the pass then returns None.
         attention_mask: None or additive [B, 1, q_len, kv_len] (models/llama_kivi.py:364-372); in a prompt pass also a
-        PromptMask."""
+        PromptMask or a PrefixMask."""
         bsz, q_len, _ = hidden_states.shape
         q, k, v = self._qkv(hidden_states, cos, sin)
         if past_key_value is not None:                                      # reference 9-tuple, decode
@@ -1029,27 +1042,74 @@ class LlamaForCausalLM_KIVI(nn.Module):
         return h
 
     @torch.no_grad()
-    def insert(self, seq: int, prompt_ids):
+    def insert(self, seq: int, prompt_ids, prefix_cache=None):
         """Start a new sequence in slot `seq` of the running batch (continuous batching): a B = 1 prompt pass at positions
         0 .. n-1 whose K/V go into that slot right-aligned to the shared length T (KiviCache.refill), then
         kv_start[seq] = T - n and the slot's position = n.  The other slots are not touched.  Returns the prompt's
-        last-position logits [vocab] fp32; the caller writes the first token into the slot's input (`_ids[seq]`)."""
+        last-position logits [vocab] fp32; the caller writes the first token into the slot's input (`_ids[seq]`).
+        prefix_cache: a kivi_b200.prefix.PrefixCache.  When it holds the prompt's first r >= MIN_REUSE tokens (r <= n - 1,
+        prefix.reuse_length), the pass runs on tokens r .. n-1 only, at positions r .. n-1, over the stored K / V and
+        its own (PrefixMask); otherwise it runs the whole prompt as without a cache.  Either way the prompt's tokens past
+        the stored path are stored."""
         assert self.cache is not None, "call init_cache() / prefill() first"
         ids = torch.as_tensor(prompt_ids, device=self.cache.device).reshape(1, -1)
         n, T = ids.shape[1], self.cache.kv_len
         if not 1 <= n <= T:
             raise ValueError(f"a prompt of {n} tokens does not fit the shared length {T} (1 <= n <= length)")
-        positions = torch.arange(n, device=ids.device).unsqueeze(0)
+        r, store = 0, lambda layer, k, v: self.cache.refill(layer, seq, k, v)       # noqa: E731
+        if prefix_cache is not None:
+            r, store, record = self._prefix_insert(prefix_cache, ids, store)
+        positions = torch.arange(r, n, device=ids.device).unsqueeze(0)
         mask = self._kernel_mask(None, n, ids.device)
-        if mask is None:
+        if r:
+            mask = PrefixMask(PromptMask(None, 0) if mask is None else mask,
+                              self._prefix_extend(prefix_cache, record[1], r, n))
+        elif mask is None:
             mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, ids.device, self.sliding_window)
-        h, _ = self._run_layers(ids, positions, None, mask,
-                                store_kv=lambda layer, k, v: self.cache.refill(layer, seq, k, v))
+        h, _ = self._run_layers(ids[:, r:], positions, None, mask, store_kv=store)
+        if prefix_cache is not None:
+            prefix_cache.insert(*record)
         self._pos[seq] = n
         self.cache.set_seq_start(seq, T - n)
         if self._processing:
             self._mark_prompt(ids, None, slice(seq, seq + 1))
         return self.lm_head(h[0, -1]).float()
+
+    def _prefix_insert(self, prefix_cache, ids, refill):
+        """insert()'s use of a PrefixCache: bind it, find the prompt's stored prefix and reserve room for the rest.
+        Returns r (the tokens to reuse, 0 for none), the store_kv that refills the slot and copies the new tokens' K / V
+        into the reserved storage, and the arguments of prefix_cache.insert once the pass is done."""
+        from .prefix import reuse_length
+        a = self.model.layers[0].self_attn
+        prefix_cache.bind(self, len(self.model.layers), a.num_key_value_heads, ids.device)
+        tokens = ids[0].tolist()
+        n = len(tokens)
+        match = prefix_cache.match(tokens)
+        r = reuse_length(match.length, n)
+        if r:
+            prefix_cache.hits += 1
+            prefix_cache.reused_tokens += r
+        storage = prefix_cache.reserve(match, n - match.length)
+        store = refill
+        if storage is not None:
+            def store(layer, k, v):
+                storage[layer, 0].copy_(k[0, :, match.length:])
+                storage[layer, 1].copy_(v[0, :, match.length:])
+                refill(layer, k, v)
+        return r, store, (tokens, match, storage)
+
+    @staticmethod
+    def _prefix_extend(prefix_cache, match, r: int, n: int):
+        """PrefixMask.extend of an insert that reuses r stored tokens of an n-token prompt: per layer, a fresh
+        [1, Hkv, n, 128] K and V holding the stored prefix, then the suffix's k / v [1, Hkv, n - r, 128]."""
+        def extend(layer, k, v):
+            kk = k.new_empty((1, k.shape[1], n, k.shape[3]))
+            vv = torch.empty_like(kk)
+            prefix_cache.copy_prefix(match, r, layer, kk[0], vv[0])
+            kk[:, :, r:].copy_(k)
+            vv[:, :, r:].copy_(v)
+            return kk, vv
+        return extend
 
     def release(self, seq: int):
         """Make slot `seq` idle (KiviCache.release): it keeps its row of every step but reads no cached byte."""

@@ -10,6 +10,7 @@ the sampling kernel of the step reads each slot's parameters on the device, so b
 A request may also carry a repetition, presence and frequency penalty and a minimum number of new tokens (logits processing
 inside the step, LlamaForCausalLM_KIVI.set_processing), read per slot on the device in the same way, and ask for the
 log-probabilities of its tokens (`logprobs`, LlamaForCausalLM_KIVI.set_logprobs), computed inside the step as well.
+With a PrefixCache (kivi_b200.prefix), an insert whose prompt starts with a stored prefix computes only the rest.
 """
 from __future__ import annotations
 
@@ -120,7 +121,7 @@ def plan_admission(T: int, tv: int, max_tokens: int, quantum: int, live_starts, 
 
 @torch.no_grad()
 def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_graph: bool = True,
-          stats: dict | None = None):
+          stats: dict | None = None, prefix_cache=None):
     """Decoding of a stream of requests with `batch` slots on one cache of `max_tokens` positions.
     requests: a list of (prompt ids 1-D, max_new_tokens), greedy, or (prompt ids, max_new_tokens, params), sampled on the
     device with params = a dict of temperature, top_k, top_p, seed, and of the logits-processing keys repetition_penalty,
@@ -138,7 +139,12 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     later prompt fits under the shared length.  Each step is one decode_step (its CUDA graph is captured once: the batch
     is ragged from the start) and one device-to-host read of the sampled ids; finished slots are released and refilled
     from the queue in order.  stats: an optional dict that receives counters (steps, slot_steps = live slots summed over
-    the steps, inserts, shifts, shifted_tokens, prefills)."""
+    the steps, inserts, shifts, shifted_tokens, prefills, prefix_hits, prefix_tokens).
+    prefix_cache: a kivi_b200.prefix.PrefixCache, or None.  Every insert reuses the longest prefix of its prompt stored
+    there (of at least prefix.MIN_REUSE tokens) and stores the rest of its prompt; stats counts the inserts that reused
+    one (prefix_hits) and their reused tokens (prefix_tokens).  The caller owns the cache, so it may outlive the call
+    (the next turn of a conversation starts with the previous prompt).  The first group's left-padded prefill neither
+    uses nor fills it."""
     reqs, params = parse_requests(requests)
     if not reqs:
         return
@@ -156,7 +162,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
                              f"({max_tokens})")
     if stats is None:
         stats = {}
-    for key in ("steps", "slot_steps", "inserts", "shifts", "shifted_tokens", "prefills"):
+    for key in ("steps", "slot_steps", "inserts", "shifts", "shifted_tokens", "prefills", "prefix_hits", "prefix_tokens"):
         stats.setdefault(key, 0)
     cache = model.cache
     if cache is None or cache.batch != batch or cache.max_tokens != max_tokens:
@@ -271,7 +277,12 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
                         stats["shifts"] += 1
                         stats["shifted_tokens"] += plan[0]
                     i = queue.popleft()
-                    tok = first_token(model.insert(slot, p.to(dev)), slot, i)
+                    if prefix_cache is not None:
+                        hits, reused = prefix_cache.hits, prefix_cache.reused_tokens
+                    tok = first_token(model.insert(slot, p.to(dev), prefix_cache), slot, i)
+                    if prefix_cache is not None:
+                        stats["prefix_hits"] += prefix_cache.hits - hits
+                        stats["prefix_tokens"] += prefix_cache.reused_tokens - reused
                     tok = read(tok.view(1).expand(batch))[0] if want_lp else int(tok)
                     model._ids[slot] = tok
                     owner[slot] = i
