@@ -137,9 +137,13 @@ int kivi_unpack_dequant_lastdim_f16(const void* code, const void* scale, const v
  * touching q / k_new.  Without the flag the q.K^T kernel is an ordinary launch (safe directly after
  * kivi_cache_advance / kivi_cache_prefill_f16 / a previous attention call on the same cache). */
 #define KIVI_CACHE_OVERLAP_PROLOGUE 1
-/* Bits 4..6 of kivi_cache_t.flags: how many query heads of a KV head share one work unit of the decode attention
- * (their MMAs and every packed byte): 0 = chosen from the geometry (4 if nh/nh_kv % 4 == 0, else 2, else 1), or an
- * explicit 1 / 2 / 4 dividing nh/nh_kv.  kivi_decode_workspace_bytes and kivi_decode_attention_f16 must see the same value. */
+/* Bits 4..6 of kivi_cache_t.flags: how many query heads G of a KV head share one work unit of the decode attention
+ * (their MMAs and every packed byte).  The ratio = nh/nh_kv query heads of a KV head form ceil(ratio / G) units, each of
+ * which streams all of the KV head's packed blocks.  0 = chosen from the geometry: the largest G in {1, 2, 4} that divides
+ * the ratio, except that odd ratios above 2 take 4 (ratio 1 -> 1, 2 -> 2, 3 -> 4, 4 -> 4, 5 -> 4, 6 -> 2, 7 -> 4, 8 -> 4);
+ * or an explicit 1 / 2 / 4, whether or not it divides the ratio.
+ * When it does not, the last unit of a KV head serves fewer than G heads: its missing heads compute on q = 0 and write
+ * nothing.  kivi_decode_workspace_bytes and kivi_decode_attention_f16 must see the same value. */
 #define KIVI_CACHE_GQA_CHUNK_SHIFT 4
 #define KIVI_CACHE_GQA_CHUNK(g)    ((g) << KIVI_CACHE_GQA_CHUNK_SHIFT)
 
@@ -262,6 +266,12 @@ int kivi_debug_ragged_items(int n_units, int n_b, int n_w, int w_cap, int kernel
  * window item i).  unit_start: NULL (no padding) or the kv_start of every unit's sequence. */
 int kivi_debug_window_items(int n_units, int n_b, int n_w, int w_cap, int kernel, const int* unit_start, int T, int window,
                             int* issued, int* consumed, int64_t cap, int64_t* n_out);
+
+/* Test hook: the work-unit geometry of the decode attention for GQA ratio `ratio` (>= 1) and kivi_cache_t.flags `flags`,
+ * evaluated on the host with the code the entries use (KIVI_CACHE_GQA_CHUNK above).  Returns G, the query heads per work
+ * unit, and stores ceil(ratio / G), the work units per KV head, in *hchunks; KIVI_ERR_SHAPE for ratio < 1 or a NULL
+ * hchunks. */
+int kivi_debug_gqa_chunk(int ratio, int flags, int* hchunks);
 
 /* Advance `state` by one token (the bookkeeping of :343-356, :386-399); once per step, all layers. */
 int kivi_cache_advance(const kivi_cache_t* cache, void* stream);

@@ -224,8 +224,8 @@ static inline int timeline_fetch(unsigned long long* host_out) {
 #endif
 
 struct Workspace {                     // carved from the caller's buffer (kivi_decode_workspace_bytes)
-    __half* lg; long long ld;          // [B*H][ld] scaled logits (fp16), ld % 128 == 0
-    float2* stats; int stat_cap;       // [B*H][stat_cap] (max, sum exp(x - max)) per qk item
+    __half* lg; long long ld;          // [n_units*G][ld] scaled logits (fp16), row unit * G + h; ld % 128 == 0
+    float2* stats; int stat_cap;       // [n_units*G][stat_cap] (max, sum exp(x - max)) per qk item
     float* part; int part_cap;         // [n_units][part_cap][G][2][128] partial outputs (packed | window)
     int* count;                        // [n_units] arrivals of sv ranges; the last arriver resets it to 0
     int* ready;                        // [n_units] q.K^T ranges of the unit that have published logits + statistics (reset by the finaliser)
@@ -243,6 +243,22 @@ struct AttnParams {
     int max_kv_len;                     // what the workspace rows were sized for
     int window;                         // sliding window W (RAGGED kernels): positions below T - W are invisible; 0 = none
 };
+
+// Query heads of a KV head, ratio = H / Hkv, are served in hchunks = ceil(ratio / G) chunks of G (work units); lane head h
+// of chunk hc is query head hc * G + h of the KV head.  When G does not divide the ratio the last chunk holds fewer real
+// heads.  Its missing ("ghost") heads load q = 0 and take part in the MMAs like the others (the MMA columns of one head never
+// mix into another's), but write nothing the caller sees: no output row, no dbg_logits / dbg_probs row.  The workspace rows
+// of logits and statistics are numbered by (unit, lane head) = unit * G + h, so a ghost head has rows of its own and the
+// kernels' hot loops need no test for it; when G divides the ratio that number is the query head's (u * ratio + hc * G + h).
+__device__ __forceinline__ int chunk_heads(int G, int ratio, int hc) { return min(G, ratio - hc * G); }
+// the first query head of work unit `un` (rows of q, out and the debug outputs)
+__device__ __forceinline__ int unit_head0(int G, int ratio, int hchunks, int un) {
+    return hchunks == 1 ? un * ratio : (un / hchunks) * ratio + (un % hchunks) * G;
+}
+// the real heads of work unit `un`
+__device__ __forceinline__ int unit_heads(int G, int ratio, int hchunks, int un) {
+    return G == 1 ? 1 : chunk_heads(G, ratio, hchunks == 1 ? 0 : un % hchunks);
+}
 
 // ------------------------------------------------------------------------------------------------
 // Sliding window (kivi_decode_attention_window_f16).  With T the shared length including the new token, sequence b sees the
@@ -999,12 +1015,15 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     uint2 qf[G], ql[G];
     auto fetch_q = [&](int un) {
         const int u_ = p.hchunks == 1 ? un : un / p.hchunks, hc_ = p.hchunks == 1 ? 0 : un % p.hchunks;
-        const int row0 = u_ * ratio + hc_ * G;
+        const int row0 = u_ * ratio + hc_ * G, nh_ = chunk_heads(G, ratio, hc_);
         #pragma unroll
         for (int h = 0; h < G; ++h) {
-            const uint32_t* qh = reinterpret_cast<const uint32_t*>(p.q + (int64_t)(row0 + h) * kD + 16 * (lane >> 2) + 2 * (lane & 3));
-            qf[h] = make_uint2(__ldg(qh), __ldg(qh + 4));
-            ql[h] = __ldg(reinterpret_cast<const uint2*>(p.q + (int64_t)(row0 + h) * kD) + lane);
+            qf[h] = make_uint2(0u, 0u); ql[h] = qf[h];                       // a ghost head: q = 0
+            if (G == 1 || h < nh_) {
+                const uint32_t* qh = reinterpret_cast<const uint32_t*>(p.q + (int64_t)(row0 + h) * kD + 16 * (lane >> 2) + 2 * (lane & 3));
+                qf[h] = make_uint2(__ldg(qh), __ldg(qh + 4));
+                ql[h] = __ldg(reinterpret_cast<const uint2*>(p.q + (int64_t)(row0 + h) * kD) + lane);
+            }
         }
     };
     pdl_wait();                                                              // q / k_new come from the previous kernel of the stream
@@ -1014,9 +1033,12 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
     KIVI_TL(0, gw, 1);
     #pragma unroll 1
     while (left > 0) {
-        const int u = p.hchunks == 1 ? unit : unit / p.hchunks, hc = p.hchunks == 1 ? 0 : unit % p.hchunks;
+        const int u = p.hchunks == 1 ? unit : unit / p.hchunks;
         const int b = u / c.Hkv;
-        const int uq0 = u * ratio + hc * G;
+        const int wq0 = unit * G;                                            // first workspace row (logits, statistics)
+        // debug rows: the unit's first query head and its real heads, evaluated where they are written (cold)
+        auto uq0 = [&]() { return unit_head0(G, ratio, p.hchunks, unit); };
+        auto nreal = [&]() { return unit_heads(G, ratio, p.hchunks, unit); };
         const int j_first = j;
         const int n_here = min(left, s.ipu - j);                             // this warp's pseudo-blocks of this unit
         const int start = RAGGED ? unit_start(p, s, unit) : 0;              // positions below it are padding
@@ -1091,8 +1113,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     for (int grp = 0; grp < NG; ++grp) zsel[grp] *= dn;
                     post *= pow2f(kshift);
                 }
-                const int64_t rowi = uq0 + h_l;
-                __half* row = p.w.lg + rowi * p.w.ld + jb * kBlockTokens;
+                __half* row = p.w.lg + (int64_t)(wq0 + h_l) * p.w.ld + jb * kBlockTokens;
                 const int nvalid = s.tk - jb * kBlockTokens;                 // < 128 only in the last block when R < 128
                 const bool padded = RAGGED && jb * kBlockTokens < start;     // partly hidden: the masking epilogue
                 // the lane's logits by compile-time slot; slots of MMAs this lane does not own and tokens past the packed
@@ -1113,7 +1134,8 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                             __half hv = scale_logit(v);                      // fp16 scaled (+ mask): the softmax input
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + jb * kBlockTokens + o);
                             row[o] = hv;
-                            if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + jb * kBlockTokens + o] = hv;
+                            if (p.dbg_logits && h_l < nreal())
+                                p.dbg_logits[(int64_t)(uq0() + h_l) * p.dbg_stride + jb * kBlockTokens + o] = hv;
                             if (!padded || jb * kBlockTokens + o >= start) x[slot] = __half2float(hv);   // hidden: no value
                         }
                     });
@@ -1142,7 +1164,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 qk_issue_next<KB, GS, RAGGED>(pp, cur, p, s, j0.k, lane, pol);
                 // lane (g8 < G, t): head g8, tokens 2t, 2t+1 (tile 0) and 8+2t, 9+2t (tile 1)
                 if (g8 < G) {
-                    const int64_t rowi = uq0 + g8;
+                    const int64_t rowi = wq0 + g8;
                     float x[4];
                     #pragma unroll
                     for (int e = 0; e < 4; ++e) {
@@ -1152,7 +1174,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                             __half hv = scale_logit((e < 2 ? d0[e] : d1[e - 2]) * qpost_win);
                             if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + s.tk + t0 + t);
                             p.w.lg[rowi * p.w.ld + s.tk + t0 + t] = hv;
-                            if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + s.tk + t0 + t] = hv;
+                            if (p.dbg_logits && g8 < nreal()) p.dbg_logits[(int64_t)(uq0() + g8) * p.dbg_stride + s.tk + t0 + t] = hv;
                             if (!RAGGED || s.tk + t0 + t >= start) x[e] = __half2float(hv);   // padding: no value
                         }
                     }
@@ -1170,10 +1192,9 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     sum = warp_sum(sum);
                     if (lane == 4 * h) {                                     // the lane that keeps head h's window statistics
                         __half hv = scale_logit(sum);
-                        const int64_t rowi = uq0 + h;
                         if (p.mask) hv = apply_mask(hv, p.mask, (int64_t)b * s.T + s.T - 1);
-                        p.w.lg[rowi * p.w.ld + s.T - 1] = hv;
-                        if (p.dbg_logits) p.dbg_logits[rowi * p.dbg_stride + s.T - 1] = hv;
+                        p.w.lg[(int64_t)(wq0 + h) * p.w.ld + s.T - 1] = hv;
+                        if (p.dbg_logits && h < nreal()) p.dbg_logits[(int64_t)(uq0() + h) * p.dbg_stride + s.T - 1] = hv;
                         const float x1[1] = {__half2float(hv)};
                         fold_stats(m_win, s_win, x1);
                     }
@@ -1194,7 +1215,7 @@ qk_kernel(const KIVI_PARAM_QUAL AttnParams p)
             }
             float M, S;
             warp_max_sum(m, sm, M, S);
-            if (lane == 0) p.w.stats[(int64_t)(uq0 + h) * p.w.stat_cap + (gw - w_first)] = make_float2(M, S);
+            if (lane == 0) p.w.stats[(int64_t)(wq0 + h) * p.w.stat_cap + (gw - w_first)] = make_float2(M, S);
         }
 #if KIVI_UNIT_FLAGS
         // publish: this range's logits (all lanes) and statistics of the unit happen-before the counter increment
@@ -1277,7 +1298,7 @@ __device__ __forceinline__ void wait_unit_ready(const AttnParams& p, const Sched
 
 template <int VB, int G, int GS, bool RAGGED>
 __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnParams& p, const Sched& s, int j0,
-                                              int ratio, int lane, uint64_t pol, const Ranges<CostQK>& rq, int& ready_unit)
+                                              int lane, uint64_t pol, const Ranges<CostQK>& rq, int& ready_unit)
 {
     const CacheDesc& c = p.c;
     if constexpr (RAGGED) {
@@ -1290,7 +1311,7 @@ __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnP
     }
     if (cur.unit != ready_unit) { wait_unit_ready(p, s, rq, cur.unit, lane); ready_unit = cur.unit; }
     if (lane == 0) {
-        const int u = p.hchunks == 1 ? cur.unit : cur.unit / p.hchunks, hc = p.hchunks == 1 ? 0 : cur.unit % p.hchunks;
+        const int u = p.hchunks == 1 ? cur.unit : cur.unit / p.hchunks;
         uint8_t* dst = pp.prod();
         uint64_t* bar = pp.prod_bar();
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -1305,10 +1326,10 @@ __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnP
                 bulk_g2s(dst, blk + cur.half * cb, cb, bar, pol);
                 bulk_g2s(dst + cb, blk + kParts * cb + cur.half * mb, (uint32_t)mb, bar, pol);
             }
-            const int uq0 = u * ratio + hc * G;
+            const int wq0 = cur.unit * G;
             for (int h = 0; h < G; ++h)                               // the logits of the item's tokens (workspace rows)
                 bulk_g2s(dst + cb + mb + h * kPartTokens * 2,
-                         p.w.lg + (int64_t)(uq0 + h) * p.w.ld + (cur.j + j0) * kBlockTokens + cur.half * kPartTokens,
+                         p.w.lg + (int64_t)(wq0 + h) * p.w.ld + (cur.j + j0) * kBlockTokens + cur.half * kPartTokens,
                          kPartTokens * 2, bar, pol);
         } else {
             const int i = cur.j - s.n_vb;
@@ -1321,9 +1342,9 @@ __device__ __forceinline__ void sv_issue_next(Pipe& pp, Cursor& cur, const AttnP
                 mbar_expect_tx(bar, (uint32_t)(nt * kD * 2 + G * 48));
                 bulk_g2s(dst, c.v_res + ((int64_t)u * c.v_res_cap + slot0) * kD, (uint32_t)(nt * kD * 2), bar, pol);
                 const int l0 = i < s.vr1 ? i * kResTile : s.seg1 + (i - s.vr1) * kResTile;
-                const int uq0 = u * ratio + hc * G;
+                const int wq0 = cur.unit * G;
                 for (int h = 0; h < G; ++h) {
-                    const int64_t e0 = ((int64_t)(uq0 + h) * p.w.ld + s.tv + l0) & ~(int64_t)7;
+                    const int64_t e0 = ((int64_t)(wq0 + h) * p.w.ld + s.tv + l0) & ~(int64_t)7;
                     bulk_g2s(dst + kResBytes + h * 64, p.w.lg + e0, 48u, bar, pol);
                 }
             } else {
@@ -1379,6 +1400,9 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
     rg.lo(gw, u_lo, j_lo); rg.lo(gw + 1, u_hi, j_hi);
     const int n_mine = (u_hi - u_lo) * s.bpu + (j_hi - j_lo);
     const int ratio = c.H / c.Hkv;
+    // real heads of work unit `un`: evaluated in the debug and output paths only (a register held across the block loop
+    // would spill the G = 4 kernels)
+    auto heads_of = [&](int un) { return unit_heads(G, ratio, p.hchunks, un); };
     Pipe pp;
     pp.init(smem + (size_t)warp * p.spw * p.stage_bytes, full_all + warp * p.spw, p.spw, p.stage_bytes);
     Cursor cur;
@@ -1425,8 +1449,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
     float2 sn[G];
     int nstat = 0;
     auto fetch_stats = [&](int un) {
-        const int u_ = p.hchunks == 1 ? un : un / p.hchunks, hc_ = p.hchunks == 1 ? 0 : un % p.hchunks;
-        const int row0 = u_ * ratio + hc_ * G;
+        const int row0 = un * G;                                             // the unit's workspace rows
         nstat = rq.owner(un, s.ipu - 1) - rq.owner(un, 0) + 1;
         if (un != ready_unit) { wait_unit_ready(p, s, rq, un, lane); ready_unit = un; }
         #pragma unroll
@@ -1458,7 +1481,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         }
         pp.push();
     }
-    for (int i = commit_async ? 1 : 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
+    for (int i = commit_async ? 1 : 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, lane, pol, rq, ready_unit);
     KIVI_TL(1, gw, 1);
     if (commit_async) {
         pp.wait();
@@ -1470,12 +1493,12 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         if (s.L + 1 > c.R) in.vold = *reinterpret_cast<const uint2*>(st + 512 + 2 * (win_off(s.vhead, lane * 4) - s.vhead * kD));
         __syncwarp();
         pp.pop();
-        sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);     // the freed stage takes the next item at once
+        sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, lane, pol, rq, ready_unit);     // the freed stage takes the next item at once
         commit_unit<KB, VB>(p, s, cu0, lane, scratch, in);
         for (int uu = cu0 + 1; uu < cu1; ++uu) commit_unit<KB, VB>(p, s, uu, lane, scratch, commit_fetch(p, s, uu, lane));
     }
 #else
-    for (int i = 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
+    for (int i = 0; i < p.spw; ++i) sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, lane, pol, rq, ready_unit);
     KIVI_TL(1, gw, 1);
 #if KIVI_EARLY_COMMIT && KIVI_COMMIT_LATE && !KIVI_COMMIT_IN_QK
     commit_share();
@@ -1501,7 +1524,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
     // The last warp to arrive for a unit adds the records in range order, rounds, writes the output, updates the cache.
     auto finish_unit = [&](int un, int nparts, const CommitIn& cin) {
         const int u = p.hchunks == 1 ? un : un / p.hchunks, hc = p.hchunks == 1 ? 0 : un % p.hchunks;
-        const int uq0 = u * ratio + hc * G;
+        const int uq0 = u * ratio + hc * G, nh_ = G == 1 ? 1 : chunk_heads(G, ratio, hc);
 #if KIVI_REL_ARRIVE
         if (nparts > 1 && lane == 0) asm volatile("fence.acq_rel.gpu;" ::: "memory");   // the last arriver acquires: the counter value it read (relaxed) + this fence
 #endif
@@ -1525,7 +1548,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 #pragma unroll
                 for (int h = 0; h < G; ++h) {
                     a[k][h] = make_float4(0.f, 0.f, 0.f, 0.f); b4[k][h] = a[k][h];
-                    if (w0 + k < nparts) {
+                    if (w0 + k < nparts && h < nh_) {                      // a ghost head's records are not read
                         a[k][h] = __ldcg(reinterpret_cast<const float4*>(r0 + (int64_t)(w0 + k) * rec + (h * 2 + 0) * kD) + lane);
                         b4[k][h] = __ldcg(reinterpret_cast<const float4*>(r0 + (int64_t)(w0 + k) * rec + (h * 2 + 1) * kD) + lane);
                     }
@@ -1540,6 +1563,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         }
         #pragma unroll
         for (int h = 0; h < G; ++h) {
+            if (h >= nh_) break;                                             // ghost heads have no output row
             __align__(8) __half o4[4];
             #pragma unroll
             for (int e = 0; e < 4; ++e) {
@@ -1557,8 +1581,8 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
     };
     #pragma unroll 1
     while (left > 0) {
-        const int u = p.hchunks == 1 ? unit : unit / p.hchunks, hc = p.hchunks == 1 ? 0 : unit % p.hchunks;
-        const int uq0 = u * ratio + hc * G;
+        const int u = p.hchunks == 1 ? unit : unit / p.hchunks;
+        auto uq0 = [&]() { return unit_head0(G, ratio, p.hchunks, unit); };   // debug rows (cold)
         const int n_here = min(left, s.bpu - j);                             // this warp's pseudo-blocks of this unit
         const int start = RAGGED ? unit_start(p, s, unit) : 0;              // positions below it are padding
 
@@ -1568,7 +1592,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
         #pragma unroll
         for (int h = 0; h < G; ++h) {
             float mx = sn[h].x, sm = sn[h].y;
-            const float2* st = p.w.stats + (int64_t)(uq0 + h) * p.w.stat_cap;
+            const float2* st = p.w.stats + (int64_t)(unit * G + h) * p.w.stat_cap;
             for (int i = lane + 32; i < nstat; i += 32) {                    // more than 32 ranges on one unit: few, long units
                 const float2 v = __ldcg(st + i);
                 const float mn = fmaxf(mx, v.x);
@@ -1662,9 +1686,9 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                                 if (t0 + tt + 1 < start) pr = __float2half2_rn(0.f);
                                 else if (t0 + tt < start) pr = __halves2half2(__float2half_rn(0.f), __high2half(pr));
                             }
-                            if (p.dbg_probs) {
-                                if (tt < nt) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + t0 + tt] = __low2half(pr);
-                                if (tt + 1 < nt) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + t0 + tt + 1] = __high2half(pr);
+                            if (p.dbg_probs && (G == 1 || h < heads_of(unit))) {
+                                if (tt < nt) p.dbg_probs[(int64_t)(uq0() + h) * p.dbg_stride + t0 + tt] = __low2half(pr);
+                                if (tt + 1 < nt) p.dbg_probs[(int64_t)(uq0() + h) * p.dbg_stride + t0 + tt + 1] = __high2half(pr);
                             }
                             pr = __hmul2(pr, f1);                            // exact
                             if (boost) pr = __hmul2(pr, f2);
@@ -1679,7 +1703,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                     }, acc, zc, lane);
                     __syncwarp();
                     pp.pop();
-                    sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
+                    sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, lane, pol, rq, ready_unit);
                 }
                 float zsel[NG];
                 gather_z<G, GS>(zc, lane, zsel);
@@ -1720,14 +1744,14 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                         float x = 0.f;
                         if (hidden) {
                         } else if (win_bulk) {
-                            const int off = (int)(((int64_t)(uq0 + h) * p.w.ld + s.tv + l0) & 7);
+                            const int off = (int)(((int64_t)(unit * G + h) * p.w.ld + s.tv + l0) & 7);
                             x = __half2float(reinterpret_cast<const __half*>(st + kResBytes + h * 64)[off + lane]);
                         } else {
-                            x = __half2float(__ldcg(p.w.lg + (int64_t)(uq0 + h) * p.w.ld + s.tv + l0 + lane));
+                            x = __half2float(__ldcg(p.w.lg + (int64_t)(unit * G + h) * p.w.ld + s.tv + l0 + lane));
                         }
                         __half pr = __float2half_rn(prob_f32(x, M[h], nMl[h], S[h], rS[h]));
                         if (hidden) pr = __float2half_rn(0.f);                   // hidden: probability 0
-                        if (p.dbg_probs) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + s.tv + l0 + lane] = pr;
+                        if (p.dbg_probs && (G == 1 || h < heads_of(unit))) p.dbg_probs[(int64_t)(uq0() + h) * p.dbg_stride + s.tv + l0 + lane] = pr;
                         pl[h] = __half2float(pr);
                     }
                 }
@@ -1760,7 +1784,7 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 }
                 __syncwarp();
                 pp.pop();
-                sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, ratio, lane, pol, rq, ready_unit);
+                sv_issue_next<VB, G, GS, RAGGED>(pp, cur, p, s, j0.v, lane, pol, rq, ready_unit);
                 // lane (g8, t): oacc[mt] = D[16mt + g8 | + 8][heads 2t, 2t+1] -> channel order through shared memory
                 #pragma unroll
                 for (int mt = 0; mt < 8; ++mt)
@@ -1783,9 +1807,9 @@ sv_kernel(const KIVI_PARAM_QUAL AttnParams p)
                 const float2 v01 = __half22float2(vh[0]), v23 = __half22float2(vh[1]);
                 #pragma unroll
                 for (int h = 0; h < G; ++h) {
-                    const float x = __half2float(__ldcg(p.w.lg + (int64_t)(uq0 + h) * p.w.ld + s.T - 1));
+                    const float x = __half2float(__ldcg(p.w.lg + (int64_t)(unit * G + h) * p.w.ld + s.T - 1));
                     const __half prh = __float2half_rn(prob_f32(x, M[h], nMl[h], S[h], rS[h]));
-                    if (p.dbg_probs && lane == 0) p.dbg_probs[(int64_t)(uq0 + h) * p.dbg_stride + s.T - 1] = prh;
+                    if (p.dbg_probs && lane == 0 && (G == 1 || h < heads_of(unit))) p.dbg_probs[(int64_t)(uq0() + h) * p.dbg_stride + s.T - 1] = prh;
                     const float pr = __half2float(prh);
                     orr[h][0] = fmaf(pr, v01.x, orr[h][0]); orr[h][1] = fmaf(pr, v01.y, orr[h][1]);
                     orr[h][2] = fmaf(pr, v23.x, orr[h][2]); orr[h][3] = fmaf(pr, v23.y, orr[h][3]);
@@ -1843,7 +1867,7 @@ static inline int64_t carve_workspace(const CacheDesc& c, int n_units, int G, in
     DeviceInfo di;
     const int drc = device_info(&di);
     if (drc) return drc < 0 ? drc : -(int64_t)drc;
-    const int64_t rows = (int64_t)c.B * c.H;
+    const int64_t rows = (int64_t)n_units * G;                              // (unit, lane head): B * H when G divides the ratio
     const int64_t ld = ((int64_t)max_kv_len + 16 + 127) / 128 * 128 + 128;
     const int bpu_max = cdiv(max_kv_len, kBlockTokens) + cdiv(c.R + 1, kResTile) + 4;
     const int warps = di.num_sms * kMaxCtasPerSm * kCW;                     // the largest CTA any instantiation launches

@@ -13,11 +13,16 @@ int attention_k4v2(AttnParams& p, int G, bool overlap_prologue, cudaStream_t st)
 using namespace kivi;
 
 // query heads of a KV head that share one unit's MMAs: from the cache geometry, or the explicit KIVI_CACHE_GQA_CHUNK
-// field of cache->flags (the same struct sizes the workspace and launches, so both always agree)
+// field of cache->flags (the same struct sizes the workspace and launches, so both always agree).  Every chunk streams
+// all of its KV head's packed blocks, so fewer chunks ceil(ratio / G) read fewer bytes.  The geometry picks the largest G
+// in {1, 2, 4} that divides the ratio, except for odd ratios above 2, which would otherwise run one head per unit: they
+// take G = 4 with a partly filled last chunk (its missing heads compute on q = 0 and write nothing).  Ratios that 2 but
+// not 4 divides (6: Qwen2.5-1.5B) keep G = 2: at B 32, T 4096 on an H100 G = 4 measured up to 10 % slower there
+// (DESIGN.md section 5), its two units per KV head leaving more of the GPU idle than the three of G = 2.
 static int gqa_chunk(int ratio, int flags) {
-    int G = ratio % 4 == 0 ? 4 : (ratio % 2 == 0 ? 2 : 1);
+    int G = ratio % 4 == 0 ? 4 : ratio % 2 == 0 ? 2 : ratio >= 3 ? 4 : 1;
     const int want = (flags >> KIVI_CACHE_GQA_CHUNK_SHIFT) & 7;
-    if ((want == 1 || want == 2 || want == 4) && ratio % want == 0) G = want;
+    if (want == 1 || want == 2 || want == 4) G = want;
     return G;
 }
 
@@ -28,7 +33,17 @@ extern "C" int64_t kivi_decode_workspace_bytes(const kivi_cache_t* cache, int ma
     if (rc) return rc;
     if (max_kv_len <= 0) return KIVI_ERR_SHAPE;
     const int ratio = c.H / c.Hkv, G = gqa_chunk(ratio, cache->flags);
-    return carve_workspace(c, c.B * c.Hkv * (ratio / G), G, max_kv_len, nullptr, nullptr);
+    return carve_workspace(c, c.B * c.Hkv * cdiv(ratio, G), G, max_kv_len, nullptr, nullptr);
+}
+
+// Test hook (tests/test_qwen2_cpu.py): the work-unit geometry of the decode attention for a GQA ratio and cache flags,
+// evaluated on the host.  Returns G (query heads per unit) and stores ceil(ratio / G) (units per KV head) in *hchunks.
+extern "C" int kivi_debug_gqa_chunk(int ratio, int flags, int* hchunks)
+{
+    if (ratio < 1 || !hchunks) return KIVI_ERR_SHAPE;
+    const int G = gqa_chunk(ratio, flags);
+    *hchunks = cdiv(ratio, G);
+    return G;
 }
 
 // all entries: kv_start == NULL and window == 0 is the unpadded call (the kernels without any padding logic)
@@ -52,7 +67,7 @@ static int decode_attention(const kivi_cache_t* cache, const void* q, const void
     const bool overlap = (cache->flags & KIVI_CACHE_OVERLAP_PROLOGUE) != 0;   // the q.K^T launch may overlap its predecessor
     const int ratio = p.c.H / p.c.Hkv;
     const int G = gqa_chunk(ratio, cache->flags);
-    p.hchunks = ratio / G;
+    p.hchunks = cdiv(ratio, G);
     p.n_units = p.c.B * p.c.Hkv * p.hchunks;
     p.max_kv_len = max_kv_len;
     const int64_t need = carve_workspace(p.c, p.n_units, G, max_kv_len, workspace, &p.w);

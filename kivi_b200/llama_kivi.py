@@ -137,6 +137,11 @@ def default_config(name: str = "llama-2-7b", **kw):
                             num_key_value_heads=40, vocab_size=32000, rope_theta=10000.0, rms_norm_eps=1e-5),
         "llama-2-70b": dict(hidden_size=8192, intermediate_size=28672, num_hidden_layers=80, num_attention_heads=64,
                             num_key_value_heads=8, vocab_size=32000, rope_theta=10000.0, rms_norm_eps=1e-5),
+        "qwen2.5-7b": dict(model_type="qwen2", hidden_size=3584, intermediate_size=18944, num_hidden_layers=28,
+                           num_attention_heads=28, num_key_value_heads=4, vocab_size=152064, rope_theta=1000000.0,
+                           rms_norm_eps=1e-6),
+        "llama-3.2-3b": dict(hidden_size=3072, intermediate_size=8192, num_hidden_layers=28, num_attention_heads=24,
+                             num_key_value_heads=8, vocab_size=128256, rope_theta=500000.0, rms_norm_eps=1e-5),
         "tiny": dict(hidden_size=256, intermediate_size=512, num_hidden_layers=2, num_attention_heads=2,
                      num_key_value_heads=2, vocab_size=512, rope_theta=10000.0, rms_norm_eps=1e-5),
     }
@@ -195,8 +200,16 @@ def rope_settings(config):
 def sliding_window(config):
     """The sliding window W of a config (config.sliding_window; None or absent = attention over the whole cache).  A
     config whose `layer_types` mixes attention kinds (per-layer windows) raises NotImplementedError; one whose layers are
-    all full attention has no window."""
+    all full attention has no window.  A Qwen2 config.json names its window next to `use_sliding_window`, which decides:
+    false means no window whatever `sliding_window` says; true puts windows on layers max_window_layers and above (as
+    transformers' Qwen2Config derives `layer_types`), so a max_window_layers between 0 and the layer count is refused."""
+    use = getattr(config, "use_sliding_window", None)
+    if use is not None and not use:
+        return None
     kinds = set(getattr(config, "layer_types", None) or ())
+    if not kinds and use:
+        n, first = config.num_hidden_layers, getattr(config, "max_window_layers", config.num_hidden_layers)
+        kinds = {"sliding_attention" if i >= first else "full_attention" for i in range(n)}
     if len(kinds) > 1:
         raise NotImplementedError(f"layer_types {sorted(kinds)}: per-layer attention kinds (sliding windows on some layers "
                                   "only) are not supported")
@@ -260,6 +273,15 @@ class PrefixMask(NamedTuple):
     extend: Callable
 
 
+def attention_biases(config):
+    """(q / k / v bias, o_proj bias) of a config: Qwen2 (model_type "qwen2") has biases on q, k and v and none on o_proj;
+    Llama and Mistral have one `attention_bias` flag for all four projections."""
+    if getattr(config, "model_type", None) == "qwen2":
+        return True, False
+    bias = bool(getattr(config, "attention_bias", False))
+    return bias, bias
+
+
 class LlamaFlashAttention_KIVI(nn.Module):
     """Attention layer of the reference (models/llama_kivi.py:264-466), KIVI ops on libkivi_b200."""
 
@@ -274,11 +296,11 @@ class LlamaFlashAttention_KIVI(nn.Module):
         self.num_key_value_groups = self.num_heads // self.num_key_value_heads
         self.k_bits, self.v_bits = config.k_bits, config.v_bits            # models/llama_kivi.py:34-38
         self.group_size, self.residual_length = config.group_size, config.residual_length
-        bias = getattr(config, "attention_bias", False)
-        self.q_proj = nn.Linear(self.hidden_size, self.num_heads * self.head_dim, bias=bias)
-        self.k_proj = nn.Linear(self.hidden_size, self.num_key_value_heads * self.head_dim, bias=bias)
-        self.v_proj = nn.Linear(self.hidden_size, self.num_key_value_heads * self.head_dim, bias=bias)
-        self.o_proj = nn.Linear(self.num_heads * self.head_dim, self.hidden_size, bias=bias)
+        qkv_bias, o_bias = attention_biases(config)
+        self.q_proj = nn.Linear(self.hidden_size, self.num_heads * self.head_dim, bias=qkv_bias)
+        self.k_proj = nn.Linear(self.hidden_size, self.num_key_value_heads * self.head_dim, bias=qkv_bias)
+        self.v_proj = nn.Linear(self.hidden_size, self.num_key_value_heads * self.head_dim, bias=qkv_bias)
+        self.o_proj = nn.Linear(self.num_heads * self.head_dim, self.hidden_size, bias=o_bias)
 
     def _qkv(self, hidden_states, cos, sin):
         bsz, q_len, _ = hidden_states.shape
@@ -688,7 +710,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
     @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, config=None, torch_dtype=torch.float16, device_map=None,
                         tensor_parallel: bool = False, **unused):
-        """Load a LOCAL Hugging Face Llama / Mistral checkpoint directory (config.json + *.safetensors or
+        """Load a LOCAL Hugging Face Llama / Mistral / Qwen2 checkpoint directory (config.json + *.safetensors or
         pytorch_model*.bin; there is no network here) into the KIVI model, as the reference's
         LlamaForCausalLM_KIVI.from_pretrained(config=...) does (example.py:22-28, mem_spd_test.py:24-31).  `config` is
         the user's config object carrying k_bits / v_bits / group_size / residual_length (models/llama_kivi.py:34-38);

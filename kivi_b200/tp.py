@@ -18,19 +18,23 @@ def check_divisible(config, world: int):
     if world < 1 or H % world or Hkv % world or inter % world:
         raise ValueError(f"tensor parallelism over {world} ranks needs num_attention_heads ({H}), num_key_value_heads "
                          f"({Hkv}) and intermediate_size ({inter}) divisible by {world}")
-    if getattr(config, "attention_bias", False) or getattr(config, "mlp_bias", False):
-        raise ValueError("tensor parallelism supports bias-free projections only (a sharded o_proj / down_proj bias "
-                         "would be added once per rank)")
+    from .llama_kivi import attention_biases
+    if attention_biases(config)[1] or getattr(config, "mlp_bias", False):
+        raise ValueError("tensor parallelism supports no o_proj / down_proj bias (a row-parallel bias would be added once "
+                         "per rank); q / k / v biases shard with their weight rows")
 
 
 def shard_of(name: str, config, rank: int, world: int):
-    """(dim, lo, hi): the slice of parameter `name` (HF Llama naming) that rank `rank` holds, or None if it is replicated."""
+    """(dim, lo, hi): the slice of parameter `name` (HF Llama naming) that rank `rank` holds, or None if it is replicated.
+    q / k / v biases (Qwen2) are column-parallel like their weights' rows."""
     hd = config.hidden_size // config.num_attention_heads
     q = config.num_attention_heads // world * hd
     kv = config.num_key_value_heads // world * hd
     inter = config.intermediate_size // world
     for suffix, dim, n in ((".self_attn.q_proj.weight", 0, q), (".self_attn.k_proj.weight", 0, kv),
-                           (".self_attn.v_proj.weight", 0, kv), (".self_attn.o_proj.weight", 1, q),
+                           (".self_attn.v_proj.weight", 0, kv), (".self_attn.q_proj.bias", 0, q),
+                           (".self_attn.k_proj.bias", 0, kv), (".self_attn.v_proj.bias", 0, kv),
+                           (".self_attn.o_proj.weight", 1, q),
                            (".mlp.gate_proj.weight", 0, inter), (".mlp.up_proj.weight", 0, inter),
                            (".mlp.down_proj.weight", 1, inter)):
         if name.endswith(suffix):
