@@ -362,7 +362,11 @@ int kivi_cache_import_f16(const kivi_cache_t* cache, int tk, int r, int tv, int 
  *   kivi_rope_split_f16  : qkv [B,(H+2Hkv)*128] -> q [B,H,128], k [B,Hkv,128] (rotary at position pos[b], int64,
  *                          clamped to the table_rows rows of the cos / sin tables [table_rows, 128]), v;
  *                          1 <= B <= 65535, table_rows >= 1
- *   kivi_silu_mul_f16    : gate_up [rows, 2*I] -> out [rows, I] = fp16(silu(gate)) * up;
+ *   kivi_qk_norm_rope_split_f16 : kivi_rope_split_f16 with a per-head RMSNorm (Qwen3's q_norm / k_norm) before the
+ *                          rotary: every q head n = fp16(q_norm_weight * fp16(x * rsqrt(mean(x^2) + eps))) over its 128
+ *                          channels (fp32 statistics), every k head likewise with k_norm_weight [128]; v is copied.
+ *                          Same requirements, plus non-NULL weights and a finite eps >= 0 (KIVI_ERR_SHAPE)
+ *   kivi_silu_mul_f16   : gate_up [rows, 2*I] -> out [rows, I] = fp16(silu(gate)) * up;
  *                          1 <= rows <= 65535, I even; gate_up and out 4-byte aligned
  * Misaligned pointers return KIVI_ERR_ALIGN before any launch.
  * ------------------------------------------------------------------------------------------ */
@@ -371,6 +375,10 @@ int kivi_add_rmsnorm_f16(const void* x, void* residual, const void* weight, void
 int kivi_rope_split_f16(const void* qkv, const void* cos_table, const void* sin_table, const void* pos,
                         void* q, void* k, void* v, int batch, int num_heads, int num_kv_heads, int table_rows,
                         void* stream);
+int kivi_qk_norm_rope_split_f16(const void* qkv, const void* cos_table, const void* sin_table, const void* pos,
+                                const void* q_norm_weight, const void* k_norm_weight, float eps,
+                                void* q, void* k, void* v, int batch, int num_heads, int num_kv_heads, int table_rows,
+                                void* stream);
 int kivi_silu_mul_f16(const void* gate_up, void* out, int rows, int intermediate, void* stream);
 
 /* ------------------------------------------------------------------------------------------

@@ -6,6 +6,7 @@
 
 #include <cooperative_groups.h>
 
+#include <cmath>
 #include <type_traits>
 
 namespace cg = cooperative_groups;
@@ -102,10 +103,14 @@ add_rmsnorm_kernel(const __half* __restrict__ x, __half* __restrict__ residual, 
 
 // qkv [B, (H + 2*Hkv) * 128] -> q [B,H,128], k [B,Hkv,128] (both rotated), v [B,Hkv,128]
 // apply_rotary_pos_emb: x*cos + rotate_half(x)*sin, each op rounded to fp16; cos/sin rows = position pos[b]
+// QK_NORM (Qwen3): each q / k head first goes through an RMSNorm over its 128 channels with the q or k weight, rounded
+// like LlamaRMSNorm / Qwen3RMSNorm: fp32 statistics, n = fp16(w * fp16(x * rsqrt(mean(x^2) + eps))); RoPE then rotates n.
+template <bool QK_NORM>
 __global__ void __launch_bounds__(64)
 rope_split_kernel(const __half* __restrict__ qkv, const __half* __restrict__ cos_t, const __half* __restrict__ sin_t,
                   const long long* __restrict__ pos, __half* __restrict__ q, __half* __restrict__ k, __half* __restrict__ v,
-                  int H, int Hkv, int table_rows)
+                  int H, int Hkv, int table_rows, const __half* __restrict__ q_norm_w, const __half* __restrict__ k_norm_w,
+                  float eps)
 {
     constexpr int D = 128;
     // the q.K^T kernel that follows is launched with programmatic serialization: let it set up and start streaming K blocks
@@ -113,7 +118,7 @@ rope_split_kernel(const __half* __restrict__ qkv, const __half* __restrict__ cos
     asm volatile("griddepcontrol.launch_dependents;");
     const int b = blockIdx.y, head = blockIdx.x, i = threadIdx.x;            // i < 64: pair (i, i + 64)
     const __half* src = qkv + ((int64_t)b * (H + 2 * Hkv) + head) * D;
-    if (head >= H + Hkv) {                                                   // v: plain copy
+    if (head >= H + Hkv) {                                                   // v: plain copy (the whole block: the barrier below is never split)
         __half* dst = v + ((int64_t)b * Hkv + head - H - Hkv) * D;
         dst[i] = src[i]; dst[i + 64] = src[i + 64];
         return;
@@ -122,7 +127,18 @@ rope_split_kernel(const __half* __restrict__ qkv, const __half* __restrict__ cos
     p = p < 0 ? 0 : (p >= table_rows ? table_rows - 1 : p);                  // never read outside the tables (the host checks the range)
     const __half c0 = cos_t[p * D + i], c1 = cos_t[p * D + i + 64];
     const __half s0 = sin_t[p * D + i], s1 = sin_t[p * D + i + 64];
-    const __half x0 = src[i], x1 = src[i + 64];
+    __half x0 = src[i], x1 = src[i + 64];
+    if constexpr (QK_NORM) {
+        __shared__ float red[2];
+        const float f0 = __half2float(x0), f1 = __half2float(x1);
+        const float ss = warp_sum(fmaf(f1, f1, f0 * f0));
+        if ((i & 31) == 0) red[i >> 5] = ss;
+        __syncthreads();
+        const float rs = rsqrtf((red[0] + red[1]) / (float)D + eps);
+        const __half* w = head < H ? q_norm_w : k_norm_w;
+        x0 = __hmul_rn(w[i], __float2half_rn(f0 * rs));
+        x1 = __hmul_rn(w[i + 64], __float2half_rn(f1 * rs));
+    }
     __half* dst = head < H ? q + ((int64_t)b * H + head) * D : k + ((int64_t)b * Hkv + head - H) * D;
     dst[i] = __hadd_rn(__hmul_rn(x0, c0), __hmul_rn(__hneg(x1), s0));       // rotate_half: (-x2, x1)
     dst[i + 64] = __hadd_rn(__hmul_rn(x1, c1), __hmul_rn(x0, s1));
@@ -966,9 +982,25 @@ extern "C" int kivi_rope_split_f16(const void* qkv, const void* cos_table, const
 {
     if (!qkv || !cos_table || !sin_table || !pos || !q || !k || !v) return KIVI_ERR_NULL;
     if (batch <= 0 || num_heads <= 0 || num_kv_heads <= 0 || batch > 65535 || table_rows <= 0) return KIVI_ERR_SHAPE;
-    rope_split_kernel<<<dim3(num_heads + 2 * num_kv_heads, batch), 64, 0, (cudaStream_t)stream>>>(
+    rope_split_kernel<false><<<dim3(num_heads + 2 * num_kv_heads, batch), 64, 0, (cudaStream_t)stream>>>(
         (const __half*)qkv, (const __half*)cos_table, (const __half*)sin_table, (const long long*)pos,
-        (__half*)q, (__half*)k, (__half*)v, num_heads, num_kv_heads, table_rows);
+        (__half*)q, (__half*)k, (__half*)v, num_heads, num_kv_heads, table_rows, nullptr, nullptr, 0.f);
+    return post_launch();
+}
+
+extern "C" int kivi_qk_norm_rope_split_f16(const void* qkv, const void* cos_table, const void* sin_table, const void* pos,
+                                           const void* q_norm_weight, const void* k_norm_weight, float eps,
+                                           void* q, void* k, void* v, int batch, int num_heads, int num_kv_heads,
+                                           int table_rows, void* stream)
+{
+    if (!qkv || !cos_table || !sin_table || !pos || !q || !k || !v || !q_norm_weight || !k_norm_weight)
+        return KIVI_ERR_NULL;
+    if (batch <= 0 || num_heads <= 0 || num_kv_heads <= 0 || batch > 65535 || table_rows <= 0) return KIVI_ERR_SHAPE;
+    if (!std::isfinite(eps) || eps < 0.f) return KIVI_ERR_SHAPE;
+    rope_split_kernel<true><<<dim3(num_heads + 2 * num_kv_heads, batch), 64, 0, (cudaStream_t)stream>>>(
+        (const __half*)qkv, (const __half*)cos_table, (const __half*)sin_table, (const long long*)pos,
+        (__half*)q, (__half*)k, (__half*)v, num_heads, num_kv_heads, table_rows, (const __half*)q_norm_weight,
+        (const __half*)k_norm_weight, eps);
     return post_launch();
 }
 

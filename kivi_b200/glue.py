@@ -6,6 +6,7 @@ before the call (ValueError, or RuntimeError for a CPU tensor)."""
 from __future__ import annotations
 
 import ctypes
+import math
 
 import torch
 
@@ -21,6 +22,8 @@ def _bind():
     vp, i32 = ctypes.c_void_p, ctypes.c_int
     _lib.bind("kivi_add_rmsnorm_f16", i32, [vp, vp, vp, vp, i32, i32, ctypes.c_float, vp])
     _lib.bind("kivi_rope_split_f16", i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp])
+    _lib.bind("kivi_qk_norm_rope_split_f16", i32,
+              [vp, vp, vp, vp, vp, vp, ctypes.c_float, vp, vp, vp, i32, i32, i32, i32, vp])
     _lib.bind("kivi_silu_mul_f16", i32, [vp, vp, i32, i32, vp])
     _lib.bind("kivi_greedy_sample_exchange_f32", i32, [vp, i32, i32, vp, vp, vp, i32, i32, vp, vp, vp])
     _lib.bind("kivi_sample_f32", i32, [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp])
@@ -89,8 +92,13 @@ def allreduce_add_rmsnorm(residual, weight, out, eps: float, ar, call: int = 0, 
     return out
 
 
-def rope_split(qkv, cos_table, sin_table, pos, q, k, v):
-    """qkv [B,(H+2Hkv)*128] -> q [B,H,128], k [B,Hkv,128] rotated at position pos[b] (int64), v [B,Hkv,128]."""
+def rope_split(qkv, cos_table, sin_table, pos, q, k, v, q_norm=None, k_norm=None, eps=None):
+    """qkv [B,(H+2Hkv)*128] -> q [B,H,128], k [B,Hkv,128] rotated at position pos[b] (int64), v [B,Hkv,128].
+    With q_norm and k_norm (fp16 [128] each, Qwen3's per-head RMSNorm weights) every q and k head is first normalised
+    over its 128 channels with epsilon `eps`, as LlamaRMSNorm rounds (kivi_qk_norm_rope_split_f16); one weight alone is a
+    ValueError."""
+    if (q_norm is None) != (k_norm is None):
+        raise ValueError("q_norm and k_norm: expected both or neither")
     _bind()
     if q.dim() != 3 or k.dim() != 3:
         raise ValueError(f"q, k: expected [B, heads, 128], got shapes {tuple(q.shape)}, {tuple(k.shape)}")
@@ -107,9 +115,22 @@ def rope_split(qkv, cos_table, sin_table, pos, q, k, v):
     _lib.require_cuda(pos)
     if pos.dtype != torch.int64 or pos.numel() != B or not pos.is_contiguous():
         raise ValueError(f"pos: expected {B} contiguous int64 positions, got {pos.dtype} of shape {tuple(pos.shape)}")
-    _lib.check(_lib.lib().kivi_rope_split_f16(qkv.data_ptr(), cos_table.data_ptr(), sin_table.data_ptr(), pos.data_ptr(),
-                                              q.data_ptr(), k.data_ptr(), v.data_ptr(), B, H, Hkv, cos_table.shape[0],
-                                              _lib.stream_ptr(qkv.device)), "kivi_rope_split_f16")
+    if q_norm is None:
+        _lib.check(_lib.lib().kivi_rope_split_f16(qkv.data_ptr(), cos_table.data_ptr(), sin_table.data_ptr(),
+                                                  pos.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), B, H, Hkv,
+                                                  cos_table.shape[0], _lib.stream_ptr(qkv.device)), "kivi_rope_split_f16")
+        return
+    _check("q_norm", q_norm, f16, (128,))
+    _check("k_norm", k_norm, f16, (128,))
+    for name, t in (("q_norm", q_norm), ("k_norm", k_norm)):
+        if t.device != qkv.device:
+            raise ValueError(f"{name}: on {t.device}, qkv on {qkv.device}")
+    if eps is None or not math.isfinite(eps) or eps < 0:
+        raise ValueError(f"eps: expected a finite number >= 0, got {eps!r}")
+    _lib.check(_lib.lib().kivi_qk_norm_rope_split_f16(
+        qkv.data_ptr(), cos_table.data_ptr(), sin_table.data_ptr(), pos.data_ptr(), q_norm.data_ptr(), k_norm.data_ptr(),
+        float(eps), q.data_ptr(), k.data_ptr(), v.data_ptr(), B, H, Hkv, cos_table.shape[0], _lib.stream_ptr(qkv.device)),
+        "kivi_qk_norm_rope_split_f16")
 
 
 def silu_mul(gate_up, out):

@@ -140,6 +140,13 @@ def default_config(name: str = "llama-2-7b", **kw):
         "qwen2.5-7b": dict(model_type="qwen2", hidden_size=3584, intermediate_size=18944, num_hidden_layers=28,
                            num_attention_heads=28, num_key_value_heads=4, vocab_size=152064, rope_theta=1000000.0,
                            rms_norm_eps=1e-6),
+        "qwen3-8b": dict(model_type="qwen3", hidden_size=4096, intermediate_size=12288, num_hidden_layers=36,
+                         num_attention_heads=32, num_key_value_heads=8, head_dim=128, vocab_size=151936,
+                         rope_theta=1000000.0, rms_norm_eps=1e-6),
+        # hidden 2560 != 32 heads x 128
+        "qwen3-4b": dict(model_type="qwen3", hidden_size=2560, intermediate_size=9728, num_hidden_layers=36,
+                         num_attention_heads=32, num_key_value_heads=8, head_dim=128, vocab_size=151936,
+                         rope_theta=1000000.0, rms_norm_eps=1e-6),
         "llama-3.2-3b": dict(hidden_size=3072, intermediate_size=8192, num_hidden_layers=28, num_attention_heads=24,
                              num_key_value_heads=8, vocab_size=128256, rope_theta=500000.0, rms_norm_eps=1e-5),
         "tiny": dict(hidden_size=256, intermediate_size=512, num_hidden_layers=2, num_attention_heads=2,
@@ -282,6 +289,18 @@ def attention_biases(config):
     return bias, bias
 
 
+def qk_norm(config):
+    """Whether the attention layers normalise every q and k head (Qwen3's q_norm / k_norm, an RMSNorm over head_dim
+    channels before RoPE)."""
+    return getattr(config, "model_type", None) == "qwen3"
+
+
+def head_dim(config):
+    """config.head_dim when the config names one (Qwen3 and Mistral-NeMo have hidden_size != heads x head_dim), else
+    hidden_size / num_attention_heads."""
+    return getattr(config, "head_dim", None) or config.hidden_size // config.num_attention_heads
+
+
 class LlamaFlashAttention_KIVI(nn.Module):
     """Attention layer of the reference (models/llama_kivi.py:264-466), KIVI ops on libkivi_b200."""
 
@@ -290,7 +309,7 @@ class LlamaFlashAttention_KIVI(nn.Module):
         self.config = config
         self.layer_idx = layer_idx
         self.hidden_size = config.hidden_size
-        self.head_dim = self.hidden_size // config.num_attention_heads
+        self.head_dim = head_dim(config)
         self.num_heads = config.num_attention_heads // tp_world              # this rank's heads (kivi_b200.tp)
         self.num_key_value_heads = config.num_key_value_heads // tp_world
         self.num_key_value_groups = self.num_heads // self.num_key_value_heads
@@ -301,12 +320,24 @@ class LlamaFlashAttention_KIVI(nn.Module):
         self.k_proj = nn.Linear(self.hidden_size, self.num_key_value_heads * self.head_dim, bias=qkv_bias)
         self.v_proj = nn.Linear(self.hidden_size, self.num_key_value_heads * self.head_dim, bias=qkv_bias)
         self.o_proj = nn.Linear(self.num_heads * self.head_dim, self.hidden_size, bias=o_bias)
+        if qk_norm(config):                                                 # Qwen3: replicated under tensor parallelism
+            self.q_norm = LlamaRMSNorm(self.head_dim, config.rms_norm_eps)
+            self.k_norm = LlamaRMSNorm(self.head_dim, config.rms_norm_eps)
+        else:
+            self.q_norm = self.k_norm = None
+
+    def _qk_normed(self, q, k):
+        """q and k [..., heads, D] through q_norm / k_norm (per head, before RoPE), when the model has them."""
+        if self.q_norm is None:
+            return q, k
+        return self.q_norm(q), self.k_norm(k)
 
     def _qkv(self, hidden_states, cos, sin):
         bsz, q_len, _ = hidden_states.shape
-        q = self.q_proj(hidden_states).view(bsz, q_len, self.num_heads, self.head_dim).transpose(1, 2)
-        k = self.k_proj(hidden_states).view(bsz, q_len, self.num_key_value_heads, self.head_dim).transpose(1, 2)
+        q = self.q_proj(hidden_states).view(bsz, q_len, self.num_heads, self.head_dim)
+        k = self.k_proj(hidden_states).view(bsz, q_len, self.num_key_value_heads, self.head_dim)
         v = self.v_proj(hidden_states).view(bsz, q_len, self.num_key_value_heads, self.head_dim).transpose(1, 2)
+        q, k = (t.transpose(1, 2) for t in self._qk_normed(q, k))
         q = q * cos + _rotate_half(q) * sin                                 # apply_rotary_pos_emb (:311)
         k = k * cos + _rotate_half(k) * sin
         return q, k, v
@@ -318,6 +349,7 @@ class LlamaFlashAttention_KIVI(nn.Module):
         q = self.q_proj(x).view(rows, self.num_heads, self.head_dim)
         k = self.k_proj(x).view(rows, self.num_key_value_heads, self.head_dim)
         v = self.v_proj(x).view(rows, self.num_key_value_heads, self.head_dim)
+        q, k = self._qk_normed(q, k)
         return q * cos + _rotate_half(q) * sin, k * cos + _rotate_half(k) * sin, v
 
     def _prompt_attention(self, q, k, v, attention_mask):
@@ -675,10 +707,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def __init__(self, config, tensor_parallel: bool = False):
         super().__init__()
-        head_dim = getattr(config, "head_dim", None)            # transformers configs carry it explicitly
-        if head_dim is not None and (head_dim != config.hidden_size // config.num_attention_heads or head_dim != 128):
-            raise NotImplementedError(f"head_dim {head_dim} (hidden_size {config.hidden_size}, {config.num_attention_heads} "
-                                      "heads): only head_dim = hidden_size / num_attention_heads = 128 is supported")
+        if getattr(config, "model_type", None) == "qwen3_moe":
+            raise NotImplementedError("model_type 'qwen3_moe': mixture-of-experts MLPs are not supported")
+        hd = getattr(config, "head_dim", None)                  # transformers configs carry it explicitly
+        if hd is not None and hd != 128:
+            raise NotImplementedError(f"head_dim {hd} (hidden_size {config.hidden_size}, {config.num_attention_heads} "
+                                      "heads): only head_dim 128 is supported")
         rope_settings(config)                                   # an unsupported RoPE type is refused here, not at the first forward
         self.sliding_window = sliding_window(config)            # per-layer windows are refused here
         self.config = config
@@ -710,7 +744,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
     @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, config=None, torch_dtype=torch.float16, device_map=None,
                         tensor_parallel: bool = False, **unused):
-        """Load a LOCAL Hugging Face Llama / Mistral / Qwen2 checkpoint directory (config.json + *.safetensors or
+        """Load a LOCAL Hugging Face Llama / Mistral / Qwen2 / Qwen3 checkpoint directory (config.json + *.safetensors or
         pytorch_model*.bin; there is no network here) into the KIVI model, as the reference's
         LlamaForCausalLM_KIVI.from_pretrained(config=...) does (example.py:22-28, mem_spd_test.py:24-31).  `config` is
         the user's config object carrying k_bits / v_bits / group_size / residual_length (models/llama_kivi.py:34-38);
@@ -788,9 +822,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         if self.cache is not None:
             rows = max(rows, self.cache.max_tokens + 1)   # a cache longer than the config's context still has its rows
         if self._rope is None or self._rope[0].device != device or self._rope[0].shape[0] < rows:
-            hd = self.config.hidden_size // self.config.num_attention_heads
             theta, scaling = rope_settings(self.config)
-            self._rope = _rope_tables(hd, rows, theta, device, scaling)
+            self._rope = _rope_tables(head_dim(self.config), rows, theta, device, scaling)
             self._graph = None
         return self._rope
 
@@ -1408,8 +1441,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         return f
 
     def _step_body(self):
-        """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split,
-        fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels; then lm_head, the cache advance and the argmax
+        """One decode step with 9 launches per layer: 4 cuBLAS GEMMs (q|k|v, o, gate|up, down), RoPE+split (Qwen3's
+        q_norm / k_norm folded in), fused KIVI attention, SiLU*mul and two residual-add+RMSNorm kernels; then lm_head, the cache advance and the argmax
         or sampling kernel, which set_processing() frames with the logits-processing kernel before it and the record
         kernel after it; set_logprobs() adds the log-probability kernel after the choice.  A model with attention biases adds them in the q|k|v and o GEMMs (addmm).
         Tensor-parallel (self._allreduce is a PeerAllReduce): the same launches on this rank's heads and channels, but o_proj
@@ -1442,7 +1475,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
         glue.add_rmsnorm(None, f.res, layers[0].input_layernorm.weight, f.h, eps)
         for i, l in enumerate(layers):
             linear(f.h, f.wqkv[i], f.bqkv[i], f.qkv)
-            glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
+            a = l.self_attn
+            if a.q_norm is None:
+                glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
+            else:                                            # the same kernel, normalising each q / k head first
+                glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v, a.q_norm.weight, a.k_norm.weight,
+                                a.q_norm.variance_epsilon)
             cache.decode_attention(i, f.q, f.k, f.v, out=f.attn)
             linear(f.attn.view(f.B, -1), f.wo[i], l.self_attn.o_proj.bias, partial(2 * i))
             add_rmsnorm(2 * i, l.post_attention_layernorm.weight)

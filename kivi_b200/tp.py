@@ -3,8 +3,9 @@
 Rank r of N holds the q rows of query heads [r*H/N, (r+1)*H/N), the k / v rows of KV heads [r*Hkv/N, ...) (a KV head and
 its query group stay on one rank, so the KIVI cache and attention kernels run unchanged on H/N, Hkv/N heads), the o_proj
 input columns of its query heads, the gate and up rows of intermediate channels [r*I/N, ...) and the matching down_proj
-input columns.  The embedding, the norms and lm_head are replicated.  o_proj and down_proj then produce partial sums that
-every rank adds up in fp32 in rank order: kivi_allreduce_add_rmsnorm_f16 in the decode step, `sum_partials` off it.
+input columns.  The embedding, the norms (Qwen3's per-head q_norm / k_norm too) and lm_head are replicated.  o_proj and
+down_proj then produce partial sums that every rank adds up in fp32 in rank order: kivi_allreduce_add_rmsnorm_f16 in the
+decode step, `sum_partials` off it.
 """
 from __future__ import annotations
 
@@ -26,8 +27,10 @@ def check_divisible(config, world: int):
 
 def shard_of(name: str, config, rank: int, world: int):
     """(dim, lo, hi): the slice of parameter `name` (HF Llama naming) that rank `rank` holds, or None if it is replicated.
-    q / k / v biases (Qwen2) are column-parallel like their weights' rows."""
-    hd = config.hidden_size // config.num_attention_heads
+    q / k / v biases (Qwen2) are column-parallel like their weights' rows; Qwen3's q_norm / k_norm act on one head's
+    channels and are replicated."""
+    from .llama_kivi import head_dim
+    hd = head_dim(config)
     q = config.num_attention_heads // world * hd
     kv = config.num_key_value_heads // world * hd
     inter = config.intermediate_size // world
