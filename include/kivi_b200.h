@@ -517,6 +517,40 @@ int kivi_logits_record(const void* tokens, int batch, int vocab, int32_t* counts
 int kivi_token_logprobs_f32(const void* logits, int batch, int vocab, const int64_t* tokens, int n_top, float* logprob,
                             int64_t* top_ids, float* top_logprobs, void* stream);
 
+/* LoRA deltas of one projection group (q|k|v: 3 segments, o: 1, gate|up: 2, down: 1) for a batch of rows, each row with its
+ * own adapter.  S adapters are stacked in slots 0 .. S-1:
+ *   A      fp16 [S, n_seg, R, in]   (lora_A of segment g at [s, g]; ranks below R zero-padded)
+ *   B      fp16 [S, out_total, R]   (lora_B rows of every segment, one after the other; zero-padded columns)
+ *   scale  fp32 [S]                 (alpha / r, or alpha / sqrt(r) under rsLoRA)
+ *   seg_off HOST int [n_seg + 1]    the segments' first columns, 0 = seg_off[0] < ... < seg_off[n_seg] = out_total;
+ *                                   seg(o) = the g with seg_off[g] <= o < seg_off[g + 1]
+ *   idx    int32 [rows] (device)    row b's slot; idx[b] < 0 (no adapter) or idx[b] >= S: row b of y is NOT written
+ * x fp16 [rows, in] and y fp16 [rows, out_total] are contiguous.  For row b with slot a = idx[b] in [0, S):
+ *   kivi_lora_shrink_f16:  ws[c, b, g R + j] = sum over k in chunk c of x[b, k] A[a, g, j, k]          (fp32, chunks of 512)
+ *   kivi_lora_expand_f16:  t[b, e] = sum_c ws[c, b, e] (chunk order);
+ *                          y[b, o] = fp16(float(y[b, o]) + d), d = scale[a] * sum_j B[a, o, j] t[b, seg(o) R + j],
+ *                          except that d == 0 leaves y[b, o]'s bits as they are.
+ * The shrink must precede the expand on the stream, with the same rows, in, n_seg, R, S and idx: two launches per group.
+ * ws: fp32 workspace of kivi_lora_workspace_bytes(rows, in, n_seg, R) bytes, ceil(in / 512) * rows * n_seg * R floats.
+ * Each CTA serves one slot and gathers that slot's rows from idx, so each present adapter's A and B are read once per call.
+ * Every sum has an order fixed by the shapes: row b's output depends only on row b's x, y and adapter, bit for bit -- not on
+ * the other rows, their adapters, S or the grid -- and is identical from run to run and under graph replay.
+ * Error bound (finite inputs, no overflow): with v = y + scale * sum_j B[o, j] sum_k x_k A[g, j, k] in float64 and
+ * M = |scale| sum_j |B[o, j]| sum_k |x_k A[g, j, k]|,
+ *     |y_out - v| <= 2^-11 |v| + (1 + 2^-11) c (M + |v|) + 2^-25,    c = (in + R + 3) 2^-24
+ * (fp16 x fp16 products are exact in fp32; the fp32 sums of length in and R, the scale and the add round each partial sum
+ * at most once per term; then the final fp16 rounding, relative below 2^-11 and absolute 2^-25 among subnormals.)
+ * Requirements: 0 <= rows <= 1024, in % 8 == 0 and in >= 8, 1 <= S <= 65535, n_seg in {1, 2, 3}, R % 8 == 0 and
+ * 8 <= R <= 128 (KIVI_ERR_SHAPE); x, A, B 16-byte aligned (KIVI_ERR_ALIGN); non-NULL pointers (KIVI_ERR_NULL); the
+ * expand also checks seg_off (KIVI_ERR_SHAPE).  Argument errors return before any launch; rows == 0 launches nothing.  No
+ * allocation, graph-capturable (seg_off is read at the call).  kivi_lora_workspace_bytes returns KIVI_ERR_SHAPE (< 0) for
+ * shapes the entries refuse. */
+int64_t kivi_lora_workspace_bytes(int rows, int in, int n_seg, int rank);
+int kivi_lora_shrink_f16(const void* x, int rows, int in, const void* A, int S, int n_seg, int rank, const int32_t* idx,
+                         float* ws, void* stream);
+int kivi_lora_expand_f16(const float* ws, int rows, int in, const void* B, const float* scale, int S, int n_seg, int rank,
+                         const int* seg_off, const int32_t* idx, void* y, int out_total, void* stream);
+
 /* Tensor-parallel residual-add + RMSNorm: the all-reduce after o_proj / down_proj fused into the norm that follows it.
  * With the rows of the attention heads and of the MLP columns sharded over `world` ranks, rank p holds a partial sum
  * partial_p [rows, hidden] fp16 of the projection.  Every rank computes the same bits:

@@ -133,6 +133,7 @@ class KiviCache:
         # the staging scratch (allocated on the first reorder)
         self.reorder_src = torch.arange(batch, dtype=torch.int32, device=self.device)
         self._reorder_scratch = None
+        self.adapter_idx = None         # a model's per-row LoRA adapter slots (int32 [batch]), gathered by reorder()
         # host mirror of `state` (its evolution is deterministic)
         self.tk = self.r = self.tv = self.L = self.vhead = self.kv_len = 0
 
@@ -284,6 +285,8 @@ class KiviCache:
                            "kivi_cache_reorder_f16")
             if self.ragged:
                 self.kv_start.copy_(self.kv_start.index_select(0, self.reorder_src))
+            if self.adapter_idx is not None:
+                self.adapter_idx.copy_(self.adapter_idx.index_select(0, self.reorder_src))
 
     def _mirror_reorder(self, rows):
         if self.ragged:

@@ -36,6 +36,9 @@ def _bind():
     _lib.bind("kivi_prompt_attention_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32] + [i64] * 6 + [vp, i32, vp])
     _lib.bind("kivi_prompt_attention_suffix_f16", i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32] + [i64] * 6 +
               [vp, i32, vp])
+    _lib.bind("kivi_lora_workspace_bytes", i64, [i32, i32, i32, i32])
+    _lib.bind("kivi_lora_shrink_f16", i32, [vp, i32, i32, vp, i32, i32, i32, vp, vp, vp])
+    _lib.bind("kivi_lora_expand_f16", i32, [vp, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp])
     _B = True
 
 
@@ -287,6 +290,49 @@ def token_logprobs(logits, tokens, logprob, top_ids=None, top_logprobs=None):
         logits.data_ptr(), B, V, tokens.data_ptr(), N, logprob.data_ptr(), ptr(top_ids), ptr(top_logprobs),
         _lib.stream_ptr(logits.device)), "kivi_token_logprobs_f32")
     return logprob
+
+
+def lora_workspace_bytes(rows: int, in_features: int, n_seg: int, rank: int) -> int:
+    """The fp32 workspace of lora_apply (kivi_lora_workspace_bytes); ValueError for shapes the kernels refuse."""
+    _bind()
+    n = int(_lib.lib().kivi_lora_workspace_bytes(rows, in_features, n_seg, rank))
+    if n < 0:
+        raise ValueError(f"LoRA kernels: unsupported shape rows={rows} in={in_features} n_seg={n_seg} rank={rank}")
+    return n
+
+
+def lora_apply(x, y, A, B, scale, seg_off, idx, ws):
+    """y[b] += the LoRA delta of row b's adapter idx[b] (kivi_lora_shrink_f16 then kivi_lora_expand_f16, two launches):
+    x fp16 [rows, in], y fp16 [rows, out] (in place), A fp16 [S, n_seg, R, in], B fp16 [S, out, R], scale fp32 [S],
+    seg_off the segments' first columns (a host sequence of n_seg + 1 ints, read now), idx int32 [rows] (a row with
+    idx < 0 or >= S is not written), ws fp32 of at least lora_workspace_bytes.  include/kivi_b200.h has the arithmetic
+    and the error bound.  Nothing allocated: a captured call reads new x, idx and weights on every replay."""
+    _bind()
+    if x.dim() != 2 or y.dim() != 2 or A.dim() != 4 or B.dim() != 3:
+        raise ValueError(f"lora_apply: expected x [rows, in], y [rows, out], A [S, n_seg, R, in], B [S, out, R]; got "
+                         f"{tuple(x.shape)}, {tuple(y.shape)}, {tuple(A.shape)}, {tuple(B.shape)}")
+    rows, n_in = x.shape
+    S, n_seg, R, _ = A.shape
+    out = y.shape[1]
+    for name, t, dtype, shape in (("x", x, torch.float16, (rows, n_in)), ("y", y, torch.float16, (rows, out)),
+                                  ("A", A, torch.float16, (S, n_seg, R, n_in)), ("B", B, torch.float16, (S, out, R)),
+                                  ("scale", scale, torch.float32, (S,)), ("idx", idx, torch.int32, (rows,))):
+        _check(name, t, dtype, shape)
+        if t.device != x.device:
+            raise ValueError(f"{name}: on {t.device}, x on {x.device}")
+    _check("ws", ws, torch.float32, ws.shape)
+    if ws.numel() * 4 < lora_workspace_bytes(rows, n_in, n_seg, R) or ws.device != x.device:
+        raise ValueError("ws: smaller than lora_workspace_bytes or on another device")
+    if len(seg_off) != n_seg + 1:
+        raise ValueError(f"seg_off: expected {n_seg + 1} offsets, got {len(seg_off)}")
+    segs = (ctypes.c_int * (n_seg + 1))(*[int(v) for v in seg_off])
+    stream = _lib.stream_ptr(x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().kivi_lora_shrink_f16(x.data_ptr(), rows, n_in, A.data_ptr(), S, n_seg, R, idx.data_ptr(),
+                                                   ws.data_ptr(), stream), "kivi_lora_shrink_f16")
+        _lib.check(_lib.lib().kivi_lora_expand_f16(ws.data_ptr(), rows, n_in, B.data_ptr(), scale.data_ptr(), S, n_seg, R,
+                                                   segs, idx.data_ptr(), y.data_ptr(), out, stream), "kivi_lora_expand_f16")
+    return y
 
 
 def _prompt_operands(q, k, v, out, kv_start):

@@ -301,6 +301,15 @@ def head_dim(config):
     return getattr(config, "head_dim", None) or config.hidden_size // config.num_attention_heads
 
 
+def _linear(owner, name: str, layer: int, x, lora):
+    """owner.<name>(x), plus the LoRA delta of each token's adapter when `lora` = (kivi_b200.lora.LoraState, adapter slot
+    of each token [tokens]) is given (the prompt pass and forward(); the decode step runs the LoRA kernels instead)."""
+    y = getattr(owner, name)(x)
+    if lora is not None:
+        lora[0].add(layer, name, x, y, lora[1])
+    return y
+
+
 class LlamaFlashAttention_KIVI(nn.Module):
     """Attention layer of the reference (models/llama_kivi.py:264-466), KIVI ops on libkivi_b200."""
 
@@ -332,23 +341,24 @@ class LlamaFlashAttention_KIVI(nn.Module):
             return q, k
         return self.q_norm(q), self.k_norm(k)
 
-    def _qkv(self, hidden_states, cos, sin):
+    def _qkv(self, hidden_states, cos, sin, lora=None):
         bsz, q_len, _ = hidden_states.shape
-        q = self.q_proj(hidden_states).view(bsz, q_len, self.num_heads, self.head_dim)
-        k = self.k_proj(hidden_states).view(bsz, q_len, self.num_key_value_heads, self.head_dim)
-        v = self.v_proj(hidden_states).view(bsz, q_len, self.num_key_value_heads, self.head_dim).transpose(1, 2)
+        proj = lambda name: _linear(self, name, self.layer_idx, hidden_states, lora)   # noqa: E731
+        q = proj("q_proj").view(bsz, q_len, self.num_heads, self.head_dim)
+        k = proj("k_proj").view(bsz, q_len, self.num_key_value_heads, self.head_dim)
+        v = proj("v_proj").view(bsz, q_len, self.num_key_value_heads, self.head_dim).transpose(1, 2)
         q, k = (t.transpose(1, 2) for t in self._qk_normed(q, k))
         q = q * cos + _rotate_half(q) * sin                                 # apply_rotary_pos_emb (:311)
         k = k * cos + _rotate_half(k) * sin
         return q, k, v
 
-    def _qkv_rows(self, x, cos, sin):
+    def _qkv_rows(self, x, cos, sin, lora=None):
         """_qkv on rows of tokens: x [rows, hidden], cos / sin [rows, 1, D] -> q [rows, H, D], k and v [rows, Hkv, D],
         q and k rotated."""
         rows = x.shape[0]
-        q = self.q_proj(x).view(rows, self.num_heads, self.head_dim)
-        k = self.k_proj(x).view(rows, self.num_key_value_heads, self.head_dim)
-        v = self.v_proj(x).view(rows, self.num_key_value_heads, self.head_dim)
+        q = _linear(self, "q_proj", self.layer_idx, x, lora).view(rows, self.num_heads, self.head_dim)
+        k = _linear(self, "k_proj", self.layer_idx, x, lora).view(rows, self.num_key_value_heads, self.head_dim)
+        v = _linear(self, "v_proj", self.layer_idx, x, lora).view(rows, self.num_key_value_heads, self.head_dim)
         q, k = self._qk_normed(q, k)
         return q * cos + _rotate_half(q) * sin, k * cos + _rotate_half(k) * sin, v
 
@@ -382,22 +392,22 @@ class LlamaFlashAttention_KIVI(nn.Module):
         store_kv(self.layer_idx, k, v)
         return attn_output, None
 
-    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None):
-        """hidden_states [B, q_len, hidden]; cos/sin broadcastable to [B, 1, q_len, D].
+    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None, lora=None):
+        """hidden_states [B, q_len, hidden]; cos/sin broadcastable to [B, 1, q_len, D].  lora: see _linear.
         past_key_value: None (a prompt pass, returns a 9-tuple) or the reference's 9-tuple (decode, returns the next one).
         store_kv: with a prompt pass, a callable store_kv(layer, k, v) that takes the rotated K and V [B, Hkv, q_len, D] in
         place of the 9-tuple (the fused cache: KiviCache.prefill, or a refill of one slot); the pass then returns None.
         attention_mask: None or additive [B, 1, q_len, kv_len] (models/llama_kivi.py:364-372); in a prompt pass also a
         PromptMask or a PrefixMask."""
         bsz, q_len, _ = hidden_states.shape
-        q, k, v = self._qkv(hidden_states, cos, sin)
+        q, k, v = self._qkv(hidden_states, cos, sin, lora)
         if past_key_value is not None:                                      # reference 9-tuple, decode
             attn_output, past = kivi_decode_attention_tuple(q, k, v, past_key_value, self.group_size, self.k_bits,
                                                             self.v_bits, self.residual_length, attention_mask)
             attn_output = attn_output.transpose(1, 2).contiguous().reshape(bsz, q_len, self.num_heads * self.head_dim)
         else:                                                               # prompt (:401-455)
             attn_output, past = self._prompt_core(q, k, v, attention_mask, store_kv)
-        return self.o_proj(attn_output), None, past
+        return _linear(self, "o_proj", self.layer_idx, attn_output, lora), None, past
 
 
 LlamaAttention_KIVI = LlamaFlashAttention_KIVI      # models/llama_kivi.py:19 (unreachable in the reference: ctor asserts use_flash)
@@ -411,8 +421,10 @@ class LlamaMLP(nn.Module):
         self.up_proj = nn.Linear(config.hidden_size, inter, bias=False)
         self.down_proj = nn.Linear(inter, config.hidden_size, bias=False)
 
-    def forward(self, x):
-        return self.down_proj(F.silu(self.gate_proj(x)) * self.up_proj(x))
+    def forward(self, x, lora=None, layer: int = 0):
+        """lora, layer: the LoRA deltas of the rows' adapters (_linear) in decoder layer `layer`."""
+        act = F.silu(_linear(self, "gate_proj", layer, x, lora)) * _linear(self, "up_proj", layer, x, lora)
+        return _linear(self, "down_proj", layer, act, lora)
 
 
 class LlamaDecoderLayer_KIVI(nn.Module):
@@ -424,22 +436,26 @@ class LlamaDecoderLayer_KIVI(nn.Module):
         self.post_attention_layernorm = LlamaRMSNorm(config.hidden_size, config.rms_norm_eps)
         self.tp_world = tp_world
 
-    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None):
+    def forward(self, hidden_states, cos, sin, past_key_value=None, attention_mask=None, store_kv=None, lora=None):
+        """lora: None, or (kivi_b200.lora.LoraState, adapter slot of each batch row [B]) -- every token of row b takes the
+        LoRA deltas of adapter slot b (< 0: none)."""
         if past_key_value is None and hidden_states.shape[0] * hidden_states.shape[1] > PROMPT_CHUNK_ROWS:
-            return self._prompt_in_chunks(hidden_states, cos, sin, attention_mask, store_kv)
+            return self._prompt_in_chunks(hidden_states, cos, sin, attention_mask, store_kv, lora)
+        if lora is not None:
+            lora = (lora[0], lora[1].repeat_interleave(hidden_states.shape[1]))        # a slot per token
         residual = hidden_states
         h, _, past = self.self_attn(self.input_layernorm(hidden_states), cos, sin, past_key_value, attention_mask,
-                                    store_kv)
+                                    store_kv, lora)
         if self.tp_world > 1:                                                 # partial sums of the sharded projections
             h = sum_partials(h)
         hidden_states = residual + h
-        h = self.mlp(self.post_attention_layernorm(hidden_states))
+        h = self.mlp(self.post_attention_layernorm(hidden_states), lora, self.self_attn.layer_idx)
         if self.tp_world > 1:
             h = sum_partials(h)
         hidden_states = hidden_states + h
         return hidden_states, past
 
-    def _prompt_in_chunks(self, x, cos, sin, attention_mask, store_kv):
+    def _prompt_in_chunks(self, x, cos, sin, attention_mask, store_kv, lora=None):
         """forward() of a prompt pass in bounded memory: the per-token work -- input norm, q|k|v, RoPE; after the
         attention o_proj, the residual add, the post-attention norm, the MLP and its residual add -- runs on
         PROMPT_CHUNK_ROWS rows of B * n at a time, the attention between the two halves on the whole prompt.  The layer
@@ -454,18 +470,20 @@ class LlamaDecoderLayer_KIVI(nn.Module):
         k = x.new_empty((rows, a.num_key_value_heads, D))
         v = torch.empty_like(k)
         chunks = [slice(lo, min(lo + PROMPT_CHUNK_ROWS, rows)) for lo in range(0, rows, PROMPT_CHUNK_ROWS)]
+        slots = None if lora is None else lora[1].repeat_interleave(n)          # a slot per token
+        part = lambda c: None if lora is None else (lora[0], slots[c])        # noqa: E731
         for c in chunks:
-            q[c], k[c], v[c] = a._qkv_rows(self.input_layernorm(flat[c]), cos[c], sin[c])
+            q[c], k[c], v[c] = a._qkv_rows(self.input_layernorm(flat[c]), cos[c], sin[c], part(c))
         heads = lambda t: t.view(B, n, -1, D).transpose(1, 2)                # noqa: E731 ([B, heads, n, D], as _qkv)
         attn, past = a._prompt_core(heads(q), heads(k), heads(v), attention_mask, store_kv)
         del q, k, v
         attn = attn.view(rows, -1)
         for c in chunks:
-            h = a.o_proj(attn[c])
+            h = _linear(a, "o_proj", a.layer_idx, attn[c], part(c))
             if self.tp_world > 1:
                 h = sum_partials(h)
             r = flat[c] + h
-            h = self.mlp(self.post_attention_layernorm(r))
+            h = self.mlp(self.post_attention_layernorm(r), part(c), a.layer_idx)
             if self.tp_world > 1:
                 h = sum_partials(h)
             flat[c] = r + h
@@ -739,6 +757,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._sampling = False              # the step's last kernel samples (set_sampling) instead of taking the argmax
         self._logprobs_n = None             # set_logprobs(): the step's top-N logprobs (None: off)
         self.logprobs = self.top_ids = self.top_logprobs = None
+        self._lora = None                   # kivi_b200.lora.LoraState once an adapter is loaded (load_adapter)
+        self._adapter_sel = None            # set_adapters(): None, one slot, or a slot per row
+        self._adapter_idx = None            # int32 [batch]: each cache row's adapter slot (-1: none), read by the step
 
     # ------------------------------------------------------------------ HF-style construction
     @classmethod
@@ -827,14 +848,16 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self._graph = None
         return self._rope
 
-    def _run_layers(self, input_ids, positions, pasts, attention_mask=None, store_kv=None):
+    def _run_layers(self, input_ids, positions, pasts, attention_mask=None, store_kv=None, adapters=None):
+        """adapters: None, or the adapter slot of each batch row (int32 [B]; -1: none)."""
         cos_t, sin_t = self._tables(input_ids.device)
+        lora = None if adapters is None or self._lora is None else (self._lora, adapters.to(input_ids.device))
         cos = cos_t.index_select(0, positions.reshape(-1)).view(positions.shape[0], 1, positions.shape[1], -1)
         sin = sin_t.index_select(0, positions.reshape(-1)).view(positions.shape[0], 1, positions.shape[1], -1)
         h = self.model.embed_tokens(input_ids)
         new_pasts = []
         for i, layer in enumerate(self.model.layers):
-            h, past = layer(h, cos, sin, pasts[i] if pasts is not None else None, attention_mask, store_kv)
+            h, past = layer(h, cos, sin, pasts[i] if pasts is not None else None, attention_mask, store_kv, lora)
             new_pasts.append(past)
         rows = h.shape[0] * h.shape[1]
         if rows > PROMPT_CHUNK_ROWS:                   # a long prompt: the norm's fp32 temporaries one chunk at a time
@@ -877,7 +900,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 mask = self._tuple_prompt_mask(attention_mask, B, q_len, input_ids.device)
             if mask is None:
                 mask = _additive_mask(attention_mask, q_len, start + q_len, dtype, input_ids.device, self.sliding_window, B)
-            h, pasts = self._run_layers(input_ids, position_ids, past_key_values, mask)
+            h, pasts = self._run_layers(input_ids, position_ids, past_key_values, mask, adapters=self._rows_for(B))
             logits = self.lm_head(h).float()                                     # logits.float() (:881)
         if return_dict is None:
             return_dict = getattr(self.config, "use_return_dict", False)
@@ -1031,6 +1054,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
         n_top, self._logprobs_n = self._logprobs_n, None
         self.logprobs = self.top_ids = self.top_logprobs = None
         self._tables(dev)                                   # rows for every position the cache can reach
+        self._adapter_idx = torch.full((batch,), -1, dtype=torch.int32, device=dev)
+        if self._lora is not None:
+            self.cache.adapter_idx = self._adapter_idx       # KiviCache.reorder gathers it with the rows
+            sel = self._adapter_sel
+            if isinstance(sel, int):
+                self._adapter_idx.fill_(sel)
+            elif sel is not None and len(sel) == batch:
+                self._adapter_idx.copy_(torch.tensor(sel, dtype=torch.int32))
         if n_top is not None:
             self.set_logprobs(n_top)
         return self.cache
@@ -1076,12 +1107,13 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 starts = None
         if self._processing:
             self._mark_prompt(input_ids, starts, slice(None), copies)
+        rows = None if self._lora is None else self._adapter_idx[::copies].contiguous()     # prompt b's adapter
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
             mask = self._kernel_mask(None, n, input_ids.device)
             if mask is None:
                 mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window, B)
-            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store)
+            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store, adapters=rows)
             self._pos.fill_(n)
         else:
             am = attention_mask.to(input_ids.device)
@@ -1090,14 +1122,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
             mask = self._kernel_mask(starts, n, input_ids.device)
             if mask is None:
                 mask = _additive_mask(am, n, n, self.lm_head.weight.dtype, input_ids.device, self.sliding_window)
-            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store)
+            h, _ = self._run_layers(input_ids, positions, None, mask, store_kv=store, adapters=rows)
             starts = starts.to(self._pos.device).repeat_interleave(copies)
             self._pos.copy_((n - starts).to(torch.long).view(B * copies, 1))
             self.cache.set_kv_start(starts)
         return h
 
     @torch.no_grad()
-    def insert(self, seq: int, prompt_ids, prefix_cache=None):
+    def insert(self, seq: int, prompt_ids, prefix_cache=None, adapter=None):
         """Start a new sequence in slot `seq` of the running batch (continuous batching): a B = 1 prompt pass at positions
         0 .. n-1 whose K/V go into that slot right-aligned to the shared length T (KiviCache.refill), then
         kv_start[seq] = T - n and the slot's position = n.  The other slots are not touched.  Returns the prompt's
@@ -1105,15 +1137,22 @@ class LlamaForCausalLM_KIVI(nn.Module):
         prefix_cache: a kivi_b200.prefix.PrefixCache.  When it holds the prompt's first r >= MIN_REUSE tokens (r <= n - 1,
         prefix.reuse_length), the pass runs on tokens r .. n-1 only, at positions r .. n-1, over the stored K / V and
         its own (PrefixMask); otherwise it runs the whole prompt as without a cache.  Either way the prompt's tokens past
-        the stored path are stored."""
+        the stored path are stored.  A stored prefix is reused only under the adapter it was stored with.
+        adapter: the name of a loaded LoRA adapter for the new sequence (load_adapter), or None for none."""
         assert self.cache is not None, "call init_cache() / prefill() first"
         ids = torch.as_tensor(prompt_ids, device=self.cache.device).reshape(1, -1)
         n, T = ids.shape[1], self.cache.kv_len
         if not 1 <= n <= T:
             raise ValueError(f"a prompt of {n} tokens does not fit the shared length {T} (1 <= n <= length)")
+        rows = None
+        if self._lora is not None:
+            self._adapter_idx[seq] = self._lora.slot(adapter)
+            rows = self._adapter_idx[seq:seq + 1]
+        elif adapter is not None:
+            raise ValueError(f"adapter {adapter!r}: no LoRA adapter is loaded (load_adapter)")
         r, store = 0, lambda layer, k, v: self.cache.refill(layer, seq, k, v)       # noqa: E731
         if prefix_cache is not None:
-            r, store, record = self._prefix_insert(prefix_cache, ids, store)
+            r, store, record = self._prefix_insert(prefix_cache, ids, store, adapter)
         positions = torch.arange(r, n, device=ids.device).unsqueeze(0)
         mask = self._kernel_mask(None, n, ids.device)
         if r:
@@ -1121,7 +1160,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                               self._prefix_extend(prefix_cache, record[1], r, n))
         elif mask is None:
             mask = _additive_mask(None, n, n, self.lm_head.weight.dtype, ids.device, self.sliding_window)
-        h, _ = self._run_layers(ids[:, r:], positions, None, mask, store_kv=store)
+        h, _ = self._run_layers(ids[:, r:], positions, None, mask, store_kv=store, adapters=rows)
         if prefix_cache is not None:
             prefix_cache.insert(*record)
         self._pos[seq] = n
@@ -1130,7 +1169,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self._mark_prompt(ids, None, slice(seq, seq + 1))
         return self.lm_head(h[0, -1]).float()
 
-    def _prefix_insert(self, prefix_cache, ids, refill):
+    def _prefix_insert(self, prefix_cache, ids, refill, adapter=None):
         """insert()'s use of a PrefixCache: bind it, find the prompt's stored prefix and reserve room for the rest.
         Returns r (the tokens to reuse, 0 for none), the store_kv that refills the slot and copies the new tokens' K / V
         into the reserved storage, and the arguments of prefix_cache.insert once the pass is done."""
@@ -1139,7 +1178,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         prefix_cache.bind(self, len(self.model.layers), a.num_key_value_heads, ids.device)
         tokens = ids[0].tolist()
         n = len(tokens)
-        match = prefix_cache.match(tokens)
+        match = prefix_cache.match(tokens, adapter)
         r = reuse_length(match.length, n)
         if r:
             prefix_cache.hits += 1
@@ -1151,7 +1190,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 storage[layer, 0].copy_(k[0, :, match.length:])
                 storage[layer, 1].copy_(v[0, :, match.length:])
                 refill(layer, k, v)
-        return r, store, (tokens, match, storage)
+        return r, store, (tokens, match, storage, adapter)
 
     @staticmethod
     def _prefix_extend(prefix_cache, match, r: int, n: int):
@@ -1170,6 +1209,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         """Make slot `seq` idle (KiviCache.release): it keeps its row of every step but reads no cached byte."""
         self.cache.release(seq)
         self._pos[seq] = 0
+        if self._lora is not None:
+            self._adapter_idx[seq] = -1
         if self._processing:
             p = self._proc
             for t in (p.seen, p.counts, p.n_new, p.finished):
@@ -1389,6 +1430,79 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.top_ids = torch.zeros((B, n_top), dtype=torch.long, device=dev)
             self.top_logprobs = torch.zeros((B, n_top), dtype=torch.float32, device=dev)
 
+    # ------------------------------------------------------------------ LoRA adapters
+    def load_adapter(self, path, adapter_name: str):
+        """Load the PEFT LoRA adapter in the local directory `path` under `adapter_name` (kivi_b200.lora: what is supported
+        and what is refused with a ValueError).  It is stacked beside the other loaded adapters on the model's device; the
+        base weights are not touched.  Rows choose it with set_adapters, insert(adapter=), generate(adapter=) or a serve()
+        request's "adapter".  Once an adapter is loaded the decode step adds two LoRA launches per projection group (8 per
+        layer); rows without an adapter come out bit-equal to the step without them.  The captured steps are dropped.
+        Load adapters after moving the model to its device and dtype.  NotImplementedError under tensor_parallel."""
+        if self.tensor_parallel:
+            raise NotImplementedError("load_adapter: LoRA under tensor parallelism (sharded A / B and their reduction) is "
+                                      "not supported")
+        from . import lora
+        adapter = lora.read_adapter(path, self.config)                    # every check before anything changes
+        state = self._lora if self._lora is not None else lora.LoraState(self.config, self.lm_head.weight.device)
+        state.load(adapter_name, adapter)
+        self._lora = state
+        self._graph = self._reorder_graph = None
+        if self.cache is not None:
+            self.cache.adapter_idx = self._adapter_idx
+        return state.names[adapter_name]
+
+    @property
+    def adapters(self):
+        """The names of the loaded LoRA adapters, in slot order."""
+        return [] if self._lora is None else list(self._lora.names)
+
+    def set_adapters(self, adapters=None):
+        """The LoRA adapter of every batch row: None (none), one name for every row, or a list of one name (or None) per
+        row of the cache.  forward(), prefill() and the decode step read it; init_cache() keeps a selection that fits the
+        new batch.  Unknown names are a KeyError, a list of the wrong length a ValueError."""
+        if adapters is None:
+            sel = None
+        elif self._lora is None:
+            raise ValueError("set_adapters: no LoRA adapter is loaded (load_adapter)")
+        elif isinstance(adapters, str):
+            sel = self._lora.slot(adapters)
+        else:
+            sel = [self._lora.slot(a) for a in adapters]
+            if self.cache is not None and len(sel) != self.cache.batch:
+                raise ValueError(f"set_adapters: {len(sel)} names for a batch of {self.cache.batch}")
+        self._adapter_sel = sel
+        if self._adapter_idx is not None:
+            if sel is None or isinstance(sel, int):
+                self._adapter_idx.fill_(-1 if sel is None else sel)
+            else:
+                self._adapter_idx.copy_(torch.tensor(sel, dtype=torch.int32))
+
+    def _rows_for(self, B: int):
+        """The adapter slot of each of B rows of a forward() pass (None: no adapter loaded or selected)."""
+        if self._lora is None:
+            return None
+        if self.cache is not None and self.cache.batch == B:
+            return self._adapter_idx
+        sel = self._adapter_sel
+        if sel is None:
+            return None
+        if isinstance(sel, int):
+            sel = [sel] * B
+        if len(sel) != B:
+            raise ValueError(f"set_adapters named {len(sel)} rows, the batch has {B}")
+        return torch.tensor(sel, dtype=torch.int32)
+
+    def _lora_ws(self):
+        """The decode step's LoRA workspace: fp32, the largest of the four groups' needs at this batch and rank."""
+        from . import glue
+        from .lora import GROUPS
+        lo, B = self._lora, self.cache.batch
+        need = max(glue.lora_workspace_bytes(B, lo.shapes[mods[0]][1], len(mods), lo.rank) for mods in GROUPS.values())
+        ws = getattr(self._fast, "lora_ws", None)
+        if ws is None or ws.numel() * 4 < need:
+            ws = self._fast.lora_ws = torch.empty(need // 4, dtype=torch.float32, device=self.cache.device)
+        return ws
+
     @property
     def all_tokens(self):
         if self._exchange is not None:
@@ -1471,10 +1585,22 @@ class LlamaForCausalLM_KIVI(nn.Module):
             else:
                 torch.addmm(bias, x, w, out=out)
 
+        lo = self._lora
+        if lo is not None:                                   # LoRA: shrink + expand after each GEMM, 8 launches per layer
+            ws = self._lora_ws()
+
+            def lora(i, group, x, y):
+                A, B = lo.stacks[i][group]
+                glue.lora_apply(x, y, A, B, lo.scale, lo.segs[group], self._adapter_idx, ws)
+        else:
+            def lora(i, group, x, y):
+                pass
+
         f.res.copy_(self.model.embed_tokens(self._ids)[:, 0])
         glue.add_rmsnorm(None, f.res, layers[0].input_layernorm.weight, f.h, eps)
         for i, l in enumerate(layers):
             linear(f.h, f.wqkv[i], f.bqkv[i], f.qkv)
+            lora(i, "qkv", f.h, f.qkv)                       # after the bias, before q_norm / RoPE (as PEFT)
             a = l.self_attn
             if a.q_norm is None:
                 glue.rope_split(f.qkv, cos_t, sin_t, self._pos, f.q, f.k, f.v)
@@ -1483,10 +1609,13 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                 a.q_norm.variance_epsilon)
             cache.decode_attention(i, f.q, f.k, f.v, out=f.attn)
             linear(f.attn.view(f.B, -1), f.wo[i], l.self_attn.o_proj.bias, partial(2 * i))
+            lora(i, "o", f.attn.view(f.B, -1), partial(2 * i))
             add_rmsnorm(2 * i, l.post_attention_layernorm.weight)
             torch.mm(f.h, f.wgu[i], out=f.gu)
+            lora(i, "gu", f.h, f.gu)
             glue.silu_mul(f.gu, f.act)
             torch.mm(f.act, l.mlp.down_proj.weight.t(), out=partial(2 * i + 1))
+            lora(i, "down", f.act, partial(2 * i + 1))
             nxt = layers[i + 1].input_layernorm.weight if i + 1 < len(layers) else self.model.norm.weight
             add_rmsnorm(2 * i + 1, nxt)
         if ar is not None:
@@ -1609,7 +1738,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
                  num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False,
                  eos_token_id=None, pad_token_id=None, return_dict_in_generate: bool = False, repetition_penalty=None,
                  min_length: int | None = None, min_new_tokens: int | None = None, output_scores: bool = False,
-                 output_logits: bool = False, **unused):
+                 output_logits: bool = False, adapter=None, **unused):
         """Decoding on the fused path with the call shape of HF generate (`model.generate(**inputs,
         max_new_tokens=n)`, example.py:60-61, mem_spd_test.py:66): returns [B, prompt + new] ids.  Greedy by default;
         do_sample=True samples every token, the first included, on the device with temperature / top_k / top_p (HF's
@@ -1641,7 +1770,10 @@ class LlamaForCausalLM_KIVI(nn.Module):
         per new token, also when decoding stops at EOS.  They stay on the device: rows * vocab * 4 bytes per new token
         each, as in transformers.  compute_transition_scores() turns them into per-token scores.  output_scores with
         do_sample=True (transformers returns the scores after its warpers, which the sampler never materialises) and either
-        output with beam search are NotImplementedError, before any work."""
+        output with beam search are NotImplementedError, before any work.
+        adapter: a loaded LoRA adapter's name for every prompt, or a list with one name (or None) per prompt; a prompt's
+        beams and num_return_sequences copies take its adapter.  None: no adapter on any row."""
+        names = self._adapter_names(adapter, input_ids.shape[0])
         if (output_scores or output_logits) and num_beams > 1:
             raise NotImplementedError("output_scores and output_logits in beam search are not supported")
         if output_scores and do_sample:
@@ -1656,7 +1788,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
                                           "supported: transformers applies them to log-probabilities there")
             return self._generate_many(input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample,
                                        temperature, top_k, top_p, seed, num_beams, num_return_sequences, length_penalty,
-                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate, proc, trace)
+                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate, proc, trace,
+                                       names)
         if do_sample:
             sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
         if proc is not None:
@@ -1684,11 +1817,26 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.set_processing(**proc)
         else:
             self.set_processing(None)
+        if self._lora is not None:
+            self.set_adapters(names)
         logits = self.prefill(input_ids, attention_mask)
         tok, scores = self.choose_first(logits, return_scores=True)
         _trace_add(trace, logits, scores)
         seq = torch.cat([input_ids, self._decode(tok.view(B, 1), max_new_tokens, use_graph, trace)], 1)
         return _generate_output(seq, trace) if return_dict_in_generate else seq
+
+    def _adapter_names(self, adapter, B: int):
+        """generate()'s adapter argument as a list of B names (None: no adapter), checked before any work."""
+        if adapter is None:
+            return None
+        names = [adapter] * B if isinstance(adapter, str) else list(adapter)
+        if len(names) != B:
+            raise ValueError(f"adapter: expected one name or {B} names, got {len(names)}")
+        if self._lora is None:
+            raise ValueError("adapter: no LoRA adapter is loaded (load_adapter)")
+        for a in names:
+            self._lora.slot(a)
+        return names
 
     def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits: bool = False):
         """transformers' GenerationMixin.compute_transition_scores for greedy and sampled outputs: the score of each
@@ -1740,7 +1888,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
 
     def _generate_many(self, input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample, temperature,
                        top_k, top_p, seed, num_beams, num_return_sequences, length_penalty, early_stopping, eos_token_id,
-                       pad_token_id, return_dict_in_generate, proc=None, trace=None):
+                       pad_token_id, return_dict_in_generate, proc=None, trace=None, names=None):
         """generate() with K = num_beams (beam search, kivi_b200.beam) or K = num_return_sequences (do_sample) sequences per
         prompt, in the cache's rows b * K .. b * K + K - 1.  The prompt pass runs once per prompt and its K / V fill the K
         rows (_prompt_pass(copies=K)).
@@ -1798,6 +1946,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
             self.set_processing(**proc)
         else:
             self.set_processing(None)
+        if self._lora is not None:
+            self.set_adapters(None if names is None else [a for a in names for _ in range(K)])
         logits = self.lm_head(self._prompt_pass(input_ids, attention_mask, copies=K)[:, -1]).float()    # [B, vocab]
         if do_sample:
             first = logits.repeat_interleave(K, 0)

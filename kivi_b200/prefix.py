@@ -13,7 +13,11 @@ bumped once per operation, and every decision depends on token ids, that counter
 a clock or on the allocator's state -- so tensor-parallel ranks that see the same prompts decide the same way.
 
 The tree itself runs no kernel: it slices, copies and allocates tensors on the device it is bound to (CPU tensors in the
-CPU tests).  Nodes hold no reference to their parent, so a dropped cache frees its memory at once."""
+CPU tests).  Nodes hold no reference to their parent, so a dropped cache frees its memory at once.
+
+K and V depend on the LoRA adapter a sequence runs with (its k_proj / v_proj deltas), so every adapter has a tree of its own
+(a root per adapter name, None for the base model): a prefix stored under one adapter is never matched for another.
+Eviction picks the least recently used leaf over all of them."""
 from __future__ import annotations
 
 import weakref
@@ -82,6 +86,7 @@ class PrefixCache:
         self.max_bytes = int(max_bytes)
         self.hits = self.reused_tokens = self.stored_bytes = self.peak_bytes = self.evictions = 0
         self._root = _Node((), None, None, 0, 0)
+        self._roots = {None: self._root}                 # one tree per LoRA adapter name (None: no adapter)
         self._clock = 0
         self._serial = 0
         self._owner = None
@@ -105,9 +110,10 @@ class PrefixCache:
         return self.layers * 2 * self.kv_heads * 128 * 2 * tokens
 
     # ------------------------------------------------------------------ lookup
-    def match(self, tokens) -> Match:
-        """The longest stored prefix of `tokens` (a sequence of ints).  Changes nothing."""
-        node, pos, path = self._root, 0, []
+    def match(self, tokens, adapter=None) -> Match:
+        """The longest stored prefix of `tokens` (a sequence of ints) under `adapter` (a LoRA adapter name, None for
+        none).  Changes nothing."""
+        node, pos, path = self._roots.get(adapter, _Node((), None, None, 0, 0)), 0, []
         while pos < len(tokens):
             child = node.children.get(tokens[pos])
             if child is None:
@@ -154,12 +160,14 @@ class PrefixCache:
             self._evict(*leaf)
         return True
 
-    def insert(self, tokens, match: Match, storage=None):
-        """Record an insert of `tokens` that matched `match`: every node of its path counts as used now, and with
-        `storage` (reserve()'s tensor, filled with the K / V of tokens[match.length:]) those tokens become a new leaf --
-        splitting the last node of the path where the prompt diverges inside it."""
+    def insert(self, tokens, match: Match, storage=None, adapter=None):
+        """Record an insert of `tokens` that matched `match` (under the same `adapter`): every node of its path counts as
+        used now, and with `storage` (reserve()'s tensor, filled with the K / V of tokens[match.length:]) those tokens
+        become a new leaf of the adapter's tree -- splitting the last node of the path where the prompt diverges inside it."""
         self._clock += 1
-        parent = self._root
+        if storage is None and adapter not in self._roots:
+            return
+        parent = self._roots.setdefault(adapter, _Node((), None, None, 0, 0))
         for node, take in match.path:
             if take < len(node.tokens):
                 if storage is None:
@@ -192,7 +200,7 @@ class PrefixCache:
     # ------------------------------------------------------------------ eviction
     def _edges(self):
         """(parent, node) for every node below the root."""
-        stack = [(self._root, c) for c in self._root.children.values()]
+        stack = [(root, c) for root in self._roots.values() for c in root.children.values()]
         while stack:
             parent, node = stack.pop()
             yield parent, node

@@ -11,6 +11,8 @@ A request may also carry a repetition, presence and frequency penalty and a mini
 inside the step, LlamaForCausalLM_KIVI.set_processing), read per slot on the device in the same way, and ask for the
 log-probabilities of its tokens (`logprobs`, LlamaForCausalLM_KIVI.set_logprobs), computed inside the step as well.
 With a PrefixCache (kivi_b200.prefix), an insert whose prompt starts with a stored prefix computes only the rest.
+A request may name a loaded LoRA adapter (`adapter`, LlamaForCausalLM_KIVI.load_adapter): its slot's row takes that
+adapter's deltas in the step, so requests with different adapters share a batch.
 """
 from __future__ import annotations
 
@@ -44,11 +46,17 @@ def logprobs_param(par):
     return None if par is None else par.get("logprobs")
 
 
+def adapter_param(par):
+    """The LoRA adapter a request's params name, or None."""
+    return None if par is None else par.get("adapter")
+
+
 def decoding_params(par):
-    """A request's params without `logprobs`, which never changes its tokens: None (greedy) when that was its only key."""
-    if par is None or "logprobs" not in par:
+    """A request's params without `logprobs` and `adapter`, which are not decoding parameters: None (greedy) when those
+    were its only keys."""
+    if par is None or ("logprobs" not in par and "adapter" not in par):
         return par
-    rest = {k: v for k, v in par.items() if k != "logprobs"}
+    rest = {k: v for k, v in par.items() if k not in ("logprobs", "adapter")}
     return rest or None
 
 
@@ -67,12 +75,13 @@ def processing_params(par):
     return {k: v for k, v in par.items() if k in PROCESSING_KEYS}
 
 
-def parse_requests(requests):
+def parse_requests(requests, adapters=()):
     """requests: (prompt ids, max_new_tokens) or (prompt ids, max_new_tokens, params) with params a dict of temperature,
     top_k, top_p, seed (missing keys: 1.0, 50, 1.0, 0, as generate(do_sample=True); the seed is the request's Philox key)
     and of repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens (missing keys: 1.0, 0.0, 0.0, 0;
     processing_rows), and `logprobs`: an int N, 0 <= N <= 20, the number of top log-probabilities wanted with each token.
-    A request whose params hold processing keys or `logprobs` only is greedy.
+    `adapter`: the name of a LoRA adapter, one of `adapters` (the model's loaded adapters; None: any string).
+    A request whose params hold processing keys, `logprobs` or `adapter` only is greedy.
     Returns ([(prompt int64 1-D on the host, max_new_tokens)], [params or None]); ValueError for an empty prompt, a budget
     below 1, an unknown key or a value outside its range."""
     reqs, params = [], []
@@ -85,12 +94,15 @@ def parse_requests(requests):
         reqs.append((p, int(r[1])))
         par = r[2] if len(r) == 3 else None
         if par is not None:
-            unknown = set(par) - set(SAMPLING_KEYS) - set(PROCESSING_KEYS) - {"logprobs"}
+            unknown = set(par) - set(SAMPLING_KEYS) - set(PROCESSING_KEYS) - {"logprobs", "adapter"}
             if unknown:
                 raise ValueError(f"request {i}: unknown sampling parameters {sorted(unknown)}")
             n = par.get("logprobs", 0)
             if isinstance(n, bool) or not isinstance(n, int) or not 0 <= n <= MAX_LOGPROBS:
                 raise ValueError(f"request {i}: logprobs: expected an int in [0, {MAX_LOGPROBS}], got {n!r}")
+            if "adapter" in par and (not isinstance(par["adapter"], str) or
+                                     (adapters is not None and par["adapter"] not in adapters)):
+                raise ValueError(f"request {i}: adapter {par['adapter']!r} is not loaded (loaded: {sorted(adapters)})")
             sampling_rows(1, **{k: v for k, v in par.items() if k in SAMPLING_KEYS})   # ValueError outside its range
             processing_rows(1, **{k: v for k, v in par.items() if k in PROCESSING_KEYS})
             par = dict(par)
@@ -144,10 +156,15 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     there (of at least prefix.MIN_REUSE tokens) and stores the rest of its prompt; stats counts the inserts that reused
     one (prefix_hits) and their reused tokens (prefix_tokens).  The caller owns the cache, so it may outlive the call
     (the next turn of a conversation starts with the previous prompt).  The first group's left-padded prefill neither
-    uses nor fills it."""
-    reqs, params = parse_requests(requests)
+    uses nor fills it.
+    A request's `adapter` names a LoRA adapter loaded into the model; its prompt pass and its slot's decode steps apply it,
+    and a stored prefix is reused only by requests with the same adapter.  An unknown name is a ValueError before any work."""
+    reqs, params = parse_requests(requests, adapters=None)
     if not reqs:
         return
+    lora = [adapter_param(par) for par in params]
+    if any(a is not None for a in lora):                                  # the names, before any work
+        parse_requests(requests, model.adapters)
     lp_n = [logprobs_param(par) for par in params]
     params = [decoding_params(par) for par in params]
     samp = [sampling_params(par) for par in params]
@@ -167,6 +184,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     cache = model.cache
     if cache is None or cache.batch != batch or cache.max_tokens != max_tokens:
         cache = model.init_cache(batch, max_tokens)
+    loaded = bool(model.adapters)                                         # LoRA: every slot's adapter is set below
     quantum = max(128, cache.residual_length)
     dev = cache.device
     # serve() owns the step's mode: sampling with every slot greedy until a sampled request takes it, or the greedy step
@@ -247,6 +265,8 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
             n = reqs[i][0].numel()
             ids[b, P - n:] = reqs[i][0]
             mask[b, P - n:] = 1
+        if loaded:
+            model.set_adapters([lora[i] for i in rows] + [None] * (batch - len(rows)))
         ids, mask = ids.to(dev), mask.to(dev)
         logits = model.prefill(ids, attention_mask=mask)
         cache.set_kv_start(kv_start_from_mask(mask))                      # ragged from the start: one step graph
@@ -279,7 +299,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
                     i = queue.popleft()
                     if prefix_cache is not None:
                         hits, reused = prefix_cache.hits, prefix_cache.reused_tokens
-                    tok = first_token(model.insert(slot, p.to(dev), prefix_cache), slot, i)
+                    tok = first_token(model.insert(slot, p.to(dev), prefix_cache, adapter=lora[i]), slot, i)
                     if prefix_cache is not None:
                         stats["prefix_hits"] += prefix_cache.hits - hits
                         stats["prefix_tokens"] += prefix_cache.reused_tokens - reused
