@@ -169,7 +169,7 @@ def sample(logits, temperature, top_k, top_p, seed, draw, next_local, ids_feedba
     temperature[b] == 0 is the greedy id and leaves draw[b] alone.  All operands are device tensors of B elements: the kernel
     reads them, so a captured call follows later changes.  include/kivi_b200.h (kivi_sample_f32) has the exact rules.
     The parameter VALUES are not checked here (that would read the device and break a capture): callers validate them on the
-    host before uploading, as llama_kivi.sampling_rows does; the kernel takes a row whose temperature is not > 0 as greedy.
+    host before uploading, as choice.sampling_rows does; the kernel takes a row whose temperature is not > 0 as greedy.
     dbg_u (fp32) / dbg_kept (int32): optional outputs, the uniform number and the size of the kept set."""
     _bind()
     if logits.dim() != 2:
@@ -217,7 +217,7 @@ def logits_process(logits, scores, counts, seen, n_new, finished, repetition, pr
     suppression while n_new[b] < min_new[b], and the masking of `finished` rows to pad_id; include/kivi_b200.h
     (kivi_logits_process_f32) has the exact rules.  repetition / presence / frequency fp32 [B], min_new / n_new int32 [B],
     finished uint8 [B], eos int64 [<= 8] or None.  The kernel reads every state and parameter on the device, so a captured
-    call follows later changes; the parameter VALUES are checked on the host by llama_kivi.processing_rows."""
+    call follows later changes; the parameter VALUES are checked on the host by choice.processing_rows."""
     _bind()
     if logits.dim() != 2:
         raise ValueError(f"logits: expected [B, vocab], got shape {tuple(logits.shape)}")

@@ -28,6 +28,7 @@ import torch.nn.functional as F
 
 from . import glue
 from .cache import KiviCache, kv_start_from_mask
+from .choice import TokenChoice, processing_rows, sampling_rows
 from .matmul import cuda_bmm_fA_qB_outer
 from .new_pack import triton_quantize_and_pack_along_last_dim
 from .tp import check_divisible, shard_of, shard_state_dict, shard_tensor, sum_partials  # noqa: F401 (re-export)
@@ -576,94 +577,6 @@ def _additive_mask(attention_mask, q_len: int, total: int, dtype, device, window
     return torch.zeros(keep.shape, dtype=dtype, device=device).masked_fill(~keep, torch.finfo(dtype).min)
 
 
-def sampling_rows(n: int, temperature=1.0, top_k=50, top_p=1.0, seed=0):
-    """The sampling parameters of n batch rows as four lists (temperature, top_k, top_p, seed), from scalars or length-n
-    sequences.  An int seed gives row b the Philox key seed + b (mod 2^64); a sequence gives row b its own key.
-    temperature >= 0 (0 = greedy), top_k an int (<= 0 = off), 0 <= top_p <= 1; anything else is a ValueError."""
-    import math
-
-    def rows(name, v, conv):
-        vals = list(v) if isinstance(v, (list, tuple)) or (torch.is_tensor(v) and v.dim() > 0) else [v] * n
-        if len(vals) != n:
-            raise ValueError(f"{name}: expected a scalar or {n} values, got {len(vals)}")
-        try:
-            return [conv(x) for x in vals]
-        except (TypeError, OverflowError) as e:
-            raise ValueError(f"{name}: {e}") from None
-
-    def integer(x):
-        if isinstance(x, bool) or int(x) != x:
-            raise ValueError(f"expected an integer, got {x!r}")
-        return int(x)
-
-    t, p = rows("temperature", temperature, float), rows("top_p", top_p, float)
-    k = rows("top_k", top_k, integer)
-    if isinstance(seed, (list, tuple)) or (torch.is_tensor(seed) and seed.dim() > 0):
-        sd = rows("seed", seed, integer)
-    else:
-        sd = [integer(seed) + b for b in range(n)]
-    for b in range(n):
-        if not (math.isfinite(t[b]) and t[b] >= 0.0):
-            raise ValueError(f"temperature: expected a finite value >= 0 (0 = greedy), got {t[b]}")
-        if not 0.0 <= p[b] <= 1.0:
-            raise ValueError(f"top_p: expected a value in [0, 1], got {p[b]}")
-        if not -2 ** 31 <= k[b] < 2 ** 31:
-            raise ValueError(f"top_k: {k[b]} is not an int32")
-        if sd[b] < 0:
-            raise ValueError(f"seed: expected a non-negative integer, got {sd[b]}")
-        sd[b] %= 2 ** 64
-    return t, k, p, sd
-
-
-PROCESSING_KEYS = ("repetition_penalty", "presence_penalty", "frequency_penalty", "min_new_tokens")
-
-
-def processing_rows(n: int, repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_new_tokens=0,
-                    eos_token_id=None, vocab: int | None = None):
-    """The logits-processing parameters of n batch rows as four lists (repetition, presence, frequency, min_new), from
-    scalars or length-n sequences, and the EOS ids as a list (an int, a sequence of at most 8, or None = []).
-    repetition_penalty > 0 and finite (1 = off), presence_penalty and frequency_penalty in [-2, 2] (0 = off),
-    min_new_tokens an int >= 0, EOS ids integers inside [0, vocab) (vocab None: >= 0); anything else is a ValueError."""
-    import math
-
-    def rows(name, v, conv):
-        vals = list(v) if isinstance(v, (list, tuple)) or (torch.is_tensor(v) and v.dim() > 0) else [v] * n
-        if len(vals) != n:
-            raise ValueError(f"{name}: expected a scalar or {n} values, got {len(vals)}")
-        try:
-            return [conv(x) for x in vals]
-        except (TypeError, OverflowError, ValueError) as e:
-            raise ValueError(f"{name}: {e}") from None
-
-    def integer(x):
-        if isinstance(x, bool) or int(x) != x:
-            raise ValueError(f"expected an integer, got {x!r}")
-        return int(x)
-
-    rep, pres = rows("repetition_penalty", repetition_penalty, float), rows("presence_penalty", presence_penalty, float)
-    freq, mn = rows("frequency_penalty", frequency_penalty, float), rows("min_new_tokens", min_new_tokens, integer)
-    for b in range(n):
-        if not (math.isfinite(rep[b]) and rep[b] > 0.0):
-            raise ValueError(f"repetition_penalty: expected a finite value > 0 (1 = off), got {rep[b]}")
-        for name, v in (("presence_penalty", pres[b]), ("frequency_penalty", freq[b])):
-            if not -2.0 <= v <= 2.0:
-                raise ValueError(f"{name}: expected a value in [-2, 2], got {v}")
-        if not 0 <= mn[b] < 2 ** 31:
-            raise ValueError(f"min_new_tokens: expected an int32 >= 0, got {mn[b]}")
-    eos = [] if eos_token_id is None else eos_token_id
-    eos = list(eos) if isinstance(eos, (list, tuple)) or (torch.is_tensor(eos) and eos.dim() > 0) else [eos]
-    try:
-        eos = [integer(e) for e in eos]
-    except (TypeError, OverflowError, ValueError) as e:
-        raise ValueError(f"eos_token_id: {e}") from None
-    if len(eos) > 8:
-        raise ValueError(f"eos_token_id: at most 8 ids, got {len(eos)}")
-    for e in eos:
-        if e < 0 or (vocab is not None and e >= vocab):
-            raise ValueError(f"eos_token_id: {e} is outside the vocabulary" + (f" [0, {vocab})" if vocab else ""))
-    return rep, pres, freq, mn, eos
-
-
 def _processing_args(n: int, repetition_penalty=None, min_length=None, min_new_tokens=None, eos_token_id=None,
                      pad_token_id=None):
     """generate()'s logits-processing arguments (prompt of n positions, left padding included, as transformers counts
@@ -754,9 +667,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._dist_in_graph = True
         self._exchange = None               # kivi_b200.dist.PeerTokenExchange: ids stored into the peers' buffers by the sampling kernel
         self._allreduce = None              # kivi_b200.dist.PeerAllReduce of the tensor-parallel decode step
-        self._sampling = False              # the step's last kernel samples (set_sampling) instead of taking the argmax
-        self._logprobs_n = None             # set_logprobs(): the step's top-N logprobs (None: off)
-        self.logprobs = self.top_ids = self.top_logprobs = None
+        self.choice: TokenChoice | None = None   # the cache's rows' sampling, logits processing and logprobs (init_cache)
         self._lora = None                   # kivi_b200.lora.LoraState once an adapter is loaded (load_adapter)
         self._adapter_sel = None            # set_adapters(): None, one slot, or a slot per row
         self._adapter_idx = None            # int32 [batch]: each cache row's adapter slot (-1: none), read by the step
@@ -1022,7 +933,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         dev, dtype = self.lm_head.weight.device, self.lm_head.weight.dtype
         if dtype != torch.float16:
             raise ValueError(f"the fused KIVI cache path needs fp16 weights, the model's are {dtype}: call .half() first")
-        self.cache, self._graph = None, None                 # release the previous cache before the new one is allocated
+        n_top = None if self.choice is None else self.choice.n_top
+        self.cache, self._graph, self.choice = None, None, None   # release the previous cache before the new one is allocated
         a = self.model.layers[0].self_attn                  # this rank's heads
         self.cache = KiviCache(cfg.num_hidden_layers, batch, a.num_heads, a.num_key_value_heads,
                                a.head_dim, cfg.k_bits, cfg.v_bits, cfg.group_size,
@@ -1040,19 +952,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._ids = torch.zeros((batch, 1), dtype=torch.long, device=dev)
         self._logits = torch.zeros((batch, cfg.vocab_size), dtype=torch.float32, device=dev)
         self.next_tokens = torch.zeros((batch,), dtype=torch.long, device=dev)   # the step's argmax or sample (in-graph)
-        # per-slot sampling parameters, read by the sampling kernel on the device (seed / draw: uint64 bits); greedy until
-        # set_sampling()
-        self._sampling = False
-        self._samp = SimpleNamespace(temperature=torch.zeros(batch, dtype=torch.float32, device=dev),
-                                     top_k=torch.zeros(batch, dtype=torch.int32, device=dev),
-                                     top_p=torch.ones(batch, dtype=torch.float32, device=dev),
-                                     seed=torch.zeros(batch, dtype=torch.long, device=dev),
-                                     draw=torch.zeros(batch, dtype=torch.long, device=dev))
-        # logits processing (set_processing): off, and its per-row state unallocated, until asked for
-        self._processing, self._proc = False, None
-        # log-probabilities of the chosen tokens (set_logprobs): the mode outlives the cache, its buffers take the new batch
-        n_top, self._logprobs_n = self._logprobs_n, None
-        self.logprobs = self.top_ids = self.top_logprobs = None
+        # greedy and without processing until set_sampling() / set_processing(); the logprobs mode outlives the cache
+        self.choice = TokenChoice(batch, cfg.vocab_size, dev)
+        self.choice.set_logprobs(n_top)
         self._tables(dev)                                   # rows for every position the cache can reach
         self._adapter_idx = torch.full((batch,), -1, dtype=torch.int32, device=dev)
         if self._lora is not None:
@@ -1062,8 +964,6 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 self._adapter_idx.fill_(sel)
             elif sel is not None and len(sel) == batch:
                 self._adapter_idx.copy_(torch.tensor(sel, dtype=torch.int32))
-        if n_top is not None:
-            self.set_logprobs(n_top)
         return self.cache
 
     def import_cache(self, past_key_values, max_tokens: int | None = None):
@@ -1105,8 +1005,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             starts = kv_start_from_mask(attention_mask)
             if not bool(starts.any()):
                 starts = None
-        if self._processing:
-            self._mark_prompt(input_ids, starts, slice(None), copies)
+        self.choice.mark_prompt(input_ids, starts, slice(None), copies)
         rows = None if self._lora is None else self._adapter_idx[::copies].contiguous()     # prompt b's adapter
         if starts is None:
             positions = torch.arange(n, device=input_ids.device).unsqueeze(0).expand(B, -1)
@@ -1165,8 +1064,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             prefix_cache.insert(*record)
         self._pos[seq] = n
         self.cache.set_seq_start(seq, T - n)
-        if self._processing:
-            self._mark_prompt(ids, None, slice(seq, seq + 1))
+        self.choice.mark_prompt(ids, None, slice(seq, seq + 1))
         return self.lm_head(h[0, -1]).float()
 
     def _prefix_insert(self, prefix_cache, ids, refill, adapter=None):
@@ -1211,29 +1109,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._pos[seq] = 0
         if self._lora is not None:
             self._adapter_idx[seq] = -1
-        if self._processing:
-            p = self._proc
-            for t in (p.seen, p.counts, p.n_new, p.finished):
-                t[seq].zero_()
-
-    def _mark_prompt(self, ids, starts, rows, copies: int = 1):
-        """Logits processing: the prompt ids [r, n] become the prompt bits of the batch rows `rows` (a slice of r * copies
-        rows; row j gets prompt j // copies), counting position i of prompt j only when i >= starts[j] (None: 0), so left
-        padding is not penalised.  The rows' generated counts, n_new and finished flags start from 0."""
-        p, V = self._proc, self.config.vocab_size
-        r, n = ids.shape
-        words = p.seen.shape[1]
-        live = ids.clamp(0, V - 1)
-        if starts is not None:
-            pos = torch.arange(n, device=ids.device).view(1, n)
-            live = torch.where(pos >= starts.to(ids.device).view(r, 1), live, words * 32)    # a column past the bits
-        hit = torch.zeros((r, words * 32 + 1), dtype=torch.bool, device=ids.device)
-        hit.scatter_(1, live, True)
-        w = (hit[:, :-1].view(r, words, 32).long() << torch.arange(32, device=ids.device)).sum(-1)
-        w = torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)                    # the uint32 words' bits
-        p.seen[rows] = w.repeat_interleave(copies, 0)
-        for t in (p.counts, p.n_new, p.finished):
-            t[rows].zero_()
+        self.choice.release(seq)
 
     @torch.no_grad()
     def prefill_synthetic(self, n: int, seed: int = 0):
@@ -1274,48 +1150,25 @@ class LlamaForCausalLM_KIVI(nn.Module):
         greedy.  set_sampling(None) returns the whole step to the greedy kernel.  The captured step is dropped when the
         mode changes, not when only parameters do.  Under tensor parallelism every rank calls this with the same arguments."""
         assert self.cache is not None, "call init_cache() first"
-        on = temperature is not None
-        if on:
-            if self._exchange is not None:
-                raise NotImplementedError(_P2P_SAMPLING)
-            t, k, p, sd = sampling_rows(self.cache.batch, temperature, top_k, top_p, seed)
-            s, dev = self._samp, self.cache.device
-            s.temperature.copy_(torch.tensor(t, dtype=torch.float32).to(dev))
-            s.top_k.copy_(torch.tensor(k, dtype=torch.int32).to(dev))
-            s.top_p.copy_(torch.tensor(p, dtype=torch.float32).to(dev))
-            s.seed.copy_(torch.tensor([x - 2 ** 64 if x >= 2 ** 63 else x for x in sd], dtype=torch.long).to(dev))
-            s.draw.zero_()
-        if on != self._sampling:
-            self._sampling, self._graph = on, None
+        if temperature is not None and self._exchange is not None:
+            raise NotImplementedError(_P2P_SAMPLING)
+        if self.choice.set_sampling(temperature, top_k, top_p, seed):
+            self._graph = None
 
     def set_slot_sampling(self, seq: int, temperature=1.0, top_k=50, top_p=1.0, seed=0):
         """The sampling parameters of batch row `seq` alone (a slot given to a new request), its draw counter back to 0; the
         row's key is `seed` itself.  The captured step reads them on the device: no recapture."""
-        if not self._sampling:
-            raise RuntimeError("set_slot_sampling: the step is greedy; call set_sampling() first")
-        if not 0 <= seq < self.cache.batch:
-            raise ValueError(f"seq {seq} outside the batch of {self.cache.batch}")
-        t, k, p, sd = sampling_rows(1, temperature, top_k, top_p, seed)
-        s = self._samp
-        s.temperature[seq], s.top_k[seq], s.top_p[seq] = t[0], k[0], p[0]
-        s.seed[seq] = sd[0] - 2 ** 64 if sd[0] >= 2 ** 63 else sd[0]
-        s.draw[seq] = 0
+        self.choice.set_slot_sampling(seq, temperature, top_k, top_p, seed)
 
     def sample_first(self, logits, seq: int | None = None):
         """first_tokens() under sampling: the prompt's last-position logits ([B, vocab] of prefill, or [vocab] of
         insert(seq)) go through the step's own sampling kernel with the rows' parameters and consume their next draw
         (draw 0 after set_sampling / set_slot_sampling).  Rank 0's ids under tensor parallelism, like first_tokens."""
-        from . import glue
         if not self._sampling:
             raise RuntimeError("sample_first: the step is greedy; call set_sampling() first")
-        s = self._samp
-        rows = slice(None) if seq is None else slice(seq, seq + 1)
         logits = logits.reshape(-1, logits.shape[-1]).float().contiguous()
         tok = torch.empty(logits.shape[0], dtype=torch.long, device=logits.device)
-        glue.sample(logits, s.temperature[rows], s.top_k[rows], s.top_p[rows], s.seed[rows], s.draw[rows], tok)
-        if self.tensor_parallel and self.tp_world > 1:
-            import torch.distributed as dist
-            dist.broadcast(tok, src=0)
+        tok = self._rank0(self.choice.sample(logits, slice(None) if seq is None else slice(seq, seq + 1), tok))
         return tok if seq is None else tok[0]
 
     # ------------------------------------------------------------------ logits processing
@@ -1332,49 +1185,15 @@ class LlamaForCausalLM_KIVI(nn.Module):
         dropped when processing turns on or off or pad_token_id changes, not when the other parameters do.  Under tensor
         parallelism every rank calls this with the same arguments."""
         assert self.cache is not None, "call init_cache() first"
-        on = repetition_penalty is not None
-        if on:
-            B, V, dev = self.cache.batch, self.config.vocab_size, self.cache.device
-            rep, pres, freq, mn, eos = processing_rows(B, repetition_penalty, presence_penalty, frequency_penalty,
-                                                       min_new_tokens, eos_token_id, V)
-            pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
-            if isinstance(pad, bool) or int(pad) != pad or not 0 <= int(pad) < V:
-                raise ValueError(f"pad_token_id: expected an id inside the vocabulary [0, {V}), got {pad!r}")
-            p = self._proc
-            if p is None:
-                i32 = dict(dtype=torch.int32, device=dev)
-                p = self._proc = SimpleNamespace(
-                    counts=torch.zeros((B, V), **i32), seen=torch.zeros((B, (V + 31) // 32), **i32),
-                    n_new=torch.zeros(B, **i32), finished=torch.zeros(B, dtype=torch.uint8, device=dev),
-                    repetition=torch.ones(B, dtype=torch.float32, device=dev),
-                    presence=torch.zeros(B, dtype=torch.float32, device=dev),
-                    frequency=torch.zeros(B, dtype=torch.float32, device=dev), min_new=torch.zeros(B, **i32),
-                    eos=torch.full((8,), -1, dtype=torch.long, device=dev),   # -1 matches no token: a fixed-size list
-                    scores=torch.empty((B, V), dtype=torch.float32, device=dev), pad=None, stops=False)
-            p.repetition.copy_(torch.tensor(rep, dtype=torch.float32).to(dev))
-            p.presence.copy_(torch.tensor(pres, dtype=torch.float32).to(dev))
-            p.frequency.copy_(torch.tensor(freq, dtype=torch.float32).to(dev))
-            p.min_new.copy_(torch.tensor(mn, dtype=torch.int32).to(dev))
-            p.eos.copy_(torch.tensor(eos + [-1] * (8 - len(eos)), dtype=torch.long).to(dev))
-            p.stops = bool(eos)
-            if p.pad != int(pad):
-                p.pad, self._graph = int(pad), None
-        else:
-            self._proc = None
-        if on != self._processing:
-            self._processing, self._graph = on, None
+        if self.choice.set_processing(repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens, eos_token_id,
+                                      pad_token_id):
+            self._graph = None
 
     def set_slot_processing(self, seq: int, repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0,
                             min_new_tokens=0):
         """The processing parameters of batch row `seq` alone (a slot given to a new request); its counts, length and flag
         are reset by insert().  The captured step reads them on the device: no recapture."""
-        if not self._processing:
-            raise RuntimeError("set_slot_processing: processing is off; call set_processing() first")
-        if not 0 <= seq < self.cache.batch:
-            raise ValueError(f"seq {seq} outside the batch of {self.cache.batch}")
-        rep, pres, freq, mn, _ = processing_rows(1, repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens)
-        p = self._proc
-        p.repetition[seq], p.presence[seq], p.frequency[seq], p.min_new[seq] = rep[0], pres[0], freq[0], mn[0]
+        self.choice.set_slot_processing(seq, repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens)
 
     def choose_first(self, logits, seq: int | None = None, return_scores: bool = False):
         """The first token(s) from the prompt's last-position logits ([B, vocab] of prefill, or [vocab] of insert(seq)), as
@@ -1382,25 +1201,16 @@ class LlamaForCausalLM_KIVI(nn.Module):
         (sample_first), then recorded; with set_logprobs() on, the rows' logprobs buffers receive the raw log-probabilities
         of these tokens.  Returns [B] ids, or a 0-d id for `seq`; return_scores: (ids, the scores the choice read, in the
         shape of `logits`: the processed ones, or `logits` itself with processing off)."""
-        from . import glue
-        p = self._proc if self._processing else None
-        rows = slice(None) if seq is None else slice(seq, seq + 1)
-        raw = logits
-        if p is not None:
-            flat = logits.reshape(-1, logits.shape[-1]).float().contiguous()
-            scores = torch.empty_like(flat)
-            glue.logits_process(flat, scores, p.counts[rows], p.seen[rows], p.n_new[rows], p.finished[rows],
-                                p.repetition[rows], p.presence[rows], p.frequency[rows], p.min_new[rows], p.eos, p.pad)
-            logits = scores if seq is None else scores[0]
-        tok = self.sample_first(logits, seq) if self._sampling else self.first_tokens(logits)
-        if p is not None:
-            glue.logits_record(tok.reshape(-1), p.counts[rows], p.n_new[rows], p.finished[rows], p.eos)
-        if self._logprobs_n is not None:
-            top = self._logprobs_n > 0
-            glue.token_logprobs(raw.reshape(-1, raw.shape[-1]).float().contiguous(), tok.reshape(-1),
-                                self.logprobs[rows], self.top_ids[rows] if top else None,
-                                self.top_logprobs[rows] if top else None)
-        return (tok, logits) if return_scores else tok
+        flat = logits.reshape(-1, logits.shape[-1]).float().contiguous()
+
+        def pick(scores):
+            if self._sampling:
+                return self.sample_first(scores, seq)
+            return self.first_tokens(scores if seq is None else scores[0])
+        tok, scores = self.choice.choose(flat, slice(None) if seq is None else slice(seq, seq + 1), pick)
+        if not return_scores:
+            return tok
+        return tok, logits if scores is None else scores if seq is None else scores[0]
 
     # ------------------------------------------------------------------ log-probabilities
     def set_logprobs(self, n_top=0):
@@ -1414,21 +1224,15 @@ class LlamaForCausalLM_KIVI(nn.Module):
         captured step is dropped when the mode turns on or off or n_top changes.  Under tensor parallelism every rank
         computes the same values (the logits are replicated)."""
         assert self.cache is not None, "call init_cache() first"
-        if n_top is not None:
-            from .glue import MAX_TOP_LOGPROBS
-            if isinstance(n_top, bool) or int(n_top) != n_top or not 0 <= int(n_top) <= MAX_TOP_LOGPROBS:
-                raise ValueError(f"n_top: expected an int in [0, {MAX_TOP_LOGPROBS}], got {n_top!r}")
-            n_top = int(n_top)
-        if n_top == self._logprobs_n:
-            return
-        self._logprobs_n, self._graph = n_top, None
-        if n_top is None:
-            self.logprobs = self.top_ids = self.top_logprobs = None
-        else:
-            B, dev = self.cache.batch, self.cache.device
-            self.logprobs = torch.zeros(B, dtype=torch.float32, device=dev)
-            self.top_ids = torch.zeros((B, n_top), dtype=torch.long, device=dev)
-            self.top_logprobs = torch.zeros((B, n_top), dtype=torch.float32, device=dev)
+        if self.choice.set_logprobs(n_top):
+            self._graph = None
+
+    logprobs = property(lambda self: None if self.choice is None else self.choice.logprobs)
+    top_ids = property(lambda self: None if self.choice is None else self.choice.top_ids)
+    top_logprobs = property(lambda self: None if self.choice is None else self.choice.top_logprobs)
+    _sampling = property(lambda self: self.choice.sampling)     # the token choice's modes and state, read by the step
+    _samp = property(lambda self: self.choice.samp)
+    _proc = property(lambda self: self.choice.proc)
 
     # ------------------------------------------------------------------ LoRA adapters
     def load_adapter(self, path, adapter_name: str):
@@ -1624,31 +1428,19 @@ class LlamaForCausalLM_KIVI(nn.Module):
         self._logits.copy_(f.logits16)                                       # logits.float() (:881)
         cache._enqueue_advance()                             # decode_step advances the host mirror after each replay
         self._pos.add_(1)
-        logits, p = self._logits, self._proc if self._processing else None
-        if p is not None:
-            # logits processing (set_processing): the choice reads the processed scores, decode_step returns the raw logits
-            glue.logits_process(logits, p.scores, p.counts, p.seen, p.n_new, p.finished, p.repetition, p.presence,
-                                p.frequency, p.min_new, p.eos, p.pad)
-            logits = p.scores
+
         # greedy sampling inside the step (and inside its CUDA graph): the argmax of a sequence needs only that
         # sequence's logits, so with data-parallel replicas the exchange is the sampled ids, 8 B per sequence
-        if self._sampling:
-            # in the argmax kernel's place, one kernel as well: a draw per sequence from its own parameters, seed and counter
-            s = self._samp
-            glue.sample(logits, s.temperature, s.top_k, s.top_p, s.seed, s.draw, self.next_tokens, self._ids.view(-1))
-        else:
+        def pick(scores):
+            if self._sampling:            # in the argmax kernel's place, one kernel as well: a draw per sequence
+                return self.choice.sample(scores, slice(None), self.next_tokens, self._ids.view(-1))
             if self._exchange is not None:
                 self._exchange.step.add_(1)                  # the step number the peers' arrival counters are compared with
             # one kernel: argmax per sequence, the feed-back copy for the next step, and (replicas) the ids stored straight
             # into every peer's buffer over NVLink + arrival counters
-            glue.greedy_sample(logits, self.next_tokens, self._ids.view(-1), self._exchange)
-        if self._logprobs_n is not None:
-            # log-probabilities of the chosen ids under the raw logits (set_logprobs); one more launch
-            top = self._logprobs_n > 0
-            glue.token_logprobs(self._logits, self.next_tokens, self.logprobs, self.top_ids if top else None,
-                                self.top_logprobs if top else None)
-        if p is not None:
-            glue.logits_record(self.next_tokens, p.counts, p.n_new, p.finished, p.eos)
+            return glue.greedy_sample(scores, self.next_tokens, self._ids.view(-1), self._exchange)
+        # with processing, the choice reads the processed scores; decode_step returns the raw logits
+        self.choice.choose(self._logits, None, pick)
         if self._dist_tokens is not None and self._dist_in_graph:
             from . import dist as kdist
             kdist.gather_tokens(self.next_tokens, out=self._dist_tokens)
@@ -1656,7 +1448,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
     def first_tokens(self, logits):
         """Greedy ids of prompt logits (prefill / insert) -- under tensor parallelism rank 0's, broadcast, so the ranks can
         never start from different tokens."""
-        tok = logits.argmax(-1)
+        return self._rank0(logits.argmax(-1))
+
+    def _rank0(self, tok):
         if self.tensor_parallel and self.tp_world > 1:
             import torch.distributed as dist
             dist.broadcast(tok, src=0)
@@ -1681,28 +1475,17 @@ class LlamaForCausalLM_KIVI(nn.Module):
                 self._graph = None                                           # captured with the other attention entry
             if self._graph is None:
                 # warm-up on a side stream (cuBLAS workspaces, lazy module loading, NCCL channels), then capture
-                state = self.cache.state.clone()
-                pos, ids0 = self._pos.clone(), self._ids.clone()
-                draw = self._samp.draw.clone() if self._sampling else None
-                proc = self._proc if self._processing else None
-                proc_state = [proc.counts.clone(), proc.n_new.clone(), proc.finished.clone()] if proc is not None else None
+                saved = self.choice.snapshot(self.cache.state, self._pos, self._ids)
                 s = torch.cuda.Stream()
                 s.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(s):
                     self._step_body()
                 torch.cuda.current_stream().wait_stream(s)
                 torch.cuda.synchronize()
-                # undo the warm-up step's effect on the lengths.  Everything it wrote lies BEYOND them -- the new token's
-                # window slots (K slot r, the free slot of the V ring), a flushed K block past tk, the packed V token at
-                # tv -- and is rewritten with the same bytes by the first replayed step.
-                self.cache.state.copy_(state)
-                self._pos.copy_(pos)
-                self._ids.copy_(ids0)
-                if draw is not None:
-                    self._samp.draw.copy_(draw)                              # the warm-up step consumed a draw per row
-                if proc_state is not None:                                   # and recorded a token per row
-                    for t, saved in zip((proc.counts, proc.n_new, proc.finished), proc_state):
-                        t.copy_(saved)
+                # undo the warm-up step's effect on the lengths, positions, ids and token choice.  Everything it wrote
+                # lies BEYOND the lengths -- the new token's window slots (K slot r, the free slot of the V ring), a flushed
+                # K block past tk, the packed V token at tv -- and is rewritten with the same bytes by the first replay.
+                self.choice.restore(saved)
                 from . import _lib
                 n0 = _lib.launch_count()
                 g = torch.cuda.CUDAGraph()
@@ -1782,22 +1565,33 @@ class LlamaForCausalLM_KIVI(nn.Module):
         trace = SimpleNamespace(scores=[] if output_scores else None, logits=[] if output_logits else None)
         proc = _processing_args(input_ids.shape[1], repetition_penalty, min_length, min_new_tokens, eos_token_id,
                                 pad_token_id)
+        sampling = (temperature, top_k, top_p, seed) if do_sample else None
         if num_beams != 1 or num_return_sequences != 1:
             if num_beams > 1 and proc is not None and (proc["repetition_penalty"] != 1.0 or proc["min_new_tokens"]):
                 raise NotImplementedError("repetition_penalty, min_length and min_new_tokens in beam search are not "
                                           "supported: transformers applies them to log-probabilities there")
-            return self._generate_many(input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample,
-                                       temperature, top_k, top_p, seed, num_beams, num_return_sequences, length_penalty,
-                                       early_stopping, eos_token_id, pad_token_id, return_dict_in_generate, proc, trace,
-                                       names)
-        if do_sample:
-            sampling_rows(input_ids.shape[0], temperature, top_k, top_p, seed)   # ValueError before any work
+            return self._generate_many(input_ids, max_new_tokens, use_graph, attention_mask, max_length, sampling,
+                                       num_beams, num_return_sequences, length_penalty, early_stopping, eos_token_id,
+                                       pad_token_id, return_dict_in_generate, proc, trace, names)
+        max_new_tokens = self._generate_setup(input_ids, 1, max_new_tokens, max_length, attention_mask, sampling, proc,
+                                              names)
+        logits = self.prefill(input_ids, attention_mask)
+        tok, scores = self.choose_first(logits, return_scores=True)
+        _trace_add(trace, logits, scores)
+        seq = torch.cat([input_ids, self._decode(tok.view(-1, 1), max_new_tokens, use_graph, trace)], 1)
+        return _generate_output(seq, trace) if return_dict_in_generate else seq
+
+    def _generate_setup(self, input_ids, copies: int, max_new_tokens, max_length, attention_mask, sampling, proc, names):
+        """generate()'s set-up for `copies` rows per prompt: the argument checks (ValueError before any work), the cache,
+        the RoPE tables, the modes (sampling: set_sampling's arguments, proc: set_processing's; None: off) and the rows'
+        adapters (a prompt's copies take its adapter).  Returns max_new_tokens."""
+        n, rows = input_ids.shape[1], input_ids.shape[0] * copies
+        if sampling is not None:
+            sampling_rows(rows, *sampling)
         if proc is not None:
-            processing_rows(input_ids.shape[0], proc["repetition_penalty"], eos_token_id=proc["eos_token_id"],
-                            vocab=self.config.vocab_size)
+            processing_rows(rows, proc["repetition_penalty"], eos_token_id=proc["eos_token_id"], vocab=self.config.vocab_size)
         if attention_mask is not None:
             kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
-        B, n = input_ids.shape
         if max_new_tokens is None:
             if max_length is None:
                 raise ValueError("generate() needs max_new_tokens or max_length")
@@ -1805,12 +1599,12 @@ class LlamaForCausalLM_KIVI(nn.Module):
         cap = n + max_new_tokens
         if self.sliding_window is not None:
             cap = min(cap, max(n, self.sliding_window) + 2 * max(128, self.config.residual_length))
-        if self.cache is None or self.cache.batch != B or self.cache.max_tokens < cap:
-            self.init_cache(B, cap)
+        if self.cache is None or self.cache.batch != rows or self.cache.max_tokens < cap:
+            self.init_cache(rows, cap)
         self._tables(self.cache.device, n + max_new_tokens)                 # positions beyond a rolling cache
         # generate() owns the step's mode; it changes (and the captured step is dropped) only when do_sample does
-        if do_sample:
-            self.set_sampling(temperature, top_k, top_p, seed)
+        if sampling is not None:
+            self.set_sampling(*sampling)
         else:
             self.set_sampling(None)
         if proc is not None:
@@ -1818,12 +1612,8 @@ class LlamaForCausalLM_KIVI(nn.Module):
         else:
             self.set_processing(None)
         if self._lora is not None:
-            self.set_adapters(names)
-        logits = self.prefill(input_ids, attention_mask)
-        tok, scores = self.choose_first(logits, return_scores=True)
-        _trace_add(trace, logits, scores)
-        seq = torch.cat([input_ids, self._decode(tok.view(B, 1), max_new_tokens, use_graph, trace)], 1)
-        return _generate_output(seq, trace) if return_dict_in_generate else seq
+            self.set_adapters(None if names is None else [a for a in names for _ in range(copies)])
+        return max_new_tokens
 
     def _adapter_names(self, adapter, B: int):
         """generate()'s adapter argument as a list of B names (None: no adapter), checked before any work."""
@@ -1860,13 +1650,14 @@ class LlamaForCausalLM_KIVI(nn.Module):
         output_logits lists, already holding the first token's entries): each step's scores and logits are cloned after
         its replay, and dropped with the step that is."""
         out = [tok]
-        stops = self._processing and self._proc.stops
+        proc = self._proc
+        stops = proc is not None and proc.stops
         if stops:
             flags = [torch.empty(tok.shape[0], dtype=torch.uint8, pin_memory=True) for _ in range(2)]
             events = [torch.cuda.Event(), torch.cuda.Event()]
 
             def copy_flags(i):
-                flags[i & 1].copy_(self._proc.finished, non_blocking=True)
+                flags[i & 1].copy_(proc.finished, non_blocking=True)
                 events[i & 1].record()
             copy_flags(0)
         for i in range(1, max_new_tokens):
@@ -1875,7 +1666,7 @@ class LlamaForCausalLM_KIVI(nn.Module):
             logits = self.decode_step(out[-1], use_graph=use_graph)
             out.append(self.next_tokens.view(-1, 1).clone())
             if trace is not None:
-                _trace_add(trace, logits, self._proc.scores if self._processing else logits, clone=True)
+                _trace_add(trace, logits, logits if proc is None else proc.scores, clone=True)
             if stops:
                 copy_flags(i)
                 events[(i - 1) & 1].synchronize()
@@ -1886,9 +1677,9 @@ class LlamaForCausalLM_KIVI(nn.Module):
                     break
         return torch.cat(out, dim=1)
 
-    def _generate_many(self, input_ids, max_new_tokens, use_graph, attention_mask, max_length, do_sample, temperature,
-                       top_k, top_p, seed, num_beams, num_return_sequences, length_penalty, early_stopping, eos_token_id,
-                       pad_token_id, return_dict_in_generate, proc=None, trace=None, names=None):
+    def _generate_many(self, input_ids, max_new_tokens, use_graph, attention_mask, max_length, sampling, num_beams,
+                       num_return_sequences, length_penalty, early_stopping, eos_token_id, pad_token_id,
+                       return_dict_in_generate, proc=None, trace=None, names=None):
         """generate() with K = num_beams (beam search, kivi_b200.beam) or K = num_return_sequences (do_sample) sequences per
         prompt, in the cache's rows b * K .. b * K + K - 1.  The prompt pass runs once per prompt and its K / V fill the K
         rows (_prompt_pass(copies=K)).
@@ -1898,13 +1689,13 @@ class LlamaForCausalLM_KIVI(nn.Module):
         chosen rows and tokens back in one copy, and replays a second graph that reorders the cache's rows
         (KiviCache._enqueue_reorder: launches_per_reorder launches) and their positions.  Returns [B * n, length] ids, or
         with return_dict_in_generate an object with `sequences` and `sequences_scores`.
-        do_sample: row b * n + j samples from the Philox key seed + b * n + j (set_sampling over the B * n rows), its first
-        token from prompt b's logits, with the logits processing `proc` (generate()'s, set_processing) on every row.
+        do_sample (sampling: set_sampling's arguments, else None): row b * n + j samples from the Philox key seed + b * n + j
+        (set_sampling over the B * n rows), its first token from prompt b's logits, with the logits processing `proc` (generate()'s, set_processing) on every row.
         Returns [B * n, prompt + new] ids, or with return_dict_in_generate generate()'s GenerateDecoderOnlyOutput (`trace`:
         its output_logits, per row).
         Refused before any work: beam sampling (NotImplementedError), num_return_sequences > num_beams and several greedy
         sequences per prompt (ValueError), beams with enable_token_allgather replicas (NotImplementedError)."""
-        beams = num_beams > 1
+        beams, do_sample = num_beams > 1, sampling is not None
         if num_beams < 1 or num_return_sequences < 1:
             raise ValueError(f"num_beams ({num_beams}) and num_return_sequences ({num_return_sequences}) must be >= 1")
         if beams and do_sample:
@@ -1922,38 +1713,13 @@ class LlamaForCausalLM_KIVI(nn.Module):
         B, n = input_ids.shape
         rows = B * K
         proc = proc if do_sample else None                  # beam search reads eos_token_id itself
-        if do_sample:
-            sampling_rows(rows, temperature, top_k, top_p, seed)                # ValueError before any work
-        if proc is not None:
-            processing_rows(rows, proc["repetition_penalty"], eos_token_id=proc["eos_token_id"], vocab=self.config.vocab_size)
-        if attention_mask is not None:
-            kv_start_from_mask(attention_mask)                               # ValueError unless left-padded
-        if max_new_tokens is None:
-            if max_length is None:
-                raise ValueError("generate() needs max_new_tokens or max_length")
-            max_new_tokens = max_length - n
-        cap = n + max_new_tokens
-        if self.sliding_window is not None:
-            cap = min(cap, max(n, self.sliding_window) + 2 * max(128, self.config.residual_length))
-        if self.cache is None or self.cache.batch != rows or self.cache.max_tokens < cap:
-            self.init_cache(rows, cap)
-        self._tables(self.cache.device, n + max_new_tokens)
-        if do_sample:
-            self.set_sampling(temperature, top_k, top_p, seed)
-        else:
-            self.set_sampling(None)
-        if proc is not None:
-            self.set_processing(**proc)
-        else:
-            self.set_processing(None)
-        if self._lora is not None:
-            self.set_adapters(None if names is None else [a for a in names for _ in range(K)])
+        max_new_tokens = self._generate_setup(input_ids, K, max_new_tokens, max_length, attention_mask, sampling, proc,
+                                              names)
         logits = self.lm_head(self._prompt_pass(input_ids, attention_mask, copies=K)[:, -1]).float()    # [B, vocab]
         if do_sample:
             first = logits.repeat_interleave(K, 0)
             tok = self.choose_first(first).view(rows, 1)
-            if trace is not None:
-                _trace_add(trace, first, first)
+            _trace_add(trace, first, first)
             seq = torch.cat([input_ids.repeat_interleave(K, 0), self._decode(tok, max_new_tokens, use_graph, trace)], 1)
             scores = None
         else:

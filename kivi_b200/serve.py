@@ -24,12 +24,8 @@ from types import SimpleNamespace
 import torch
 
 from .cache import kv_start_from_mask
-from .llama_kivi import PROCESSING_KEYS, processing_rows, sampling_rows
-
-GREEDY = dict(temperature=0.0, top_k=0, top_p=1.0, seed=0)            # the slot parameters of a request without params
-SAMPLING_KEYS = ("temperature", "top_k", "top_p", "seed")
-NEUTRAL = dict(repetition_penalty=1.0, presence_penalty=0.0, frequency_penalty=0.0, min_new_tokens=0)   # no processing
-MAX_LOGPROBS = 20
+from .choice import GREEDY, NEUTRAL, PROCESSING_KEYS, SAMPLING_KEYS, processing_rows, sampling_rows
+from .glue import MAX_TOP_LOGPROBS as MAX_LOGPROBS
 
 
 class TokenLogprobs(NamedTuple):
@@ -41,38 +37,13 @@ class TokenLogprobs(NamedTuple):
     top: torch.Tensor
 
 
-def logprobs_param(par):
-    """The number of top log-probabilities a request's params ask for (0: the chosen token's only), or None."""
-    return None if par is None else par.get("logprobs")
-
-
-def adapter_param(par):
-    """The LoRA adapter a request's params name, or None."""
-    return None if par is None else par.get("adapter")
-
-
-def decoding_params(par):
-    """A request's params without `logprobs` and `adapter`, which are not decoding parameters: None (greedy) when those
-    were its only keys."""
-    if par is None or ("logprobs" not in par and "adapter" not in par):
-        return par
-    rest = {k: v for k, v in par.items() if k not in ("logprobs", "adapter")}
-    return rest or None
-
-
-def sampling_params(par):
-    """The sampling parameters of a request's params: None (greedy) for a request without params or whose params hold
-    processing keys only, else its sampling keys (the missing ones take generate(do_sample=True)'s defaults)."""
-    if par is None or (not any(k in par for k in SAMPLING_KEYS) and any(k in par for k in PROCESSING_KEYS)):
-        return None
-    return {k: v for k, v in par.items() if k in SAMPLING_KEYS}
-
-
-def processing_params(par):
-    """The logits-processing parameters of a request's params (None when it has none of the keys)."""
-    if par is None or not any(k in par for k in PROCESSING_KEYS):
-        return None
-    return {k: v for k, v in par.items() if k in PROCESSING_KEYS}
+class Params(NamedTuple):
+    """A request's params, split by what reads them: set_slot_sampling's keywords (None: greedy), set_slot_processing's
+    (None: none), the number of top log-probabilities (None: not asked for) and the LoRA adapter's name (None: none)."""
+    sampling: dict | None = None
+    processing: dict | None = None
+    logprobs: int | None = None
+    adapter: str | None = None
 
 
 def parse_requests(requests, adapters=()):
@@ -81,9 +52,9 @@ def parse_requests(requests, adapters=()):
     and of repetition_penalty, presence_penalty, frequency_penalty, min_new_tokens (missing keys: 1.0, 0.0, 0.0, 0;
     processing_rows), and `logprobs`: an int N, 0 <= N <= 20, the number of top log-probabilities wanted with each token.
     `adapter`: the name of a LoRA adapter, one of `adapters` (the model's loaded adapters; None: any string).
-    A request whose params hold processing keys, `logprobs` or `adapter` only is greedy.
-    Returns ([(prompt int64 1-D on the host, max_new_tokens)], [params or None]); ValueError for an empty prompt, a budget
-    below 1, an unknown key or a value outside its range."""
+    A request whose params hold processing keys, `logprobs` or `adapter` only is greedy; params {} sample with the
+    defaults.  Returns ([(prompt int64 1-D on the host, max_new_tokens)], [Params]); ValueError for an empty prompt, a
+    budget below 1, an unknown key or a value outside its range."""
     reqs, params = [], []
     for i, r in enumerate(requests):
         if len(r) not in (2, 3):
@@ -103,10 +74,12 @@ def parse_requests(requests, adapters=()):
             if "adapter" in par and (not isinstance(par["adapter"], str) or
                                      (adapters is not None and par["adapter"] not in adapters)):
                 raise ValueError(f"request {i}: adapter {par['adapter']!r} is not loaded (loaded: {sorted(adapters)})")
-            sampling_rows(1, **{k: v for k, v in par.items() if k in SAMPLING_KEYS})   # ValueError outside its range
-            processing_rows(1, **{k: v for k, v in par.items() if k in PROCESSING_KEYS})
-            par = dict(par)
-        params.append(par)
+            samp = {k: v for k, v in par.items() if k in SAMPLING_KEYS}
+            proc = {k: v for k, v in par.items() if k in PROCESSING_KEYS}
+            sampling_rows(1, **samp)                                      # ValueError outside its range
+            processing_rows(1, **proc)
+            par = Params(samp if samp or not par else None, proc or None, par.get("logprobs"), par.get("adapter"))
+        params.append(par or Params())
     return reqs, params
 
 
@@ -162,15 +135,11 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     reqs, params = parse_requests(requests, adapters=None)
     if not reqs:
         return
-    lora = [adapter_param(par) for par in params]
-    if any(a is not None for a in lora):                                  # the names, before any work
+    if any(par.adapter is not None for par in params):                   # the names, before any work
         parse_requests(requests, model.adapters)
-    lp_n = [logprobs_param(par) for par in params]
-    params = [decoding_params(par) for par in params]
-    samp = [sampling_params(par) for par in params]
-    proc = [processing_params(par) for par in params]
-    want_lp = any(n is not None for n in lp_n)
-    sampling, processing = any(s is not None for s in samp), any(p is not None for p in proc)
+    want_lp = any(par.logprobs is not None for par in params)
+    sampling = any(par.sampling is not None for par in params)
+    processing = any(par.processing is not None for par in params)
     eos = set() if eos_token_id is None else set(torch.as_tensor(eos_token_id).reshape(-1).tolist())
     longest = max(p.numel() for p, _ in reqs)
     for i, (p, m) in enumerate(reqs):
@@ -199,7 +168,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
     else:
         model.set_processing(None)
     if want_lp:
-        n_top = max(n for n in lp_n if n is not None)
+        n_top = max(par.logprobs for par in params if par.logprobs is not None)
         model.set_logprobs(n_top)
         host = SimpleNamespace(ids=torch.empty(batch, dtype=torch.long, pin_memory=True),
                                lp=torch.empty(batch, dtype=torch.float32, pin_memory=True),
@@ -224,10 +193,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
         """The first token(s) from prompt logits: of slot `slot` (insert) or of the whole batch, whose row b holds request
         rows[b] (prefill); a slot gets its request's parameters and a fresh draw counter here."""
         for b, i in enumerate(rows) if slot is None else [(slot, rows)]:
-            if sampling:
-                model.set_slot_sampling(b, **(GREEDY if samp[i] is None else samp[i]))
-            if processing:
-                model.set_slot_processing(b, **(NEUTRAL if proc[i] is None else proc[i]))
+            model.choice.set_slot(b, params[i].sampling, params[i].processing)
         return model.choose_first(logits, slot)
 
     queue = deque(range(len(reqs)))
@@ -240,14 +206,14 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
         """Append a token to the slot's output; finish (release) the slot on EOS or on its token budget."""
         outs[slot].append(tok)
         i = owner[slot]
-        if want_lp and lp_n[i] is not None:
-            n = lp_n[i]
+        n = params[i].logprobs
+        if want_lp and n is not None:
             lps[slot].append((host.lp[slot].clone(), host.top_ids[slot, :n].clone(), host.top[slot, :n].clone()))
         if tok in eos or len(outs[slot]) >= reqs[i][1]:
             ids = torch.tensor(outs[slot], dtype=torch.long)
             if not want_lp:
                 done.append((i, ids))
-            elif lp_n[i] is None:
+            elif n is None:
                 done.append((i, ids, None))
             else:
                 t, top_ids, top = zip(*lps[slot])
@@ -266,7 +232,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
             ids[b, P - n:] = reqs[i][0]
             mask[b, P - n:] = 1
         if loaded:
-            model.set_adapters([lora[i] for i in rows] + [None] * (batch - len(rows)))
+            model.set_adapters([params[i].adapter for i in rows] + [None] * (batch - len(rows)))
         ids, mask = ids.to(dev), mask.to(dev)
         logits = model.prefill(ids, attention_mask=mask)
         cache.set_kv_start(kv_start_from_mask(mask))                      # ragged from the start: one step graph
@@ -299,7 +265,7 @@ def serve(model, requests, batch: int, max_tokens: int, eos_token_id=None, use_g
                     i = queue.popleft()
                     if prefix_cache is not None:
                         hits, reused = prefix_cache.hits, prefix_cache.reused_tokens
-                    tok = first_token(model.insert(slot, p.to(dev), prefix_cache, adapter=lora[i]), slot, i)
+                    tok = first_token(model.insert(slot, p.to(dev), prefix_cache, adapter=params[i].adapter), slot, i)
                     if prefix_cache is not None:
                         stats["prefix_hits"] += prefix_cache.hits - hits
                         stats["prefix_tokens"] += prefix_cache.reused_tokens - reused

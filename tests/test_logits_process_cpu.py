@@ -82,7 +82,7 @@ def test_presence_frequency_and_finished_rows():
 
 
 def test_processing_rows_rejects_out_of_range():
-    from kivi_b200.llama_kivi import processing_rows
+    from kivi_b200.choice import processing_rows
     rep, pres, freq, mn, eos = processing_rows(2, [1.2, 0.8], 0.5, -0.5, 3, [2, 3], vocab=10)
     assert rep == [1.2, 0.8] and pres == [0.5, 0.5] and freq == [-0.5, -0.5] and mn == [3, 3] and eos == [2, 3]
     assert processing_rows(1, eos_token_id=4)[4] == [4] and processing_rows(1)[4] == []
@@ -97,17 +97,17 @@ def test_processing_rows_rejects_out_of_range():
 
 
 def test_parse_requests_validates_processing_keys():
-    from kivi_b200.serve import parse_requests, processing_params, sampling_params
+    from kivi_b200.serve import parse_requests
     p = torch.arange(1, 5)
     _, params = parse_requests([(p, 3, dict(repetition_penalty=1.3, presence_penalty=0.5, frequency_penalty=0.2,
                                             min_new_tokens=2, temperature=0.7))])
-    assert sampling_params(params[0]) == dict(temperature=0.7)
-    assert processing_params(params[0]) == dict(repetition_penalty=1.3, presence_penalty=0.5, frequency_penalty=0.2,
-                                                min_new_tokens=2)
+    assert params[0].sampling == dict(temperature=0.7)
+    assert params[0].processing == dict(repetition_penalty=1.3, presence_penalty=0.5, frequency_penalty=0.2,
+                                        min_new_tokens=2)
     _, params = parse_requests([(p, 3, dict(repetition_penalty=1.3)), (p, 3, {}), (p, 3)])
-    assert sampling_params(params[0]) is None                             # processing keys only: greedy
-    assert sampling_params(params[1]) == {} and processing_params(params[1]) is None     # {}: sampled, the defaults
-    assert sampling_params(params[2]) is None and processing_params(params[2]) is None
+    assert params[0].sampling is None                                     # processing keys only: greedy
+    assert params[1].sampling == {} and params[1].processing is None      # {}: sampled, the defaults
+    assert params[2].sampling is None and params[2].processing is None
     for par in (dict(repetition_penalty=0.0), dict(presence_penalty=3.0), dict(frequency_penalty=-2.5),
                 dict(min_new_tokens=-2), dict(repetition_penalty=1.1, top_p=2.0), dict(no_repeat_ngram_size=2)):
         with pytest.raises(ValueError):

@@ -116,7 +116,7 @@ def host_loop(twin, ids, new, mask=None, rep=None, min_length=None, min_new=None
     last token in the ids the processors see (the fused path does not penalise padding).  copies = K: K rows per prompt,
     the prompt run once for all of them, as generate(num_return_sequences=K)."""
     from kivi_b200 import glue
-    from kivi_b200.llama_kivi import sampling_rows
+    from kivi_b200.choice import sampling_rows
     B, n = ids.shape
     rows = B * copies
     eos_l = None if eos is None else (eos if isinstance(eos, list) else [eos])
@@ -282,22 +282,23 @@ def _params():
 def test_serve_requests_depend_on_their_own_parameters(graphs):
     """Mixed requests with penalties: the same tokens whichever slot a request gets (the first group permuted); requests
     without the new keys decode as with processing off; the step has exactly two more launches with processing."""
-    from kivi_b200.serve import processing_params, sampling_params, serve
+    from kivi_b200.serve import parse_requests, serve
     model, cfg = tiny_model(2)
     par = _params()
+    split = parse_requests([([1], 1, p) for p in par])[1]
     reqs = requests(cfg, BUDGETS, params=par)
     eos = [cfg.vocab_size - 1, cfg.vocab_size - 2]
-    off = dict(serve(model, requests(cfg, BUDGETS, params=[sampling_params(p) for p in par]), 3, 260, eos_token_id=eos))
+    off = dict(serve(model, requests(cfg, BUDGETS, params=[s.sampling for s in split]), 3, 260, eos_token_id=eos))
     off_launches = model.launches_per_step
-    assert not model._processing
+    assert model.choice.proc is None
     a = dict(serve(model, reqs, 3, 260, eos_token_id=eos))
-    assert model.launches_per_step == off_launches + 2 and model._processing
+    assert model.launches_per_step == off_launches + 2 and model.choice.proc is not None
     order = [2, 0, 1] + list(range(3, 8))                                  # the first group's slots permuted
     b_perm = dict(serve(model, [reqs[i] for i in order], 3, 260, eos_token_id=eos))
     b = {order[j]: t for j, t in b_perm.items()}
     for i in range(8):
         assert torch.equal(a[i], b[i]), i
-        if processing_params(par[i]) is None:
+        if split[i].processing is None:
             assert torch.equal(a[i], off[i]), i                           # no processing keys: as without processing
     assert sum(not torch.equal(a[i], off[i]) for i in (0, 2, 3, 6)) >= 3
     # a neighbour's parameters do not reach a request
@@ -307,7 +308,7 @@ def test_serve_requests_depend_on_their_own_parameters(graphs):
     for i in (0, 2, 3):
         assert torch.equal(c[i], a[i]), i
     again = dict(serve(model, requests(cfg, BUDGETS), 3, 260))
-    assert not model._processing and model.launches_per_step == off_launches
+    assert model.choice.proc is None and model.launches_per_step == off_launches
     plain = dict(serve(tiny_model(2)[0], requests(cfg, BUDGETS), 3, 260))
     for i in range(8):
         assert torch.equal(again[i], plain[i]), i

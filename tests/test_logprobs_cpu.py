@@ -54,12 +54,12 @@ def test_reference_ranks_like_topk():
 
 
 def test_parse_requests_validates_logprobs():
-    from kivi_b200.serve import decoding_params, logprobs_param, parse_requests, sampling_params
+    from kivi_b200.serve import parse_requests
     p = torch.arange(1, 5)
     _, params = parse_requests([(p, 3, dict(logprobs=0)), (p, 3, dict(logprobs=20, temperature=0.5)), (p, 3)])
-    assert [logprobs_param(x) for x in params] == [0, 20, None]
-    assert decoding_params(params[0]) is None                              # logprobs only: greedy, as without params
-    assert sampling_params(decoding_params(params[1])) == dict(temperature=0.5)
+    assert [x.logprobs for x in params] == [0, 20, None]
+    assert params[0].sampling is None and params[0].processing is None     # logprobs only: greedy, as without params
+    assert params[1].sampling == dict(temperature=0.5) and params[1].processing is None
     for n in (-1, 21, 2.0, True, "3", None):
         with pytest.raises(ValueError, match="logprobs"):
             parse_requests([(p, 3, dict(logprobs=n))])

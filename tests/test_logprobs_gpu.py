@@ -227,10 +227,10 @@ def _lp_params():
 
 
 def test_serve_logprobs():
-    from kivi_b200.serve import TokenLogprobs, decoding_params, serve
+    from kivi_b200.serve import TokenLogprobs, serve
     model, cfg = tiny_model(2)
     par = _lp_params()
-    plain_par = [decoding_params(p) for p in par]
+    plain_par = [None if p is None else {k: v for k, v in p.items() if k != "logprobs"} or None for p in par]
     eos = [cfg.vocab_size - 1]
     off = list(serve(model, requests(cfg, BUDGETS, params=plain_par), 3, 260, eos_token_id=eos))
     assert all(len(r) == 2 for r in off)

@@ -120,13 +120,13 @@ def test_entry_points_check_arguments():
 
 
 def test_parse_requests_adapter():
-    from kivi_b200.serve import adapter_param, decoding_params, parse_requests, sampling_params
+    from kivi_b200.serve import parse_requests
     p = torch.arange(1, 5)
     _, params = parse_requests([(p, 3, dict(adapter="a")), (p, 3, dict(adapter="b", temperature=0.5)), (p, 3)],
                                adapters=["a", "b"])
-    assert [adapter_param(x) for x in params] == ["a", "b", None]
-    assert decoding_params(params[0]) is None                              # adapter only: greedy
-    assert sampling_params(decoding_params(params[1])) == dict(temperature=0.5)
+    assert [x.adapter for x in params] == ["a", "b", None]
+    assert params[0].sampling is None and params[0].processing is None     # adapter only: greedy
+    assert params[1].sampling == dict(temperature=0.5) and params[1].processing is None
     for name in ("c", None, 3):
         with pytest.raises(ValueError, match="adapter"):
             parse_requests([(p, 3), (p, 3, dict(adapter=name))], adapters=["a", "b"])

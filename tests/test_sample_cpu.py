@@ -79,7 +79,7 @@ def test_entry_point_validates_arguments():
 
 # ------------------------------------------------------------------------------------------------ the Python surface
 def test_sampling_rows_validation():
-    from kivi_b200.llama_kivi import sampling_rows
+    from kivi_b200.choice import sampling_rows
     assert sampling_rows(3) == ([1.0] * 3, [50] * 3, [1.0] * 3, [0, 1, 2])
     t, k, p, s = sampling_rows(2, temperature=[0.0, 0.7], top_k=0, top_p=(0.9, 1.0), seed=[7, 2 ** 64 - 1])
     assert (t, k, p, s) == ([0.0, 0.7], [0, 0], [0.9, 1.0], [7, 2 ** 64 - 1])
@@ -105,12 +105,13 @@ def test_generate_rejects_bad_parameters_before_any_work():
 
 
 def test_serve_request_parsing():
-    from kivi_b200.serve import parse_requests
+    from kivi_b200.serve import Params, parse_requests
     reqs, params = parse_requests([([1, 2, 3], 4), (np.array([5]), 2)])
     assert [p.tolist() for p, _ in reqs] == [[1, 2, 3], [5]] and [m for _, m in reqs] == [4, 2]
-    assert params == [None, None]                                         # no params: serve() stays on the greedy step
+    assert params == [Params(), Params()] and params[0] == (None,) * 4   # no params: serve() stays on the greedy step
     reqs, params = parse_requests([([1], 1, {"temperature": 0.8, "seed": 3}), ([2], 1), ([3], 1, None), ([4], 1, {})])
-    assert params == [{"temperature": 0.8, "seed": 3}, None, None, {}]
+    assert [p.sampling for p in params] == [{"temperature": 0.8, "seed": 3}, None, None, {}]
+    assert all(p.processing is None and p.logprobs is None and p.adapter is None for p in params)
     for bad in ([([1], 1, {"temperature": -1})], [([1], 1, {"top_p": 2})], [([1], 1, {"min_p": 0.1})],
                 [([1], 1, {"top_k": [1, 2]})], [([], 1)], [([1], 0)], [([1],)], [([1], 1, {}, 0)]):
         with pytest.raises(ValueError):
